@@ -24,6 +24,7 @@
 // All functions are __host__ __device__: csrc/host_emul.cpp runs them phase by phase on the CPU (a
 // barrier between phases), which lets the CPU-only test-suite check every index map against the oracle.
 #pragma once
+#include <cmath>
 #include "ntt_lane.cuh"
 
 namespace nb {
@@ -121,8 +122,11 @@ constexpr int POLY_STRIDE = 16 * ROW_STRIDE;      // u64 per work polynomial
 //   BrCfg<1, 256> ("wide"):  256 threads per ciphertext: the forward phases take one sweep instead of two and the
 //                            inverse phases leave half of the warps idle; 36 % fewer instructions on the critical
 //                            path of a step.  Used when the batch fits one wave of such CTAs (latency, not throughput).
-template <int CT_, int THREADS_, int CTAS_ = 512 / THREADS_, bool TWD_GLOBAL_ = false> struct BrCfg {
+//   BrCfg<2, 256, 2, true, true> ("fft"): the throughput shape with the FP64 step (keys with spectra, see below).
+template <int CT_, int THREADS_, int CTAS_ = 512 / THREADS_, bool TWD_GLOBAL_ = false, bool FFT_ = false> struct BrCfg {
     static constexpr int CT = CT_, THREADS = THREADS_;
+    static constexpr bool FFT = FFT_;                          // the FP64 step (br_fft_step) instead of the NTT step
+    static_assert(!FFT_ || (THREADS_ == 128 * CT_ && TWD_GLOBAL_), "the FP64 step runs 128 threads per ciphertext, tables in L1");
     static constexpr int POLYS = 4 * CT;                       // work polynomials per CTA
     // Twice as many threads as forward tasks ("wide2": 1 ciphertext on 512 threads): two threads of different warps per
     // 16-element forward task, 8 outputs each (split forward phases below)
@@ -158,13 +162,16 @@ constexpr int BR2_THREADS = NB_BR_THREADS;
 using BrDefault = BrCfg<BR2_CT, BR2_THREADS, NB_BR_CTAS, NB_BR_TWD_GLOBAL != 0>;
 using BrWide = BrCfg<1, 256>;
 using BrWide2 = BrCfg<1, 512, 1>;                 // lowest latency: one ciphertext per SM, 16 warps in step
+using BrFft = BrCfg<2, 256, 2, true, true>;      // throughput shape, FP64 step
 constexpr int BR2_POLYS = BrDefault::POLYS;
 // Engine bootstrap-key row: 8 planes [(mi*2+j)*2+mo][row*64 + stored column] of plain field values plus
 // 2 correction planes K[mo] = 512 * NTT(1,...,1) * sum_{mi,j} plane, because the forward transforms run
 // on the UNSIGNED digits u = d + 512 in [0, 1023] (cheap twist, no sign handling):
 //     sum_d NTT(d) BK = sum_d NTT(u) BK - 512 NTT(1) sum_d BK.
 constexpr int BK_PLANES = 10;
-constexpr int BK_ROW_U64 = BK_PLANES * NTT_N;
+constexpr int BK_NTT_U64 = BK_PLANES * NTT_N;
+// the row continues with the 16 key spectra of the FP64 step (BK_FFT_U64 below: 16 x 512 complex doubles)
+constexpr int BK_ROW_U64 = BK_NTT_U64 + 16 * 512 * 2;
 
 // 16-byte accesses to two adjacent field elements (shared memory rows and key rows are 16-byte aligned)
 NB_HD void ld2(const u64 *p, u64 &x, u64 &y)
@@ -1152,6 +1159,306 @@ template <class Cfg = BrDefault> NB_HD bool map_inv3(int tid, int &p, int &row, 
     int pp = tid >> 6;
     p = (pp >> 1) * 4 + (pp & 1);
     return pp < 2 * Cfg::CT;
+}
+
+// ---- FP64 step (throughput shape, keys with integral coefficients) --------------------------------------------------
+// The external product as an exact floating-point computation (DESIGN.md section 3): every coefficient the step
+// produces is an integer, so a transform whose rounding error stays below 1/2 gives the same bits as the NTT.  The key
+// polynomial k (centred 32-bit integers) is split as k = k_hi 2^16 + k_lo with k_lo in [-2^15, 2^15), k_hi in
+// [-2^15, 2^15]; each half's product with the signed 10-bit digits is below 2^37 in magnitude and is rounded to an
+// integer on its own; the step then adds lo + (hi << 16) mod 2^32 to the accumulator.
+// Negacyclic fold: a polynomial a of degree < 1024 becomes z_j = (a_j + i a_{j+512}) w^j, j < 512, w = e^{i pi / 1024};
+// its 512-point DFT (root e^{-2 pi i / 512}) is a evaluated at 512 roots of X^1024 + 1 that carry z^512 = i, so the
+// point-wise product of two such spectra is the spectrum of the negacyclic product.
+// The DFT is three radix-8 passes, decimation in frequency (natural order in, digit-reversed order out); the inverse
+// is the mirrored decimation-in-time network, so the MAC works point-wise and nothing is reordered:
+//     pass 1, task n0 < 64:          x[n0 + 64 m]                -> DFT8 over m, times W512^(n0 k1) -> x[n0 + 64 k1]
+//     pass 2, task (k1, n1 < 8):     x[64 k1 + n1 + 8 m]         -> DFT8, times W64^(n1 k2)        -> x[64 k1 + n1 + 8 k2]
+//     pass 3, task (k1, k2):         x[64 k1 + 8 k2 + m]         -> DFT8                            -> x[64 k1 + 8 k2 + k3]
+// leaving X[k1 + 8 k2 + 64 k3] at position 64 k1 + 8 k2 + k3.  A spectrum is 512 complex values in shared memory,
+// position x stored at x + x / 8 (one pad per 8) so that the 16-byte accesses of every pass are bank-conflict free.
+// Every floating-point operation is an explicit, correctly rounded add / mul / fma (__dadd_rn & co. are never
+// contracted by the compiler), in the order the error bound of DESIGN.md section 3 assumes; the host emulation
+// (csrc/host_emul.cpp, no FMA contraction) computes the same bits.
+struct cplx {
+    double re, im;
+};
+constexpr int FFT_M = 512;                          // complex points per spectrum
+constexpr int FFT_SPEC_CPLX = FFT_M + FFT_M / 8;    // padded spectrum in shared memory
+NB_HD int fft_pad(int x) { return x + (x >> 3); }
+// Engine bootstrap-key row, FP64 part: 16 spectra [(m = (mi * 2 + j) * 2 + mo) * 2 + h][512] (h = 0: k_lo, 1: k_hi),
+// unpadded, complex doubles; it follows the NTT planes of the same row.
+constexpr int BK_FFT_SPECTRA = 16;
+constexpr int BK_FFT_U64 = BK_FFT_SPECTRA * FFT_M * 2;
+static_assert(BK_ROW_U64 == BK_NTT_U64 + BK_FFT_U64, "key row layout");
+// tables (tables.h: FftTables), complex, concatenated: twist w^j (512), pass-1 twiddles W512^(n0 k1) [n0][k1] (512),
+// pass-2 twiddles W64^(n1 k2) [n1][k2] (64), untwist conj(w^j) / 512 (512)
+constexpr int FFT_TAB_TWIST = 0, FFT_TAB_TW1 = 512, FFT_TAB_TW2 = 1024, FFT_TAB_UNTWIST = 1088, FFT_TAB_CPLX = 1600;
+
+#if defined(__CUDA_ARCH__)
+NB_HD double d_add(double a, double b) { return __dadd_rn(a, b); }
+NB_HD double d_sub(double a, double b) { return __dsub_rn(a, b); }
+NB_HD double d_mul(double a, double b) { return __dmul_rn(a, b); }
+NB_HD double d_fma(double a, double b, double c) { return __fma_rn(a, b, c); }
+NB_HD cplx ld_cplx_tab(const cplx *p)
+{
+    const double2 t = __ldg(reinterpret_cast<const double2 *>(p));
+    return {t.x, t.y};
+}
+NB_HD cplx ld_cplx(const cplx *p)
+{
+    const double2 t = *reinterpret_cast<const double2 *>(p);
+    return {t.x, t.y};
+}
+NB_HD void st_cplx(cplx *p, cplx v) { *reinterpret_cast<double2 *>(p) = make_double2(v.re, v.im); }
+NB_HD cplx ld_cplx_stream(const cplx *p)           // key spectra: read once per CTA, keep them out of the L1
+{
+    const double2 t = __ldcg(reinterpret_cast<const double2 *>(p));
+    return {t.x, t.y};
+}
+NB_HD i32 d_rint_lo32(double x) { return (i32)__double2ll_rn(x); }
+#else
+NB_HD double d_add(double a, double b) { return a + b; }
+NB_HD double d_sub(double a, double b) { return a - b; }
+NB_HD double d_mul(double a, double b) { return a * b; }
+NB_HD double d_fma(double a, double b, double c) { return std::fma(a, b, c); }
+NB_HD cplx ld_cplx_tab(const cplx *p) { return *p; }
+NB_HD cplx ld_cplx(const cplx *p) { return *p; }
+NB_HD void st_cplx(cplx *p, cplx v) { *p = v; }
+NB_HD cplx ld_cplx_stream(const cplx *p) { return *p; }
+NB_HD i32 d_rint_lo32(double x) { return (i32)(u32)(uint64_t)std::llrint(x); }
+#endif
+
+NB_HD cplx c_add(cplx a, cplx b) { return {d_add(a.re, b.re), d_add(a.im, b.im)}; }
+NB_HD cplx c_sub(cplx a, cplx b) { return {d_sub(a.re, b.re), d_sub(a.im, b.im)}; }
+// a * w and a * conj(w): one product and one fma per component
+NB_HD cplx c_mul(cplx a, cplx w) { return {d_fma(a.re, w.re, -d_mul(a.im, w.im)), d_fma(a.re, w.im, d_mul(a.im, w.re))}; }
+NB_HD cplx c_mul_conj(cplx a, cplx w) { return {d_fma(a.re, w.re, d_mul(a.im, w.im)), d_fma(a.im, w.re, -d_mul(a.re, w.im))}; }
+// acc + a * b (complex), four fmas
+NB_HD cplx c_mac(cplx acc, cplx a, cplx b)
+{
+    return {d_fma(-a.im, b.im, d_fma(a.re, b.re, acc.re)), d_fma(a.im, b.re, d_fma(a.re, b.im, acc.im))};
+}
+
+// 8-point DFT in place, natural order in and out: y[k] = sum_m y[m] e^{-+ 2 pi i m k / 8} (INV: the + sign), as three
+// radix-2 decimation-in-frequency layers.  Multiplications by -+i are exact (swap and sign); by e^{-+ i pi / 4} one
+// addition and one product per component with the rounded constant sqrt(1/2).
+template <bool INV> NB_HD void dft8(cplx *y)
+{
+    constexpr double S = 0.70710678118654752440;
+    auto mul_mi = [](cplx a) -> cplx { return INV ? cplx{-a.im, a.re} : cplx{a.im, -a.re}; };       // times -i (fwd) / +i (inv)
+    cplx t[8];
+    static_for<0, 4>([&](auto M) {
+        constexpr int m = decltype(M)::value;
+        t[m] = c_add(y[m], y[m + 4]);
+        t[m + 4] = c_sub(y[m], y[m + 4]);
+    });
+    // t[4 + m] *= W8^m, W8 = e^{-+ i pi / 4}
+    {
+        const cplx a = t[5];           // (re + im) S - i (re - im) S  (fwd);  (re - im) S + i (re + im) S  (inv)
+        t[5] = INV ? cplx{d_mul(d_sub(a.re, a.im), S), d_mul(d_add(a.re, a.im), S)} : cplx{d_mul(d_add(a.re, a.im), S), d_mul(d_sub(a.im, a.re), S)};
+        t[6] = mul_mi(t[6]);
+        const cplx b = t[7];           // W8^3 = -+ i W8
+        const cplx c = INV ? cplx{d_mul(d_sub(b.re, b.im), S), d_mul(d_add(b.re, b.im), S)} : cplx{d_mul(d_add(b.re, b.im), S), d_mul(d_sub(b.im, b.re), S)};
+        t[7] = mul_mi(c);
+    }
+    cplx u[8];
+    static_for<0, 2>([&](auto H) {
+        constexpr int h = 4 * decltype(H)::value;
+        u[h + 0] = c_add(t[h + 0], t[h + 2]);
+        u[h + 1] = c_add(t[h + 1], t[h + 3]);
+        u[h + 2] = c_sub(t[h + 0], t[h + 2]);
+        u[h + 3] = mul_mi(c_sub(t[h + 1], t[h + 3]));
+    });
+    // last layer; outputs of the DIF network are bit-reversed: position p holds y[brev3(p)]
+    y[0] = c_add(u[0], u[1]); y[4] = c_sub(u[0], u[1]);
+    y[2] = c_add(u[2], u[3]); y[6] = c_sub(u[2], u[3]);
+    y[1] = c_add(u[4], u[5]); y[5] = c_sub(u[4], u[5]);
+    y[3] = c_add(u[6], u[7]); y[7] = c_sub(u[6], u[7]);
+}
+
+// pass 1 (forward): x[m'] = real coefficient n0 + 64 m', m' < 16 (exact small integers as doubles); fold, twist,
+// DFT8 over m, twiddle, store
+NB_HD void fft_fwd1(int n0, const double *x, cplx *spec, const cplx *tab)
+{
+    cplx y[8];
+    static_for<0, 8>([&](auto M) {
+        constexpr int m = decltype(M)::value;
+        const cplx w = ld_cplx_tab(tab + FFT_TAB_TWIST + n0 + 64 * m);
+        y[m] = {d_fma(x[m], w.re, -d_mul(x[m + 8], w.im)), d_fma(x[m], w.im, d_mul(x[m + 8], w.re))};
+    });
+    dft8<false>(y);
+    st_cplx(spec + fft_pad(n0), y[0]);
+    static_for<1, 8>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        st_cplx(spec + fft_pad(n0 + 64 * k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k)));
+    });
+}
+// pass 2 (forward), task (k1, n1)
+NB_HD void fft_fwd2(int k1, int n1, cplx *spec, const cplx *tab)
+{
+    cplx y[8];
+    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(spec + fft_pad(64 * k1 + n1 + 8 * decltype(M)::value)); });
+    dft8<false>(y);
+    st_cplx(spec + fft_pad(64 * k1 + n1), y[0]);
+    static_for<1, 8>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        st_cplx(spec + fft_pad(64 * k1 + n1 + 8 * k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW2 + n1 * 8 + k)));
+    });
+}
+// pass 3 (forward), task (k1, k2)
+NB_HD void fft_fwd3(int k1, int k2, cplx *spec)
+{
+    cplx y[8];
+    cplx *s = spec + fft_pad(64 * k1 + 8 * k2);        // the 8 positions are contiguous (one pad per 8)
+    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(s + decltype(M)::value); });
+    dft8<false>(y);
+    static_for<0, 8>([&](auto K) { st_cplx(s + decltype(K)::value, y[decltype(K)::value]); });
+}
+// the inverse passes, mirrored
+NB_HD void fft_inv3(int k1, int k2, cplx *spec)
+{
+    cplx y[8];
+    cplx *s = spec + fft_pad(64 * k1 + 8 * k2);
+    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(s + decltype(M)::value); });
+    dft8<true>(y);
+    static_for<0, 8>([&](auto K) { st_cplx(s + decltype(K)::value, y[decltype(K)::value]); });
+}
+NB_HD void fft_inv2(int k1, int n1, cplx *spec, const cplx *tab)
+{
+    cplx y[8];
+    y[0] = ld_cplx(spec + fft_pad(64 * k1 + n1));
+    static_for<1, 8>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        y[k] = c_mul_conj(ld_cplx(spec + fft_pad(64 * k1 + n1 + 8 * k)), ld_cplx_tab(tab + FFT_TAB_TW2 + n1 * 8 + k));
+    });
+    dft8<true>(y);
+    static_for<0, 8>([&](auto M) { st_cplx(spec + fft_pad(64 * k1 + n1 + 8 * decltype(M)::value), y[decltype(M)::value]); });
+}
+// pass 1 (inverse): x[m'] = the (unrounded) real coefficient n0 + 64 m', m' < 16
+NB_HD void fft_inv1(int n0, const cplx *spec, const cplx *tab, double *x)
+{
+    cplx y[8];
+    y[0] = ld_cplx(spec + fft_pad(n0));
+    static_for<1, 8>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        y[k] = c_mul_conj(ld_cplx(spec + fft_pad(n0 + 64 * k)), ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k));
+    });
+    dft8<true>(y);
+    static_for<0, 8>([&](auto M) {
+        constexpr int m = decltype(M)::value;
+        const cplx v = c_mul(y[m], ld_cplx_tab(tab + FFT_TAB_UNTWIST + n0 + 64 * m));
+        x[m] = v.re;
+        x[m + 8] = v.im;
+    });
+}
+
+// ---- the FP64 step of a CTA of CT ciphertexts on 128 CT threads; spectra [ct * 4 + s][FFT_SPEC_CPLX], s = mi * 2 + j
+// before the MAC and s = mo * 2 + h after it.
+// fwd1: task (pm = ct * 2 + mi, n0): the rotated coefficients serve both digit polynomials (as phase_fwd1_both_digits)
+template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, cplx *spec_all, const cplx *tab, const int *rot_a)
+{
+    const int n0 = task & 63, pm = task >> 6;
+    const i32 *acc = acc_all + pm * NTT_N;
+    const int a = ROTATE ? rot_a[pm >> 1] : 0;
+    const int ar = a & (NTT_N - 1);
+    const bool flip = (a >> 10) & 1;
+    u32 t[16];
+    static_for<0, 16>([&](auto J) {
+        constexpr int j1 = decltype(J)::value;
+        const int idx = 64 * j1 + n0;
+        const i32 c = ROTATE ? rotate_minus_one(acc, idx, ar, flip) : acc[idx];
+        t[j1] = (u32)c + (0x80000000u + (1u << 21));
+    });
+    cplx *spec = spec_all + pm * 2 * FFT_SPEC_CPLX;
+#if defined(__CUDA_ARCH__)
+#pragma unroll 1
+#endif
+    for (int j = 0; j < 2; j++) {
+        const int sh = 22 - 10 * j;
+        double x[16];
+        static_for<0, 16>([&](auto J) { x[decltype(J)::value] = (double)((int)((t[decltype(J)::value] >> sh) & 1023u) - 512); });
+        fft_fwd1(n0, x, spec + j * FFT_SPEC_CPLX, tab);
+    }
+}
+// fwd2 / fwd3 / inv3 / inv2: task x < 256 CT = (spectrum s = x / 64, a = (x / 8) % 8, b = x % 8)
+NB_HD void fft_phase_fwd2(int x, cplx *spec_all, const cplx *tab) { fft_fwd2((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX, tab); }
+NB_HD void fft_phase_fwd3(int x, cplx *spec_all) { fft_fwd3((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX); }
+NB_HD void fft_phase_inv3(int x, cplx *spec_all) { fft_inv3((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX); }
+NB_HD void fft_phase_inv2(int x, cplx *spec_all, const cplx *tab) { fft_inv2((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX, tab); }
+
+// MAC at point P (< 512) of every ciphertext of the CTA: out[mo][h] = sum_d D_d K[d][mo][h]; the key values are loaded
+// once for all CT ciphertexts, the outputs overwrite the digit spectra at the same point (the thread holds them)
+template <int CT> NB_HD void fft_mac_point(int P, cplx *spec_all, const cplx *key)
+{
+    cplx dg[CT][4];
+    static_for<0, CT>([&](auto C) {
+        static_for<0, 4>([&](auto D) {
+            dg[decltype(C)::value][decltype(D)::value] = ld_cplx(spec_all + (decltype(C)::value * 4 + decltype(D)::value) * FFT_SPEC_CPLX + fft_pad(P));
+        });
+    });
+    static_for<0, 4>([&](auto S) {
+        constexpr int mo = decltype(S)::value >> 1, h = decltype(S)::value & 1;      // output spectrum mo * 2 + h
+        cplx k[4];
+#ifdef NB_FFT_KEY_L1_BOUND
+        // TIMING EXPERIMENT ONLY (wrong results): every key load hits the same 2 KB of the row -- what the step would
+        // take if the key stream cost nothing (DESIGN.md section 4, FP64 step breakdown)
+        const int kp = P & 15;
+#else
+        const int kp = P;
+#endif
+        static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(key + ((decltype(D)::value * 2 + mo) * 2 + h) * FFT_M + kp); });
+        static_for<0, CT>([&](auto C) {
+            constexpr int c = decltype(C)::value;
+            cplx o = {d_mul(dg[c][0].re, k[0].re), d_mul(dg[c][0].re, k[0].im)};
+            o = {d_fma(-dg[c][0].im, k[0].im, o.re), d_fma(dg[c][0].im, k[0].re, o.im)};
+            static_for<1, 4>([&](auto D) { o = c_mac(o, dg[c][decltype(D)::value], k[decltype(D)::value]); });
+            st_cplx(spec_all + (c * 4 + mo * 2 + h) * FFT_SPEC_CPLX + fft_pad(P), o);
+        });
+    });
+}
+template <int CT, int THREADS> NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
+{
+#if defined(__CUDA_ARCH__)
+#pragma unroll 1
+#endif
+    for (int P = tid; P < FFT_M; P += THREADS) fft_mac_point<CT>(P, spec_all, key);
+}
+// inv1: task (pp = ct * 2 + mo, n0): both key halves of output polynomial mo, rounded and recombined mod 2^32.
+// ACCUMULATE: acc += result, else acc = result.
+template <bool ACCUMULATE> NB_HD void fft_phase_inv1(int task, i32 *acc_all, const cplx *spec_all, const cplx *tab)
+{
+    const int n0 = task & 63, pp = task >> 6;
+    const int ct = pp >> 1, mo = pp & 1;
+    const cplx *spec = spec_all + (ct * 4 + mo * 2) * FFT_SPEC_CPLX;
+    u32 r[16];
+    {
+        double x[16];
+        fft_inv1(n0, spec, tab, x);
+        static_for<0, 16>([&](auto J) { r[decltype(J)::value] = (u32)d_rint_lo32(x[decltype(J)::value]); });
+    }
+    {
+        double x[16];
+        fft_inv1(n0, spec + FFT_SPEC_CPLX, tab, x);
+        static_for<0, 16>([&](auto J) { r[decltype(J)::value] += (u32)d_rint_lo32(x[decltype(J)::value]) << 16; });
+    }
+    i32 *acc = acc_all + pp * NTT_N;
+    static_for<0, 16>([&](auto J) {
+        constexpr int j1 = decltype(J)::value;
+        const int idx = 64 * j1 + n0;
+        acc[idx] = ACCUMULATE ? (i32)((u32)acc[idx] + r[j1]) : (i32)r[j1];
+    });
+}
+
+// key preparation: the 16 real coefficients n0 + 64 m' of one key polynomial (centred integers, |k| <= 2^31) split into
+// k_lo in [-2^15, 2^15) and k_hi = (k - k_lo) / 2^16 in [-2^15, 2^15]
+NB_HD void fft_split_key(const long long *k, double *lo, double *hi)
+{
+    for (int m = 0; m < 16; m++) {
+        const long long l = ((k[m] + 32768) & 65535) - 32768;
+        lo[m] = (double)l;
+        hi[m] = (double)((k[m] - l) / 65536);
+    }
 }
 
 }  // namespace nb

@@ -3,6 +3,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <vector>
 #include <nvtx3/nvToolsExt.h>
 #include "../../include/nufhe_b200.h"
 #include "kernels.cuh"
@@ -15,6 +16,11 @@ struct nb_ctx {
     cudaStream_t stream;
     u64 *d_ph_fwd, *d_ph_inv;            // middle-twiddle tables [row][j2] of the transform passes
     u64 *d_ones512;                      // 512 * NTT(all-ones), natural order (bk_prepare)
+    cplx *d_fft_tab;                     // tables of the FP64 step (tables.h: FftTables)
+    // engine keys prepared on this context whose coefficients are centred 32-bit integers: they carry the spectra of
+    // the FP64 step, which the throughput shape runs on them (begin, end of the key's rows)
+    std::vector<std::pair<const u64 *, const u64 *>> spectral_keys;
+    int fft;                             // developer knob: 0 keeps the NTT step for every key
     int sm_count;
     size_t wide_max;                     // largest batch launched in the wide (1 ciphertext / 256 threads) shape
     size_t wide2_max;                    // largest batch launched in the wide2 (1 ciphertext / 512 threads / SM) shape
@@ -102,6 +108,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     ctx->device = device;
     ctx->stream = (cudaStream_t)stream;
     ctx->d_ph_fwd = ctx->d_ph_inv = ctx->d_ones512 = nullptr;
+    ctx->d_fft_tab = nullptr;
     ctx->d_sched = nullptr; ctx->d_state = nullptr; ctx->sched_words = ctx->state_words = 0;
     ctx->d_cv_blocks = nullptr; ctx->cv_words = 0;
     *out = ctx;   // returned even on failure so that nb_last_error() can be read; caller destroys it
@@ -117,6 +124,8 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
         ctx->force_chunks = e ? atoi(e) : 0;
         e = getenv("NUFHE_B200_STAGGER");
         ctx->stagger_cycles = e ? atoi(e) : 12000;        // about a quarter of a CMux step (measured best of 0 / 12k / 24k / 36k)
+        e = getenv("NUFHE_B200_FFT");
+        ctx->fft = e ? atoi(e) : 1;
     }
     if (const char *e = getenv("NUFHE_B200_FORCE_RARE_PATH")) {
         // test knob: run the canonicalisation fix-up of the deferred-canonicalisation phases on every task
@@ -135,6 +144,13 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check(ctx, cudaMemcpy(ctx->d_ph_inv, pt.inv.data(), NTT_N * sizeof(u64), cudaMemcpyHostToDevice), "memcpy"));
     NB_TRY(check(ctx, cudaMalloc(&ctx->d_ones512, NTT_N * sizeof(u64)), "cudaMalloc"));
     NB_TRY(check(ctx, cudaMemcpy(ctx->d_ones512, pt.ones512.data(), NTT_N * sizeof(u64), cudaMemcpyHostToDevice), "memcpy"));
+    {
+        FftTables ft;
+        NB_TRY(check(ctx, cudaMalloc(&ctx->d_fft_tab, FFT_TAB_CPLX * sizeof(cplx)), "cudaMalloc"));
+        NB_TRY(check(ctx, cudaMemcpy(ctx->d_fft_tab, ft.tab.data(), FFT_TAB_CPLX * sizeof(cplx), cudaMemcpyHostToDevice), "memcpy"));
+    }
+    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrFft>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)br_smem_bytes<BrFft>()), "cudaFuncSetAttribute(blind_rotate fft)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrDefault>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)br_smem_bytes<BrDefault>()), "cudaFuncSetAttribute(blind_rotate)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrWide>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -150,6 +166,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check_resident<BrDefault>(ctx));
     NB_TRY(check_resident<BrWide>(ctx));
     NB_TRY(check_resident<BrWide2>(ctx));
+    NB_TRY(check_resident<BrFft>(ctx));
     {   // batches that fit one wave of wide CTAs (one ciphertext on 256 threads) take the low-latency shape
         const char *e = getenv("NUFHE_B200_WIDE_MAX");
         // up to one wave the wide shape has the shortest step; between one and ~1.7 waves it still wins, time-sliced
@@ -203,6 +220,7 @@ void nb_ctx_destroy(nb_ctx *ctx)
     if (ctx->d_ph_fwd) cudaFree(ctx->d_ph_fwd);
     if (ctx->d_ph_inv) cudaFree(ctx->d_ph_inv);
     if (ctx->d_ones512) cudaFree(ctx->d_ones512);
+    if (ctx->d_fft_tab) cudaFree(ctx->d_fft_tab);
     if (ctx->d_sched) cudaFree(ctx->d_sched);
     if (ctx->d_state) cudaFree(ctx->d_state);
     if (ctx->d_cv_blocks) cudaFree(ctx->d_cv_blocks);
@@ -319,7 +337,32 @@ int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t 
     size_t total = rows * NTT_N, blocks = (total + 255) / 256, cap = (size_t)ctx->sm_count * 16;
     bk_prepare_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>((const u64 *)bk_ref, (u64 *)bk_int,
                                                                                   ctx->d_ones512, rows);
-    return launch_check(ctx, "bk_prepare_kernel");
+    NB_TRY(launch_check(ctx, "bk_prepare_kernel"));
+    // the FP64 part of every row: key polynomials back to coefficients (plain form, inverse transform), integrality
+    // check, 16-bit split, spectra (kernels.cuh: bk_spectra_kernel)
+    const u64 *key_begin = (const u64 *)bk_int, *key_end = key_begin + rows * BK_ROW_U64;
+    for (size_t i = 0; i < ctx->spectral_keys.size();) {       // forget keys this one overwrites
+        if (ctx->spectral_keys[i].first < key_end && key_begin < ctx->spectral_keys[i].second) ctx->spectral_keys.erase(ctx->spectral_keys.begin() + i);
+        else i++;
+    }
+    const size_t polys = rows * 8, words = polys * NTT_N;
+    u64 *tmp = nullptr;
+    NB_TRY(check(ctx, cudaMalloc(&tmp, 2 * words * sizeof(u64) + sizeof(int)), "cudaMalloc(bk_prepare)"));
+    int *d_flag = (int *)(tmp + 2 * words), not_integral = 0;
+    int rc = check(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), ctx->stream), "cudaMemsetAsync");
+    if (rc == NB_OK) {
+        blocks = (words + 255) / 256;
+        bk_plain_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>((const u64 *)bk_ref, tmp, words);
+        ntt_inverse_kernel<false><<<ntt_grid(ctx, polys), NTT_SWEEP_THREADS, ntt_smem_bytes(NTT_RAW_U64_BYTES), ctx->stream>>>(tmp, tmp + words, ctx->d_ph_inv, polys);
+        bk_spectra_kernel<<<(unsigned)polys, 64, 0, ctx->stream>>>(tmp + words, (u64 *)bk_int, ctx->d_fft_tab, d_flag);
+        rc = launch_check(ctx, "bk_spectra_kernel");
+    }
+    if (rc == NB_OK) rc = check(ctx, cudaMemcpyAsync(&not_integral, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream), "cudaMemcpyAsync");
+    if (rc == NB_OK) rc = check(ctx, cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize");
+    cudaFree(tmp);
+    NB_TRY(rc);
+    if (!not_integral) ctx->spectral_keys.emplace_back(key_begin, key_end);
+    return NB_OK;
 }
 
 }  // extern "C"
@@ -365,6 +408,7 @@ template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
     p.chunks = (unsigned)chunks;
     p.sched = nullptr; p.state = nullptr;
     p.sm_count = ctx->sm_count; p.stagger_cycles = ctx->stagger_cycles;
+    p.fft_tab = ctx->d_fft_tab;
     size_t grid = chains;
     if (chains > slots) {
         // more than one wave: persistent CTAs pull (chain, chunk) tickets
@@ -382,7 +426,8 @@ template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
 }
 
 // One launch of the fused kernel in the shape that suits the batch: "wide" CTAs (1 ciphertext on 256 threads,
-// shortest step) while the batch fits one wave of them, else 2 ciphertexts per CTA (highest throughput).
+// shortest step) while the batch fits one wave of them, else 2 ciphertexts per CTA (highest throughput), with the FP64
+// step when the key has spectra.
 static int launch_br(nb_ctx *ctx, BlindRotateArgs &p)
 {
     if (!p.plain && p.n > 0 && p.batch <= ctx->pair_max) {
@@ -394,6 +439,11 @@ static int launch_br(nb_ctx *ctx, BlindRotateArgs &p)
     }
     if (p.batch <= ctx->wide2_max) return launch_br_cfg<BrWide2>(ctx, p);
     if (p.batch <= ctx->wide_max) return launch_br_cfg<BrWide>(ctx, p);
+    if (ctx->fft) {
+        // the FP64 step needs the key's spectra: keys with integral coefficients prepared on this context
+        for (const auto &k : ctx->spectral_keys)
+            if (k.first <= p.bk && p.bk < k.second) return launch_br_cfg<BrFft>(ctx, p);
+    }
     return launch_br_cfg<BrDefault>(ctx, p);
 }
 

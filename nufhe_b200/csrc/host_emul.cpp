@@ -228,6 +228,107 @@ void emul_phase_step_wide2(i32 *acc_io, const u64 *bk_ref_row, const int *rot)
     phase_step<BrWide2>(acc_io, bk_ref_row, rot, 1);
 }
 
+// ---- the FP64 step (br_phases.cuh: FP64 step) ----
+// key spectra of one polynomial from its centred integer coefficients k[1024], as bk_spectra_kernel computes them:
+// spec[h][512] unpadded (h = 0: k_lo, 1: k_hi)
+static void fft_key_spectra(const long long *k, cplx *spec, const FftTables &F)
+{
+    std::vector<cplx> w(2 * FFT_SPEC_CPLX);
+    for (int n0 = 0; n0 < 64; n0++) {
+        long long kk[16];
+        double lo[16], hi[16];
+        for (int j = 0; j < 16; j++) kk[j] = k[64 * j + n0];
+        fft_split_key(kk, lo, hi);
+        fft_fwd1(n0, lo, w.data(), F.tab.data());
+        fft_fwd1(n0, hi, w.data() + FFT_SPEC_CPLX, F.tab.data());
+    }
+    for (int h = 0; h < 2; h++) for (int t = 0; t < 64; t++) fft_fwd2(t >> 3, t & 7, w.data() + h * FFT_SPEC_CPLX, F.tab.data());
+    for (int h = 0; h < 2; h++) for (int t = 0; t < 64; t++) fft_fwd3(t >> 3, t & 7, w.data() + h * FFT_SPEC_CPLX);
+    for (int h = 0; h < 2; h++) for (int P = 0; P < FFT_M; P++) spec[h * FFT_M + P] = w[h * FFT_SPEC_CPLX + fft_pad(P)];
+}
+
+// the FP64 part of one engine key row from the reference row (Montgomery, natural order): -1 if a coefficient is not a
+// centred 32-bit integer
+static int fft_key_row(const u64 *bk_ref_row, std::vector<cplx> &key)
+{
+    static FftTables F;
+    key.assign(BK_FFT_SPECTRA * FFT_M, cplx{0, 0});
+    std::vector<u64> plain(NTT_N), coef(NTT_N);
+    std::vector<long long> k(NTT_N);
+    for (int m = 0; m < 8; m++) {
+        for (int i = 0; i < NTT_N; i++) plain[i] = ff_mul(ff_canon(bk_ref_row[m * NTT_N + i]), FF_RINV);
+        emul_ntt_inverse(plain.data(), coef.data(), 1);
+        for (int i = 0; i < NTT_N; i++) {
+            const u64 v = coef[i], half = 1ull << 31;
+            if (v < half) k[i] = (long long)v;
+            else if (v >= FF_P - half) k[i] = -(long long)(FF_P - v);
+            else return -1;
+        }
+        fft_key_spectra(k.data(), key.data() + m * 2 * FFT_M, F);
+    }
+    return 0;
+}
+
+// One CMux step (rot != NULL) or plain external product of the FP64 step for nct <= 2 ciphertexts, phase by phase as
+// br_fft_step runs them (BrFft: 256 threads); returns -1 for a key without integral coefficients
+int emul_fft_step(i32 *acc_io, const u64 *bk_ref_row, const int *rot, int nct)
+{
+    static FftTables F;
+    using Cfg = BrFft;
+    std::vector<cplx> key;
+    if (fft_key_row(bk_ref_row, key)) return -1;
+    std::vector<i32> acc(Cfg::CT * 2 * NTT_N, 0);
+    std::vector<cplx> w(Cfg::POLYS * FFT_SPEC_CPLX, cplx{1e300, -1e300});
+    for (int c = 0; c < nct; c++) memcpy(&acc[c * 2 * NTT_N], acc_io + c * 2 * NTT_N, sizeof(i32) * 2 * NTT_N);
+    int rots[2] = {0, 0};
+    if (rot) for (int c = 0; c < nct; c++) rots[c] = rot[c];
+    const cplx *tab = F.tab.data();
+    constexpr int TH = Cfg::THREADS;
+    for (int tid = 0; tid < TH; tid++) {
+        if (rot) fft_phase_fwd1<true>(tid, acc.data(), w.data(), tab, rots); else fft_phase_fwd1<false>(tid, acc.data(), w.data(), tab, rots);
+    }
+    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_fwd2(x, w.data(), tab);
+    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_fwd3(x, w.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_mac<Cfg::CT, TH>(tid, w.data(), key.data());
+    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_inv3(x, w.data());
+    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_inv2(x, w.data(), tab);
+    for (int tid = 0; tid < TH; tid++) {
+        if (rot) fft_phase_inv1<true>(tid, acc.data(), w.data(), tab); else fft_phase_inv1<false>(tid, acc.data(), w.data(), tab);
+    }
+    for (int c = 0; c < nct; c++) memcpy(acc_io + c * 2 * NTT_N, &acc[c * 2 * NTT_N], sizeof(i32) * 2 * NTT_N);
+    return 0;
+}
+
+// The transform chain of the FP64 step on given inputs, for the exactness tests: digit polynomials dig[4][1024] (signed,
+// |d| <= 512) and key polynomials key[4][1024] (centred 32-bit); out[h][1024] = the UNROUNDED coefficients of
+// sum_d dig_d * key_d,h mod X^1024 + 1 for the key halves h = 0 (lo), 1 (hi), through the same passes and MAC as the
+// kernel (one ciphertext, one output polynomial).
+void emul_fft_product(const double *dig, const long long *key, double *out)
+{
+    static FftTables F;
+    const cplx *tab = F.tab.data();
+    std::vector<cplx> ks(BK_FFT_SPECTRA * FFT_M, cplx{0, 0});
+    for (int d = 0; d < 4; d++) fft_key_spectra(key + d * NTT_N, ks.data() + (d * 2 + 0) * 2 * FFT_M, F);   // mo = 0
+    std::vector<cplx> w(BrFft::POLYS * FFT_SPEC_CPLX, cplx{0, 0});
+    for (int d = 0; d < 4; d++)
+        for (int n0 = 0; n0 < 64; n0++) {
+            double x[16];
+            for (int j = 0; j < 16; j++) x[j] = dig[d * NTT_N + 64 * j + n0];
+            fft_fwd1(n0, x, w.data() + d * FFT_SPEC_CPLX, tab);
+        }
+    for (int x = 0; x < 64 * 4; x++) fft_phase_fwd2(x, w.data(), tab);
+    for (int x = 0; x < 64 * 4; x++) fft_phase_fwd3(x, w.data());
+    for (int P = 0; P < FFT_M; P++) fft_mac_point<1>(P, w.data(), ks.data());
+    for (int x = 0; x < 64 * 2; x++) fft_phase_inv3(x, w.data());       // spectra 0, 1: mo = 0, h = 0 / 1
+    for (int x = 0; x < 64 * 2; x++) fft_phase_inv2(x, w.data(), tab);
+    for (int h = 0; h < 2; h++)
+        for (int n0 = 0; n0 < 64; n0++) {
+            double x[16];
+            fft_inv1(n0, w.data() + h * FFT_SPEC_CPLX, tab, x);
+            for (int j = 0; j < 16; j++) out[h * NTT_N + 64 * j + n0] = x[j];
+        }
+}
+
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)
 { for (size_t i = 0; i < n; i++) out[i] = ff_shl_var(in[i], s[i]); }
 void emul_ff_mul(const u64 *a, const u64 *b, u64 *out, size_t n)

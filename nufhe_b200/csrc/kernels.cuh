@@ -265,14 +265,60 @@ __global__ void bk_prepare_kernel(const u64 *__restrict__ bk_ref, u64 *__restric
     }
 }
 
+// ---- FP64 part of the engine key (br_phases.cuh: FP64 step) ----------------------------------------------------------
+// plain[i] = the reference key value i out of Montgomery form (natural order): the input of the inverse transform that
+// recovers the key polynomials' coefficients
+__global__ void bk_plain_kernel(const u64 *__restrict__ bk_ref, u64 *__restrict__ plain, size_t n)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        plain[i] = ff_mul(ff_canon(bk_ref[i]), FF_RINV);
+}
+// One CTA of 64 threads per key polynomial (blockIdx.x = row * 8 + m): its coefficients mod p (natural order) must be
+// centred 32-bit integers; they are split into 16-bit halves and both halves transformed with the passes of the
+// bootstrap.  A coefficient outside [-2^31, 2^31) sets *not_integral (the key then keeps the NTT step everywhere).
+__global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ coef, u64 *__restrict__ bk_int,
+                                                        const cplx *__restrict__ tab, int *__restrict__ not_integral)
+{
+    __shared__ __align__(16) cplx spec[2][FFT_SPEC_CPLX];
+    const size_t poly = blockIdx.x, row = poly >> 3;
+    const int m = (int)(poly & 7), n0 = threadIdx.x;
+    long long k[16];
+    bool bad = false;
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+        const u64 v = ff_canon(coef[poly * NTT_N + 64 * j + n0]);
+        const u64 half = 1ull << 31;
+        if (v < half) k[j] = (long long)v;
+        else if (v >= FF_P - half) k[j] = -(long long)(FF_P - v);
+        else { k[j] = 0; bad = true; }
+    }
+    if (bad) atomicOr(not_integral, 1);
+    {
+        double lo[16], hi[16];
+        fft_split_key(k, lo, hi);
+        fft_fwd1(n0, lo, spec[0], tab);
+        fft_fwd1(n0, hi, spec[1], tab);
+    }
+    __syncthreads();
+    for (int h = 0; h < 2; h++) fft_fwd2(n0 >> 3, n0 & 7, spec[h], tab);
+    __syncthreads();
+    for (int h = 0; h < 2; h++) fft_fwd3(n0 >> 3, n0 & 7, spec[h]);
+    __syncthreads();
+    cplx *out = reinterpret_cast<cplx *>(bk_int + row * BK_ROW_U64 + BK_NTT_U64) + (size_t)m * 2 * FFT_M;
+    for (int P = n0; P < FFT_M; P += 64)
+        for (int h = 0; h < 2; h++) out[h * FFT_M + P] = spec[h][fft_pad(P)];
+}
+
 // mod-switch to [0, 2N) (numeric_functions_gpu.py:55-71)
 NB_HD i32 modswitch_2n(i32 x) { return (i32)(((u32)x + (1u << 20)) >> 21); }
 
 // ---- fused bootstrap: CTA-wide phases over shared-memory-resident polynomials (br_phases.cuh) -----
+// u64 per work polynomial: an NTT work polynomial, or a padded spectrum of the FP64 step
+template <class Cfg> NB_HDC int br_poly_u64() { return Cfg::FFT ? FFT_SPEC_CPLX * 2 : POLY_STRIDE; }
 template <class Cfg> constexpr size_t br_smem_bytes()
 {
-    return (size_t)Cfg::CT * 2 * NTT_N * sizeof(i32) + (size_t)Cfg::POLYS * POLY_STRIDE * sizeof(u64) +
-           (Cfg::TWD_GLOBAL ? 0 : 2 * NTT_N * sizeof(u64)) + 64 + (Cfg::STAGE_KEY ? BK_ROW_U64 * sizeof(u64) : 0);
+    return (size_t)Cfg::CT * 2 * NTT_N * sizeof(i32) + (size_t)Cfg::POLYS * br_poly_u64<Cfg>() * sizeof(u64) +
+           (Cfg::TWD_GLOBAL ? 0 : 2 * NTT_N * sizeof(u64)) + 64 + (Cfg::STAGE_KEY ? BK_NTT_U64 * sizeof(u64) : 0);
 }
 constexpr size_t BR2_SMEM_BYTES = br_smem_bytes<BrDefault>();
 
@@ -289,6 +335,7 @@ struct BlindRotateArgs {
     // mode B (BlindRotate_gpu, blind_rotate.py:262-281): explicit accumulator (B,2,1024) and bara (B,n)
     const i32 *accum, *bara;
     const u64 *bk;          // internal layout, n rows
+    const cplx *fft_tab;    // tables of the FP64 step (tables.h: FftTables)
     i32 *out_a, *out_b;     // extracted LWE samples (B,1024), (B,)
     i32 *accum_out;         // optional: final accumulators (B,2,1024)
     int n;                  // LWE dimension (500); n = 0 with `plain` = one external product
@@ -311,14 +358,14 @@ struct Br2Smem {
     u64 *twd_fwd;  // [16][64]
     u64 *twd_inv;
     int *rot;      // [2][CT], 64 bytes
-    u64 *key;      // Cfg::STAGE_KEY: the key row of the current step, [BK_PLANES][1024]
+    u64 *key;      // Cfg::STAGE_KEY: the NTT part of the key row of the current step, [BK_PLANES][1024]
 };
 
 template <class Cfg> NB_D Br2Smem br2_carve(unsigned char *raw)
 {
     Br2Smem s;
     s.w = reinterpret_cast<u64 *>(raw);
-    s.twd_fwd = s.w + Cfg::POLYS * POLY_STRIDE;
+    s.twd_fwd = s.w + Cfg::POLYS * br_poly_u64<Cfg>();
     s.twd_inv = s.twd_fwd + (Cfg::TWD_GLOBAL ? 0 : NTT_N);
     s.acc = reinterpret_cast<i32 *>(s.twd_inv + (Cfg::TWD_GLOBAL ? 0 : NTT_N));
     s.rot = reinterpret_cast<int *>(s.acc + Cfg::CT * 2 * NTT_N);
@@ -361,7 +408,7 @@ NB_D i32 br2_initial_acc(const BlindRotateArgs &p, size_t c, int mi, int x)
 // 16-byte cp.async requests for one key row, spread over `nthreads` threads (t = 0 .. nthreads - 1); one commit group
 NB_D void br2_stage_key(u64 *key, const u64 *__restrict__ bk_row, int t, int nthreads)
 {
-    for (int x = t; x < BK_ROW_U64 / 2; x += nthreads) cp_async16(key + 2 * x, bk_row + 2 * x);
+    for (int x = t; x < BK_NTT_U64 / 2; x += nthreads) cp_async16(key + 2 * x, bk_row + 2 * x);
     cp_async_commit();
 }
 
@@ -446,6 +493,31 @@ NB_D void br2_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *
     }
 }
 
+// The FP64 step (br_phases.cuh: FP64 step): the same seven barrier-separated phases as br2_step, on spectra of 512
+// complex doubles instead of NTT work polynomials; bk_row: the whole engine key row (its FP64 part is read)
+template <bool ROTATE, class Cfg>
+NB_D void br_fft_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *rot, int tid, const cplx *__restrict__ tab)
+{
+    cplx *spec = reinterpret_cast<cplx *>(s.w);
+    fft_phase_fwd1<ROTATE>(tid, s.acc, spec, tab, rot);          // 128 CT tasks: (ct, mi, n0), both digits
+    __syncthreads();
+#pragma unroll 1
+    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_fwd2(x, spec, tab);
+    __syncthreads();
+#pragma unroll 1
+    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_fwd3(x, spec);
+    __syncthreads();
+    fft_phase_mac<Cfg::CT, Cfg::THREADS>(tid, spec, reinterpret_cast<const cplx *>(bk_row + BK_NTT_U64));
+    __syncthreads();
+#pragma unroll 1
+    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_inv3(x, spec);
+    __syncthreads();
+#pragma unroll 1
+    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_inv2(x, spec, tab);
+    __syncthreads();
+    fft_phase_inv1<ROTATE>(tid, s.acc, spec, tab);                // 128 CT tasks: (ct, mo, n0), both key halves
+}
+
 NB_D unsigned ld_acquire_u32(const unsigned *p)
 {
     unsigned v;
@@ -479,7 +551,9 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
     Br2Smem s = br2_carve<Cfg>(smem_raw);
     __shared__ unsigned s_item, s_entry;
     const int tid = threadIdx.x;
-    if (Cfg::TWD_GLOBAL) {
+    if (Cfg::FFT) {
+        // the FP64 step reads its tables through the L1 (p.fft_tab)
+    } else if (Cfg::TWD_GLOBAL) {
         s.twd_fwd = const_cast<u64 *>(twd_fwd_g); s.twd_inv = const_cast<u64 *>(twd_inv_g);
     } else {
         for (int i = tid; i < NTT_N; i += Cfg::THREADS) { s.twd_fwd[i] = twd_fwd_g[i]; s.twd_inv[i] = twd_inv_g[i]; }
@@ -542,7 +616,8 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
         }
         if (p.plain) {
             __syncthreads();
-            br2_step<false, Cfg>(s, p.bk, s.rot, tid);
+            if constexpr (Cfg::FFT) br_fft_step<false, Cfg>(s, p.bk, s.rot, tid, p.fft_tab);
+            else br2_step<false, Cfg>(s, p.bk, s.rot, tid);
             __syncthreads();
         } else {
             if (tid < Cfg::CT) s.rot[(step0 & 1) * Cfg::CT + tid] = br2_rotation(p, ct_of(tid), step0);
@@ -550,8 +625,11 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
             for (int i = step0; i < step1; i++) {
                 int next = 0;
                 if (tid < Cfg::CT && i + 1 < step1) next = br2_rotation(p, ct_of(tid), i + 1);
-                br2_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid,
-                                    i + 1 < step1 ? p.bk + (size_t)(i + 1) * BK_ROW_U64 : nullptr);
+                if constexpr (Cfg::FFT)
+                    br_fft_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid, p.fft_tab);
+                else
+                    br2_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid,
+                                        i + 1 < step1 ? p.bk + (size_t)(i + 1) * BK_ROW_U64 : nullptr);
                 if (tid < Cfg::CT) s.rot[((i + 1) & 1) * Cfg::CT + tid] = next;
                 __syncthreads();
             }

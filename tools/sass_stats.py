@@ -1,12 +1,16 @@
 #!/usr/bin/env python
 """Static per-phase / per-pipe instruction counts of the fused bootstrap kernel, from the SASS of the built
-library (no GPU needed).  The kernel is bound by the integer ALU pipe, so the ALU column of the step loop is
+library (no GPU needed).  The NTT step is bound by the integer ALU pipe, so the ALU column of its step loop is
 the number that predicts its run time; use this to judge an arithmetic change before spending GPU minutes.
+The default kernel is the one the benchmark's workload launches: the throughput shape with the FP64 step
+(`br_fft_step`, BrFft); its FP64 instructions (DADD / DMUL / DFMA, 2 cycles per warp-instruction on an H100 SXM SM
+sub-partition) are counted in the `fp64` column.  The NTT throughput shape is
+`--kernel blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0`.
 
     python tools/sass_stats.py [--kernel blind_rotate_kernel] [--by-func] [--lib path/to/lib.so]
 
 Each SASS instruction is attributed (through nvdisasm's inline chains, the library is built with -lineinfo)
-to the line of `br2_step` in kernels.cuh that called it, i.e. to a phase.  Counts are static: fwd1 / fwd2 /
+to the line of `br2_step` (or `br_fft_step`) in kernels.cuh that called it, i.e. to a phase.  Counts are static: fwd1 / fwd2 /
 fwd3 are multiplied by their two sweeps per step (the `it` loops are not unrolled), the MAC by its two row
 iterations, and code inside the warp-uniform `switch (g)` of fwd2 / inv2 counts a quarter -- see `per step`.
 """
@@ -24,6 +28,7 @@ ALU = ('IADD3', 'IADD', 'LOP3', 'SHF', 'SEL', 'ISETP', 'PRMT', 'VIADD', 'LEA', '
        'R2P', 'IABS', 'FLO', 'POPC', 'BREV', 'SGXT', 'BMSK', 'LOP', 'FSEL', 'FMNMX', 'CS2R', 'VABSDIFF', 'FSETP', 'I2FP')
 FMA = ('IMAD', 'FFMA', 'FMUL', 'FADD', 'HFMA2', 'IDP')
 LSU = ('LDS', 'STS', 'LDG', 'STG', 'LD', 'ST', 'LDSM', 'ATOMS', 'ATOMG', 'RED', 'LDC', 'LDCU', 'UBLKCP', 'SYNCS')
+FP64 = ('DADD', 'DMUL', 'DFMA', 'DSETP', 'DMNMX', 'F2F', 'F2I', 'I2F')
 UNI = ('UMOV', 'UIADD3', 'ULEA', 'ULOP3', 'UISETP', 'USHF', 'UIMAD', 'S2UR', 'UPLOP3', 'USEL', 'UPRMT', 'R2UR', 'UFLO',
        'UP2UR', 'UIADD')
 
@@ -38,11 +43,16 @@ def pipe_of(op):
         return 'lsu'
     if base in UNI:
         return 'uni'
+    if base in FP64:
+        return 'fp64'
     return 'other'
 
 
 COST = {'IMAD.WIDE(+R64)': 4, 'IMAD.WIDE(+RZ)': 4}
-STEP_MULT = {'phase_fwd1': 2, 'phase_fwd2': 2, 'phase_fwd3': 2, 'phase_mac': 2}
+STEP_MULT = {'phase_fwd1': 2, 'phase_fwd2': 2, 'phase_fwd3': 2, 'phase_mac': 2,
+             # the FP64 step (2 ciphertexts on 256 threads): two tasks per thread in the four middle passes and two MAC
+             # points (loops not unrolled); fwd1's digit loop is weighted by `twice_lines`
+             'fft_phase_fwd2': 2, 'fft_phase_fwd3': 2, 'fft_phase_inv3': 2, 'fft_phase_inv2': 2, 'fft_phase_mac': 2}
 
 
 def instruction_form(op, rest):
@@ -79,8 +89,9 @@ def enclosing_functions(path):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--lib', default=os.path.join(ROOT, 'nufhe_b200', 'csrc', 'libnufhe_b200.so'))
-    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256',
-                    help='substring of the mangled kernel name (default: the 2-ciphertext shape; the wide shape is '
+    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb1ELb1',
+                    help='substring of the mangled kernel name (default: the 2-ciphertext shape with the FP64 step; the '
+                         'NTT one is blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0, the wide shape '
                          'blind_rotate_kernelINS_5BrCfgILi1ELi256)')
     ap.add_argument('--by-func', action='store_true', help='also split each phase by innermost ff.cuh / br_phases function')
     ap.add_argument('--opcodes', action='store_true', help='per-step histogram of instruction forms (carry-out variants split)')
@@ -99,15 +110,15 @@ def main():
     phase_lines = {}
     in_step = False
     for i, line in enumerate(ksrc, 1):
-        if 'void br2_step' in line:
+        if 'void br2_step' in line or 'void br_fft_step' in line:
             in_step = True
         if in_step:
-            m = re.search(r'(phase_[a-z0-9_]+)', line)
+            m = re.search(r'((?:fft_)?phase_[a-z0-9_]+)', line)
             if m:
                 phase_lines[i] = m.group(1)
             if line.startswith('}'):
                 in_step = False
-    step_call_lines = [i for i, l in enumerate(ksrc, 1) if 'br2_step<true' in l and 'void' not in l]
+    step_call_lines = [i for i, l in enumerate(ksrc, 1) if ('br2_step<true' in l or 'br_fft_step<true' in l) and 'void' not in l]
     if 'pair' in args.kernel:
         # the pair shape (blind_rotate_pair_kernel): phases are the pair_* calls of its step loop.  Each pair_* wrapper
         # holds BOTH thread halves (`if (h) f<1>(...) else f<0>(...)`), so a thread executes about half of the static
@@ -210,7 +221,7 @@ def main():
             counts['rare:' + phase][pipe] += w
             continue
         counts[phase][pipe] += w
-        if args.opcodes and phase.startswith('phase_'):
+        if args.opcodes and phase.startswith(('phase_', 'fft_phase_')):
             forms[instruction_form(op, m.group(2))] += w * (
                 1 if ('BrCfgILi1E' in args.kernel and phase.startswith('phase_fwd')) else STEP_MULT.get(phase, 1))
         if args.by_func and chain:
@@ -230,23 +241,23 @@ def main():
         import json
         tot = collections.Counter()
         for phase, c in counts.items():
-            if phase.startswith('phase_'):
+            if phase.startswith(('phase_', 'fft_phase_')):
                 for k, v in c.items():
                     tot[k] += v * mult.get(phase, 1)
-        print(json.dumps({'kernel': args.kernel, 'per_thread_step': {k: tot[k] for k in ('alu', 'fma', 'lsu', 'uni', 'other')},
+        print(json.dumps({'kernel': args.kernel, 'per_thread_step': {k: tot[k] for k in ('alu', 'fma', 'fp64', 'lsu', 'uni', 'other')},
                           'per_thread_step_total': sum(tot.values()),
-                          'phases': {ph: sum(c.values()) * mult.get(ph, 1) for ph, c in counts.items() if ph.startswith('phase_')}}))
+                          'phases': {ph: sum(c.values()) * mult.get(ph, 1) for ph, c in counts.items() if ph.startswith(('phase_', 'fft_phase_'))}}))
         return 0
-    print('%-22s %7s %7s %7s %7s %7s %8s' % ('phase (static)', 'alu', 'fma', 'lsu', 'uni', 'other', 'total'))
+    print('%-22s %7s %7s %7s %7s %7s %7s %8s' % ('phase (static)', 'alu', 'fma', 'fp64', 'lsu', 'uni', 'other', 'total'))
     tot = collections.Counter()
     for phase in sorted(counts):
         c = counts[phase]
-        print('%-22s %7d %7d %7d %7d %7d %8d' % (phase, c['alu'], c['fma'], c['lsu'], c['uni'], c['other'], sum(c.values())))
-        if phase.startswith('phase_'):
+        print('%-22s %7d %7d %7d %7d %7d %7d %8d' % (phase, c['alu'], c['fma'], c['fp64'], c['lsu'], c['uni'], c['other'], sum(c.values())))
+        if phase.startswith(('phase_', 'fft_phase_')):
             for k, v in c.items():
                 tot[k] += v * mult.get(phase, 1)
-    print('%-22s %7d %7d %7d %7d %7d %8d   (sweeps, MAC rows and switch weights applied)' % (
-        'per step, per thread', tot['alu'], tot['fma'], tot['lsu'], tot['uni'], tot['other'], sum(tot.values())))
+    print('%-22s %7d %7d %7d %7d %7d %7d %8d   (sweeps, MAC rows and switch weights applied)' % (
+        'per step, per thread', tot['alu'], tot['fma'], tot['fp64'], tot['lsu'], tot['uni'], tot['other'], sum(tot.values())))
     if args.opcodes:
         # issue cost in SMSP cycles per warp-instruction (tools/microbench/pipes.cu): 2 on either integer
         # pipe, except IMAD.WIDE with a 64-bit addend: 4
@@ -260,7 +271,7 @@ def main():
                 print('   %-20s %7.0f' % (k, v))
     if args.by_func:
         for phase in sorted(byfunc):
-            if not phase.startswith('phase_'):
+            if not phase.startswith(('phase_', 'fft_phase_')):
                 continue
             print('--', phase)
             agg = collections.defaultdict(collections.Counter)
