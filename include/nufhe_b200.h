@@ -71,7 +71,9 @@ int nb_ff_elementwise(nb_ctx *ctx, int op, const uint64_t *a, const uint64_t *b,
  * Re-lays `rows` reference rows (each 2*2*2*1024 uint64) into the engine's internal row format:
  * nb_bk_row_u64() uint64 per row (the 8 planes re-ordered and un-Montgomery-ed + 2 correction planes, then the
  * FP64 spectra of the 16-bit key halves).  Synchronises the context's stream: it records whether the key's
- * coefficients are centred 32-bit integers, which decides whether the throughput shape runs the FP64 step on it. */
+ * coefficients are centred 32-bit integers, which decides whether the throughput shape runs the FP64 step on it.
+ * That choice is made per call and covers only the `rows` rows of that call: a launch takes the FP64 step only when
+ * every key row it reads was prepared by one such call (a key assembled from several calls keeps the NTT step). */
 size_t nb_bk_row_u64(void);
 int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t rows);
 

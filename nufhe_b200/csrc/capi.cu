@@ -440,9 +440,11 @@ static int launch_br(nb_ctx *ctx, BlindRotateArgs &p)
     if (p.batch <= ctx->wide2_max) return launch_br_cfg<BrWide2>(ctx, p);
     if (p.batch <= ctx->wide_max) return launch_br_cfg<BrWide>(ctx, p);
     if (ctx->fft) {
-        // the FP64 step needs the key's spectra: keys with integral coefficients prepared on this context
+        // the FP64 step needs the spectra of every row the launch reads: all of them must come from one nb_bk_prepare
+        // call on this context whose key had integral coefficients (rows prepared by other calls may have none)
+        const u64 *end = p.bk + (size_t)(p.plain ? 1 : p.n) * BK_ROW_U64;
         for (const auto &k : ctx->spectral_keys)
-            if (k.first <= p.bk && p.bk < k.second) return launch_br_cfg<BrFft>(ctx, p);
+            if (k.first <= p.bk && end <= k.second) return launch_br_cfg<BrFft>(ctx, p);
     }
     return launch_br_cfg<BrDefault>(ctx, p);
 }

@@ -269,6 +269,17 @@ static int fft_key_row(const u64 *bk_ref_row, std::vector<cplx> &key)
     return 0;
 }
 
+// The FP64 part of one engine key row (BK_FFT_U64 doubles: 16 spectra of 512 complex values, the layout
+// bk_spectra_kernel writes after the NTT planes) from the reference row; -1 if a coefficient is not a centred 32-bit
+// integer
+int emul_fft_key_row(const u64 *bk_ref_row, double *out)
+{
+    std::vector<cplx> key;
+    if (fft_key_row(bk_ref_row, key)) return -1;
+    memcpy(out, key.data(), key.size() * sizeof(cplx));
+    return 0;
+}
+
 // One CMux step (rot != NULL) or plain external product of the FP64 step for nct <= 2 ciphertexts, phase by phase as
 // br_fft_step runs them (BrFft: 256 threads); returns -1 for a key without integral coefficients
 int emul_fft_step(i32 *acc_io, const u64 *bk_ref_row, const int *rot, int nct)

@@ -386,6 +386,15 @@ def poly_mul_i32(a, b):
     return out
 
 
+def bk_transform(raw):
+    """Bootstrap-key polynomials (..., N) int32 -> the reference's form: NTT, Montgomery (tgsw_transform_samples,
+    tlwe_gpu.py:199-236); linear over the field, so keys with coefficients outside int32 are sums of two transforms."""
+    raw = _c(raw, numpy.int32)
+    out = numpy.empty(raw.shape, numpy.uint64)
+    lib().orc_bk_transform(_p(out), _p(raw), _sz(_batch(raw)))
+    return out
+
+
 class OracleKeys:
     """Secret + cloud key material as host arrays, drawn in the reference's order from a seed."""
 
@@ -417,9 +426,7 @@ class OracleKeys:
                 bk[:, mi, :, mi, 0] += self.lwe_key[:, None] * base_powers[None, :]
         self.bk_raw = bk
         # tgsw_transform_samples: NTT + Montgomery form (tlwe_gpu.py:199-236)
-        out = numpy.empty(bk.shape, numpy.uint64)
-        lib().orc_bk_transform(_p(out), _p(bk), _sz(bk.size // N))
-        self.bk = out
+        self.bk = bk_transform(bk)
         # (4) key-switch key, lwe.py:265-295 + lwe_cpu.py:26-59; input size k * N
         t, base = KS_T, 2**KS_LOG2_BASE
         size_in = k * N

@@ -118,24 +118,26 @@ def test_full_size_batches_decrypt_to_truth_table(eng, keys, dev_keys, batch):
 
 
 def test_all_cta_shapes_give_the_same_bits(keys, monkeypatch):
-    """The fused bootstrap has four shapes: 2 ciphertexts per 256 threads (throughput), 1 ciphertext per 256 threads
-    (inverse phases split over thread pairs), 1 ciphertext per 512 threads (forward phases split as well; batches
-    up to 1.5 ciphertexts per SM) and 1 ciphertext per cluster of two 256-thread CTAs on two SMs (partial sums of the
-    MAC exchanged through distributed shared memory, in both exchange variants; batches whose clusters all fit).  Force
-    each shape for the same
-    inputs, including a ragged batch and one larger than a wave (time-sliced, or clusters queued by the hardware); all
-    must equal the oracle and each other."""
+    """The fused bootstrap has four shapes: 2 ciphertexts per 256 threads (throughput, with the FP64 step or, forced,
+    the NTT step), 1 ciphertext per 256 threads (inverse phases split over thread pairs), 1 ciphertext per 512 threads
+    (forward phases split as well; batches up to 1.5 ciphertexts per SM) and 1 ciphertext per cluster of two
+    256-thread CTAs on two SMs (partial sums of the MAC exchanged through distributed shared memory, in both exchange
+    variants; batches whose clusters all fit).  Force each shape for the same inputs, including a ragged batch and one
+    larger than a wave (time-sliced, or clusters queued by the hardware); all must equal the oracle and each other."""
     from nufhe_b200.engine import Engine
     rng = G.rs(480)
-    shapes = {'default': ('0', '0', '0', '1'), 'wide': ('1000000', '0', '0', '1'), 'wide2': ('1000000', '1000000', '0', '1'),
-              'pair': ('0', '0', '1000000', '1'),            # exchange by st.async + mbarrier (the default)
-              'pair_barrier': ('0', '0', '1000000', '0')}    # exchange by plain remote stores + barrier.cluster
+    shapes = {'default': ('0', '0', '0', '1', '1'),          # the throughput shape with the FP64 step (integral key)
+              'default_ntt': ('0', '0', '0', '1', '0'),      # the throughput shape with the NTT step
+              'wide': ('1000000', '0', '0', '1', '1'), 'wide2': ('1000000', '1000000', '0', '1', '1'),
+              'pair': ('0', '0', '1000000', '1', '1'),       # exchange by st.async + mbarrier (the default)
+              'pair_barrier': ('0', '0', '1000000', '0', '1')}  # exchange by plain remote stores + barrier.cluster
     for B in (1, 5, 301):
         bits_a, bits_b = rng.randint(0, 2, B).astype(bool), rng.randint(0, 2, B).astype(bool)
         a, b = keys.encrypt(bits_a), keys.encrypt(bits_b)
         want = O.gate_binary('nand', a, b, keys.bk, keys.ks) if B <= 5 else None
         outs = {}
-        for name, (wide_max, wide2_max, pair_max, pair_async) in shapes.items():
+        for name, (wide_max, wide2_max, pair_max, pair_async, fft) in shapes.items():
+            monkeypatch.setenv('NUFHE_B200_FFT', fft)
             monkeypatch.setenv('NUFHE_B200_WIDE_MAX', wide_max)
             monkeypatch.setenv('NUFHE_B200_WIDE2_MAX', wide2_max)
             monkeypatch.setenv('NUFHE_B200_PAIR_MAX', pair_max)
@@ -148,7 +150,7 @@ def test_all_cta_shapes_give_the_same_bits(keys, monkeypatch):
             if want is not None:
                 assert (out[0] == want[0]).all() and (out[1] == want[1]).all(), (B, name)
             assert (keys.decrypt(out) == ~(bits_a & bits_b)).all()
-        for name in ('wide', 'wide2', 'pair', 'pair_barrier'):
+        for name in ('default_ntt', 'wide', 'wide2', 'pair', 'pair_barrier'):
             for x, y in zip(outs['default'], outs[name]):
                 assert (x[0] == y[0]).all() and (x[1] == y[1]).all(), (B, name)
 
@@ -279,19 +281,21 @@ print('rare path ok')
 '''
 
 
-@pytest.mark.parametrize('wide_max', ['0', '1000000', 'wide2', 'pair'])
+@pytest.mark.parametrize('wide_max', ['throughput_fp64', 'throughput_ntt', '1000000', 'wide2', 'pair'])
 def test_canonicalisation_rare_path_forced(wide_max):
     """NUFHE_B200_FORCE_RARE_PATH=1 lowers the trigger of the deferred canonicalisation so that EVERY task of fwd1,
     inv1 and the MAC runs its fix-up code (normally 2^-32 per element); results must not change.  Runs in a fresh
-    process because the trigger is a __constant__ set when the context is created."""
+    process because the trigger is a __constant__ set when the context is created.  The throughput shape runs the
+    FP64 step on the (integral) gate key unless NUFHE_B200_FFT=0 keeps its NTT step, which has the fix-up code."""
     import os
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     env = dict(os.environ, NUFHE_B200_FORCE_RARE_PATH='1')
+    env['NUFHE_B200_FFT'] = '0' if wide_max == 'throughput_ntt' else '1'
     env['NUFHE_B200_PAIR_MAX'] = '1000000' if wide_max == 'pair' else '0'
     env.update({'NUFHE_B200_WIDE_MAX': '1000000', 'NUFHE_B200_WIDE2_MAX': '1000000'} if wide_max == 'wide2' else
-               {'NUFHE_B200_WIDE_MAX': '0' if wide_max == 'pair' else wide_max, 'NUFHE_B200_WIDE2_MAX': '0'})
+               {'NUFHE_B200_WIDE_MAX': '1000000' if wide_max == '1000000' else '0', 'NUFHE_B200_WIDE2_MAX': '0'})
     r = subprocess.run([sys.executable, '-c', _RARE_PATH_SCRIPT % {'root': root}], env=env, capture_output=True,
                        text=True, timeout=600)
     assert r.returncode == 0 and 'rare path ok' in r.stdout, r.stdout + r.stderr

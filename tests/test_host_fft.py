@@ -120,6 +120,26 @@ def test_fft_step_matches_oracle(emul):
         assert (a == O.tgsw_external_mul(acc, keys.bk, 1)).all()
 
 
+def test_fft_key_row_accepts_exactly_the_32_bit_range(emul):
+    """Key preparation on the host (emul_fft_key_row, the computation of kernels.cuh: bk_spectra_kernel): the extreme
+    centred 32-bit coefficients -2^31 and 2^31 - 1 are accepted; one coefficient just outside that range, at the last
+    position of the last polynomial of the row, rejects the whole row."""
+    out = numpy.empty(16 * 512 * 2, numpy.float64)
+    lows = numpy.full((2, 2, 2, 1024), -2**31, numpy.int32)
+    assert emul.emul_fft_key_row(_p(O.bk_transform(lows)), _p(out)) == 0
+    spec = out.view(numpy.complex128).reshape(8, 2, 512)        # [m][h][P]
+    assert (spec[:, 0] == 0).all()                 # -2^31 = 0 + 2^16 * (-2^15): the low half is zero ...
+    assert (numpy.abs(spec[:, 1]) > 0).all()       # ... the high half, all -2^15, is 2 c / (1 - z) at each root z
+    highs = numpy.full((2, 2, 2, 1024), 2**31 - 1, numpy.int32)
+    assert emul.emul_fft_key_row(_p(O.bk_transform(highs)), _p(out)) == 0
+    for edge, step in ((2**31 - 1, 1), (-2**31, -1)):          # 2^31, -2^31 - 1 at (m = 7, coefficient 1023)
+        raw = numpy.zeros((2, 2, 2, 1024), numpy.int32)
+        one = numpy.zeros_like(raw)
+        raw[1, 1, 1, 1023], one[1, 1, 1, 1023] = edge, step
+        assert emul.emul_fft_key_row(_p(O.ff_add(O.bk_transform(raw), O.bk_transform(one))), _p(out)) == -1
+        assert emul.emul_fft_key_row(_p(O.bk_transform(raw)), _p(out)) == 0
+
+
 def test_fft_step_refuses_random_field_keys(emul):
     """A key whose polynomials are not centred 32-bit integers (uniformly random field elements) has no spectra: such
     keys keep the NTT step in every shape."""
