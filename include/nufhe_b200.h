@@ -1,6 +1,7 @@
 /*
  * nufhe_b200.h -- C ABI of libnufhe_b200.so, the H100 (sm_90a) engine for the gate-bootstrapping hot
- * path of nucypher/nufhe.
+ * path of nucypher/nufhe, and for programmable bootstrapping (lookup tables on small encrypted integers,
+ * nb_bootstrap_lut_extract).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -91,6 +92,18 @@ int nb_blind_rotate(nb_ctx *ctx, const int32_t *accum, const int32_t *bara, cons
 int nb_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
                          const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
                          const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch);
+
+/* ---- programmable bootstrap: the same prologue, x = (0, c) + s1 * in1 + s2 * in2, with an arbitrary test vector.
+ * tv: 1024 int32 per vector, one for the batch (tv_stride 0) or one per ciphertext (tv_stride 1024); never NULL.
+ * barb and every bara_i are rounded to multiples of 2^L (L = log2_outputs, 0..2), the accumulator starts as
+ * (0, X^(2N - barb) * tv), and after the blind rotation the samples at indices j = 0 .. 2^L - 1 (coefficient j of the
+ * phase: extraction after a rotation by X^(-j)) go to rows c * 2^L + j.  Output: out_a (B * 2^L, 1024),
+ * out_b (B * 2^L,).  NB_EINVAL for a NULL tv, a stride other than 0 / 1024 or L outside 0..2.  The key switch of
+ * the B * 2^L samples that usually follows needs nb_ctx_reserve(B * 2^L) before a graph capture. */
+int nb_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                             const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv,
+                             size_t tv_stride, int log2_outputs, const uint64_t *bk_int, size_t n, int32_t *out_a,
+                             int32_t *out_b, size_t batch);
 
 /* Two bootstraps in one launch (gate_mux, gates.py:638-655): job A on ciphertexts [0, B), job B on [B, 2B);
  * out_a (2B,1024), out_b (2B,).  Halves the latency of small-batch MUX gates. */

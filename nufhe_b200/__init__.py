@@ -8,6 +8,8 @@ from .api_low_level import (
     make_key_pair,
     encrypt,
     decrypt,
+    encrypt_int,
+    decrypt_int,
     empty_ciphertext,
     NuFHEParameters,
     NuFHESecretKey,
@@ -32,6 +34,12 @@ from .gates import (
     gate_orny,
     gate_oryn,
     gate_mux,
+    )
+from .lut import (
+    LookupTable,
+    make_test_vector,
+    bootstrap_lut,
+    check_noise,
     )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG

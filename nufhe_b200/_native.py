@@ -38,6 +38,7 @@ SIGNATURES = {
     'nb_external_product': [_vp, _vp, _vp, _sz, _sz],
     'nb_blind_rotate': [_vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _sz],
     'nb_bootstrap_extract': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp, _sz],
+    'nb_bootstrap_lut_extract': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _int, _vp, _sz, _vp, _vp, _sz],
     'nb_bootstrap_extract2': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32,
                               _vp, _sz, _vp, _vp, _sz],
     'nb_keyswitch': [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp, _vp, _vp, _sz],

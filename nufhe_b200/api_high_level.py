@@ -2,8 +2,8 @@
 import torch
 
 from .api_low_level import (
-    NuFHEParameters, NuFHESecretKey, NuFHECloudKey, encrypt, decrypt, empty_ciphertext)
-from .lwe import LweSampleArray
+    NuFHEParameters, NuFHESecretKey, NuFHECloudKey, encrypt, decrypt, encrypt_int, decrypt_int, empty_ciphertext)
+from .lwe import LweSampleArray, lwe_copy, lwe_add_to
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -110,6 +110,13 @@ class Context:
     def decrypt(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray):
         return decrypt(self.thread, secret_key, ciphertext)
 
+    def encrypt_int(self, secret_key: NuFHESecretKey, values, bits):
+        """Integers in [0, 2^bits), bits = 1..3, for lookup tables (VirtualMachine.lut)."""
+        return encrypt_int(self.thread, self.rng, secret_key, values, bits)
+
+    def decrypt_int(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray, bits):
+        return decrypt_int(self.thread, secret_key, ciphertext, bits)
+
     def make_virtual_machine(self, cloud_key: NuFHECloudKey, perf_params: PerformanceParameters = None):
         return VirtualMachine(self.thread, cloud_key, perf_params=perf_params)
 
@@ -162,9 +169,38 @@ class VirtualMachine:
         gate_func(self.thread, self.cloud_key, dest, *args, perf_params=self.perf_params)
         return dest
 
+    def make_lut(self, table_or_tables, bits, out='int', log2_outputs=None):
+        """A lookup table on `bits`-bit integers (nufhe_b200/lut.py: LookupTable): one table of 2^bits entries, or a
+        list of 2 or 4 of them for as many outputs of one bootstrap; out='bool' gives gate-compatible bits."""
+        from .lut import LookupTable
+        return LookupTable(self.thread, table_or_tables, bits, log2_outputs=log2_outputs, out=out)
+
+    def lut(self, table, x, y=None, shift=0, dest=None):
+        """f(x), or f(x * 2^shift + y), in one programmable bootstrap; a list of ciphertexts for a table with several
+        outputs.  Raises ValueError for a configuration without enough noise margin (lut.check_noise)."""
+        from .lut import bootstrap_lut
+        if dest is None:
+            shape = result_shape(get_shape(x), *([] if y is None else [get_shape(y)]))
+            dest = [self.empty_ciphertext(shape) for _ in range(table.outputs)]
+        elif isinstance(dest, LweSampleArray):
+            dest = [dest]
+        bootstrap_lut(self.thread, dest, self.cloud_key.bootstrap_key, self.cloud_key.keyswitch_key, table, x, y,
+                      shift, perf_params=self.perf_params)
+        return dest if table.outputs > 1 else dest[0]
+
+    def int_add(self, x, y, dest=None):
+        """x + y of two integer ciphertexts without a bootstrap (the caller keeps the sum below 2^bits)."""
+        if dest is None:
+            dest = self.empty_ciphertext(result_shape(get_shape(x), get_shape(y)))
+        gates.check_shape(dest, x, y)
+        lwe_copy(self.thread, dest, x)          # both nb_lwe_affine, with broadcasting and variances
+        lwe_add_to(self.thread, dest, y)
+        return dest
+
     def capture(self, circuit, reserve_batch=None):
         """Record `circuit()` -- any sequence of this VM's gates on device-resident ciphertexts -- into a CUDA graph;
-        returns a `GateGraph` whose `replay()` re-runs the whole circuit with one launch (nufhe_b200/graph.py)."""
+        returns a `GateGraph` whose `replay()` re-runs the whole circuit with one launch (nufhe_b200/graph.py).
+        A LUT with 2^L outputs key-switches B * 2^L samples: size `reserve_batch` for that."""
         from .graph import GateGraph
         return GateGraph(self.thread, circuit, reserve_batch=reserve_batch)
 

@@ -173,6 +173,22 @@ def decrypt(thr, key: NuFHESecretKey, ciphertext: LweSampleArray):
     return t32_to_bool(mus)
 
 
+def encrypt_int(thr, rng, key: NuFHESecretKey, values, bits):
+    """Encrypt integers in [0, 2^bits), bits = 1..3, for lookup tables (nufhe_b200/lut.py: m * 2^(31 - bits))."""
+    from .lut import encode_int
+    values = numpy.asarray(values)
+    result = empty_ciphertext(thr, key.params, values.shape)
+    mus = thr.to_device(numpy.ascontiguousarray(encode_int(values, bits)))
+    lwe_encrypt(thr, rng, result, mus, key.params.in_out_params.min_noise, key.lwe_key)
+    return result
+
+
+def decrypt_int(thr, key: NuFHESecretKey, ciphertext: LweSampleArray, bits):
+    """The integers in [0, 2^bits) that `ciphertext` holds (encrypt_int's encoding)."""
+    from .lut import decode_int
+    return decode_int(lwe_decrypt(thr, ciphertext, key.lwe_key), bits)
+
+
 def empty_ciphertext(thr, params: NuFHEParameters, shape):
     """api_low_level.py:298-302"""
     return LweSampleArray.empty(thr, params.in_out_params, tuple(shape))

@@ -87,14 +87,19 @@ struct NvtxRange {
 
 // A CTA of the fused bootstrap's work queue may wait for work that another resident CTA produces, so all the
 // sm_count x CTAS_PER_SM CTAs a launch is sized for must be co-resident: fail at context creation instead of hanging.
+// (the gate kernel and the programmable-bootstrap kernel of each shape)
 template <class Cfg> static int check_resident(nb_ctx *ctx)
 {
-    int n = 0;
-    NB_TRY(check(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, blind_rotate_kernel<Cfg>, Cfg::THREADS,
-                                                                    br_smem_bytes<Cfg>()), "cudaOccupancyMaxActiveBlocksPerMultiprocessor"));
-    if (n < Cfg::CTAS_PER_SM)
-        return fail(ctx, NB_EUNSUPPORTED, "blind_rotate_kernel: " + std::to_string(n) + " resident CTAs per SM, the work "
-                                          "queue needs " + std::to_string(Cfg::CTAS_PER_SM));
+    for (auto kernel : {blind_rotate_kernel<Cfg>, blind_rotate_kernel<Cfg, true>}) {
+        int n = 0;
+        NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<Cfg>()),
+                     "cudaFuncSetAttribute(blind_rotate)"));
+        NB_TRY(check(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, Cfg::THREADS, br_smem_bytes<Cfg>()),
+                     "cudaOccupancyMaxActiveBlocksPerMultiprocessor"));
+        if (n < Cfg::CTAS_PER_SM)
+            return fail(ctx, NB_EUNSUPPORTED, "blind_rotate_kernel: " + std::to_string(n) + " resident CTAs per SM, the work "
+                                              "queue needs " + std::to_string(Cfg::CTAS_PER_SM));
+    }
     return NB_OK;
 }
 
@@ -149,18 +154,11 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
         NB_TRY(check(ctx, cudaMalloc(&ctx->d_fft_tab, FFT_TAB_CPLX * sizeof(cplx)), "cudaMalloc"));
         NB_TRY(check(ctx, cudaMemcpy(ctx->d_fft_tab, ft.tab.data(), FFT_TAB_CPLX * sizeof(cplx), cudaMemcpyHostToDevice), "memcpy"));
     }
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrFft>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)br_smem_bytes<BrFft>()), "cudaFuncSetAttribute(blind_rotate fft)"));
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrDefault>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)br_smem_bytes<BrDefault>()), "cudaFuncSetAttribute(blind_rotate)"));
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrWide>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)br_smem_bytes<BrWide>()), "cudaFuncSetAttribute(blind_rotate wide)"));
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_kernel<BrWide2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)br_smem_bytes<BrWide2>()), "cudaFuncSetAttribute(blind_rotate wide2)"));
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)BR_PAIR_SMEM_BYTES), "cudaFuncSetAttribute(blind_rotate pair)"));
-    NB_TRY(check(ctx, cudaFuncSetAttribute(blind_rotate_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)BR_PAIR_SMEM_BYTES), "cudaFuncSetAttribute(blind_rotate pair)"));
+    // (check_resident sets the shared-memory limit of the single-CTA shapes)
+    for (auto kernel : {blind_rotate_pair_kernel<true>, blind_rotate_pair_kernel<false>, blind_rotate_pair_kernel<true, true>,
+                        blind_rotate_pair_kernel<false, true>})
+        NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BR_PAIR_SMEM_BYTES),
+                     "cudaFuncSetAttribute(blind_rotate pair)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)KS_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch)"));
     NB_TRY(check_resident<BrDefault>(ctx));
@@ -421,7 +419,8 @@ template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
         p.sched = ctx->d_sched; p.state = ctx->d_state;
         grid = slots;
     }
-    blind_rotate_kernel<Cfg><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
+    if (p.tv) blind_rotate_kernel<Cfg, true><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
+    else blind_rotate_kernel<Cfg><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
     return NB_OK;
 }
 
@@ -433,8 +432,9 @@ static int launch_br(nb_ctx *ctx, BlindRotateArgs &p)
     if (!p.plain && p.n > 0 && p.batch <= ctx->pair_max) {
         p.sched = nullptr; p.state = nullptr; p.chains = (unsigned)p.batch; p.chunks = 1; p.steps_per_chunk = p.n;
         p.sm_count = ctx->sm_count; p.stagger_cycles = 0;
-        if (ctx->pair_async) blind_rotate_pair_kernel<true><<<(unsigned)(2 * p.batch), PAIR_THREADS, BR_PAIR_SMEM_BYTES, ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
-        else blind_rotate_pair_kernel<false><<<(unsigned)(2 * p.batch), PAIR_THREADS, BR_PAIR_SMEM_BYTES, ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
+        auto kernel = p.tv ? (ctx->pair_async ? blind_rotate_pair_kernel<true, true> : blind_rotate_pair_kernel<false, true>)
+                           : (ctx->pair_async ? blind_rotate_pair_kernel<true> : blind_rotate_pair_kernel<false>);
+        kernel<<<(unsigned)(2 * p.batch), PAIR_THREADS, BR_PAIR_SMEM_BYTES, ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
         return NB_OK;
     }
     if (p.batch <= ctx->wide2_max) return launch_br_cfg<BrWide2>(ctx, p);
@@ -456,7 +456,8 @@ int nb_ctx_reserve(nb_ctx *ctx, size_t batch)
     if (!ctx) return NB_EINVAL;
     NB_ON_DEVICE(ctx);
     // everything launch_br_cfg / nb_keyswitch could ask for with up to `batch` ciphertexts (2 * batch for gate_mux's
-    // double launch is the caller's business): after this, those calls never allocate, so they can be captured
+    // double launch, B * 2^L for the key switch of nb_bootstrap_lut_extract's samples, is the caller's business): after
+    // this, those calls never allocate, so they can be captured
     NB_TRY(reserve_words(ctx, (void **)&ctx->d_sched, &ctx->sched_words, BR_SCHED_HEADER + (batch + 1) * (size_t)ctx->max_chunks, sizeof(unsigned)));
     NB_TRY(reserve_words(ctx, (void **)&ctx->d_state, &ctx->state_words, (batch + 2) * 2 * NTT_N, sizeof(int32_t)));
     NB_TRY(reserve_words(ctx, (void **)&ctx->d_cv_blocks, &ctx->cv_words, batch * KS_CV_BLOCKS, sizeof(float)));
@@ -480,6 +481,8 @@ int nb_external_product(nb_ctx *ctx, int32_t *accum, const uint64_t *bk_int, siz
 static int launch_blind_rotate(nb_ctx *ctx, BlindRotateArgs &p)
 {
     if (p.n <= 0 || p.n > LWE_N_MAX) return fail(ctx, NB_EUNSUPPORTED, "LWE dimension out of range");
+    // the LUT kernels have one job and read no explicit accumulator
+    if (p.tv && (p.job_batch || p.accum || p.bara)) return fail(ctx, NB_EINVAL, "a test vector takes a single gate-style job");
     if (p.batch == 0) return NB_OK;
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:gate_prologue+blind_rotate+extract");
@@ -510,6 +513,25 @@ int nb_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b
     BlindRotateArgs p{};
     p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
     p.c = c; p.s1 = s1; p.s2 = s2; p.mu = mu;
+    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
+    return launch_blind_rotate(ctx, p);
+}
+
+int nb_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                             const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv, size_t tv_stride,
+                             int log2_outputs, const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b,
+                             size_t batch)
+{
+    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
+    if (!ctx || !in1_a || !in1_b || !tv || !bk_int || !out_a || !out_b)
+        return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: null argument");
+    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: in2_a/in2_b must come together");
+    if (tv_stride != 0 && tv_stride != (size_t)NTT_N) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: tv_stride must be 0 or 1024");
+    if (log2_outputs < 0 || log2_outputs > 2) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: log2_outputs must be 0, 1 or 2");
+    BlindRotateArgs p{};
+    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
+    p.c = c; p.s1 = s1; p.s2 = s2;
+    p.tv = tv; p.tv_stride = tv_stride; p.log2_outputs = log2_outputs;
     p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
     return launch_blind_rotate(ctx, p);
 }

@@ -6,6 +6,7 @@
 #include <cstring>
 #include <vector>
 #include "tables.h"
+#include "lut_index.cuh"
 
 using namespace nb;
 
@@ -338,6 +339,21 @@ void emul_fft_product(const double *dig, const long long *key, double *out)
             fft_inv1(n0, w.data() + h * FFT_SPEC_CPLX, tab, x);
             for (int j = 0; j < 16; j++) out[h * NTT_N + 64 * j + n0] = x[j];
         }
+}
+
+// The programmable bootstrap's index functions (lut_index.cuh): the rounded mod-switch, the initial accumulator
+// polynomial X^(2N - barb) * tv, and the sample extracted at index j from an accumulator (2, 1024).
+int emul_modswitch_lut(i32 x, int log2_outputs) { return modswitch_lut(x, log2_outputs); }
+
+void emul_lut_head(const i32 *tv, int barb, i32 *out)
+{
+    for (int x = 0; x < NTT_N; x++) out[x] = lut_head_coef(tv, barb, x);
+}
+
+void emul_lut_tail(const i32 *acc, int j, i32 *out_a, i32 *out_b)
+{
+    for (int x = 0; x < NTT_N; x++) out_a[x] = lut_tail_a(acc, j, x);
+    *out_b = acc[NTT_N + j];
 }
 
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)

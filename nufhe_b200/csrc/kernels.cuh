@@ -8,7 +8,9 @@
 // divides along the two accumulator polynomials, one 8 KB exchange per step through distributed shared memory).
 // The stand-alone transforms reuse the same phases behind cp.async-staged, 128-bit input / output.  The key switch is a
 // TMA-fed producer / consumer pipeline.  Then the separate steps of the reference's multi-kernel bootstrap, and the
-// key-generation kernels (LWE dot product, key-switch key).
+// key-generation kernels (LWE dot product, key-switch key).  The fused bootstrap kernels also have a programmable-bootstrap
+// instantiation (template argument LUT): a test vector read from memory in the head, the phase rounded to multiples of
+// 2^L, and 2^L samples extracted in the tail (lut_index.cuh).
 //
 // Reference counterparts: nufhe/blind_rotate.mako:18-226 (fused bootstrap), tgsw_gpu.py:110-169
 // (external product), transform/computation.mako:18-143 (stand-alone transform), lwe_gpu.mako:59-118
@@ -19,6 +21,7 @@
 #include <cuda_runtime.h>
 #include "ntt_lane.cuh"
 #include "br_phases.cuh"
+#include "lut_index.cuh"
 
 namespace nb {
 
@@ -349,6 +352,13 @@ struct BlindRotateArgs {
     unsigned chains, chunks;
     int steps_per_chunk;
     int sm_count, stagger_cycles;   // single-wave launches: the second CTA of every SM starts this much later
+    // mode A with a test vector (the programmable bootstrap, the LUT instantiations of the kernels below):
+    // ciphertext c starts from X^(2N - barb) * tv[c * tv_stride ..] instead of the constant mu; barb and every bara_i
+    // are rounded to multiples of 2^log2_outputs, and samples are extracted at indices j = 0 .. 2^log2_outputs - 1
+    // into rows c * 2^log2_outputs + j of out_a / out_b (lut_index.cuh)
+    const i32 *tv;
+    size_t tv_stride;       // 0: one test vector for the batch, NTT_N: one per ciphertext
+    int log2_outputs;
 };
 constexpr int BR_SCHED_HEADER = 32;      // the ticket counter has a 128-byte line of its own
 
@@ -403,6 +413,32 @@ NB_D i32 br2_initial_acc(const BlindRotateArgs &p, size_t c, int mi, int x)
     const int q = 2 * NTT_N - modswitch_2n((i32)xb);
     if (q < NTT_N) return x < q ? (i32)(0u - (u32)p.mu) : p.mu;
     return x < q - NTT_N ? p.mu : (i32)(0u - (u32)p.mu);
+}
+
+// The same two for the programmable bootstrap (single job, no explicit accumulator): rounded mod-switch, test vector
+NB_D int lut_rotation(const BlindRotateArgs &p, size_t c, int i)
+{
+    u32 xa = (u32)p.s1 * (u32)p.in1_a[c * p.n + i] + (p.in2_a ? (u32)p.s2 * (u32)p.in2_a[c * p.n + i] : 0u);
+    return modswitch_lut((i32)xa, p.log2_outputs);
+}
+
+NB_D i32 lut_initial_acc(const BlindRotateArgs &p, size_t c, int mi, int x)
+{
+    if (mi == 0) return 0;
+    const u32 xb = (u32)p.c + (u32)p.s1 * (u32)p.in1_b[c] + (p.in2_b ? (u32)p.s2 * (u32)p.in2_b[c] : 0u);
+    return lut_head_coef(p.tv + c * p.tv_stride, modswitch_lut((i32)xb, p.log2_outputs), x);
+}
+
+template <bool LUT> NB_D int br_rotation(const BlindRotateArgs &p, size_t c, int i)
+{
+    if constexpr (LUT) return lut_rotation(p, c, i);
+    else return br2_rotation(p, c, i);
+}
+
+template <bool LUT> NB_D i32 br_initial_acc(const BlindRotateArgs &p, size_t c, int mi, int x)
+{
+    if constexpr (LUT) return lut_initial_acc(p, c, mi, x);
+    else return br2_initial_acc(p, c, mi, x);
 }
 
 // 16-byte cp.async requests for one key row, spread over `nthreads` threads (t = 0 .. nthreads - 1); one commit group
@@ -543,7 +579,8 @@ NB_D void st_release_u32(unsigned *p, unsigned v)
 // a CTA waits for is always produced by a chunk that is running on another resident CTA, so the wait cannot deadlock,
 // and a ready chain never waits behind an unready one -- with in-order tickets and per-chain progress counters, which
 // this replaces, a launch with slightly more chains than CTAs lost time to such head-of-line waits.
-template <class Cfg>
+// LUT: the programmable bootstrap (BlindRotateArgs::tv); its own instantiation, so that the gate kernels keep their code.
+template <class Cfg, bool LUT = false>
 __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g,
                                                                        const u64 *__restrict__ twd_inv_g)
 {
@@ -601,7 +638,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
             // accumulator initialisation: CT x 2 polynomials x 1024 coefficients
             for (int e = tid; e < ACC_WORDS; e += Cfg::THREADS) {
                 const int slot = e >> 11, mi = (e >> 10) & 1, x = e & (NTT_N - 1);
-                s.acc[e] = br2_initial_acc(p, ct_of(slot), mi, x);
+                s.acc[e] = br_initial_acc<LUT>(p, ct_of(slot), mi, x);
             }
         } else {
             // resume a parked chain: its queue entry was published after the accumulators (release / acquire above)
@@ -620,11 +657,11 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
             else br2_step<false, Cfg>(s, p.bk, s.rot, tid);
             __syncthreads();
         } else {
-            if (tid < Cfg::CT) s.rot[(step0 & 1) * Cfg::CT + tid] = br2_rotation(p, ct_of(tid), step0);
+            if (tid < Cfg::CT) s.rot[(step0 & 1) * Cfg::CT + tid] = br_rotation<LUT>(p, ct_of(tid), step0);
             __syncthreads();
             for (int i = step0; i < step1; i++) {
                 int next = 0;
-                if (tid < Cfg::CT && i + 1 < step1) next = br2_rotation(p, ct_of(tid), i + 1);
+                if (tid < Cfg::CT && i + 1 < step1) next = br_rotation<LUT>(p, ct_of(tid), i + 1);
                 if constexpr (Cfg::FFT)
                     br_fft_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid, p.fft_tab);
                 else
@@ -645,6 +682,18 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
                 const unsigned slot = p.chains + atomicAdd(p.sched + 1, 1u);   // appended entries follow the initial ones
                 st_release_u32(p.sched + BR_SCHED_HEADER + slot, 1u + chain + p.chains * (chunk + 1));
             }
+        } else if constexpr (LUT) {
+            // samples j = 0 .. 2^L - 1 of every ciphertext, into rows c * 2^L + j
+            const int L = p.log2_outputs;
+            for (int e = tid; e < (Cfg::CT * NTT_N) << L; e += Cfg::THREADS) {
+                const int slot = e >> (10 + L), j = (e >> 10) & ((1 << L) - 1), x = e & (NTT_N - 1);
+                const size_t c = ct0 + slot;
+                if (c >= p.batch) continue;
+                const i32 *a0 = s.acc + slot * 2 * NTT_N;
+                const size_t row = (c << L) + j;
+                p.out_a[row * NTT_N + x] = lut_tail_a(a0, j, x);
+                if (x == 0) p.out_b[row] = a0[NTT_N + j];
+            }
         } else {
             for (int e = tid; e < ACC_WORDS; e += Cfg::THREADS) {
                 const int slot = e >> 11, mi = (e >> 10) & 1, x = e & (NTT_N - 1);
@@ -662,6 +711,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
         if (!p.sched) break;
     }
 }
+
 
 // ---- pair shape: one ciphertext per cluster of two CTAs (br_phases.cuh: "pair shape") -------------------------------
 // Lowest latency for batches up to 3/8 of the SM count (capi.cu: pair_max).  No work queue (one cluster per ciphertext,
@@ -722,7 +772,8 @@ NB_D void st_async_peer(unsigned raddr, u64 x, u64 y, unsigned rbar)
 // !ASYNC: plain remote stores and one barrier.cluster per step -- ptxas implements its release / acquire with a
 // GPU-scope memory barrier and an L1 invalidation, which is why the other variant exists; kept as the reference
 // implementation (NUFHE_B200_PAIR_ASYNC=0).
-template <bool ASYNC>
+// LUT: the programmable bootstrap, as in blind_rotate_kernel.
+template <bool ASYNC, bool LUT = false>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(PAIR_THREADS, 1)
 blind_rotate_pair_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g, const u64 *__restrict__ twd_inv_g)
 {
@@ -754,11 +805,11 @@ blind_rotate_pair_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g, c
     if (p.n > 0) stage_key(0, tid, PAIR_THREADS);
     for (int i = tid; i < NTT_N; i += PAIR_THREADS) {
         twd_fwd[i] = twd_fwd_g[i]; twd_inv[i] = twd_inv_g[i];
-        acc[i] = br2_initial_acc(p, c, rank, i);
+        acc[i] = br_initial_acc<LUT>(p, c, rank, i);
     }
     const unsigned bar0 = (unsigned)__cvta_generic_to_shared(s_bar);
     if (tid == 0) {
-        rot[0] = br2_rotation(p, c, 0);
+        rot[0] = br_rotation<LUT>(p, c, 0);
         if (ASYNC) {
             mbar_init(bar0, 1); mbar_init(bar0 + 8, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -777,7 +828,7 @@ blind_rotate_pair_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g, c
         int next = 0;
         if (tid == 0) {
             if (ASYNC) mbar_expect_tx(bar0 + 8 * par, PAIR_EXCHANGE_BYTES);
-            if (i + 1 < p.n) next = br2_rotation(p, c, i + 1);
+            if (i + 1 < p.n) next = br_rotation<LUT>(p, c, i + 1);
         }
         pair_fwd1(tid, acc, w, twd_fwd, r);
         __syncthreads();
@@ -815,12 +866,23 @@ blind_rotate_pair_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g, c
         __syncthreads();
     }
 
-    for (int x = tid; x < NTT_N; x += PAIR_THREADS) {
-        if (p.accum_out) p.accum_out[(c * 2 + rank) * NTT_N + x] = acc[x];
-        if (p.extract) {
-            // sample extraction (tlwe_gpu.mako:63-82; blind_rotate.mako:213-224): a from polynomial 0, b from polynomial 1
-            if (rank == 0) p.out_a[c * NTT_N + x] = x == 0 ? acc[0] : (i32)(0u - (u32)acc[NTT_N - x]);
-            else if (x == 0) p.out_b[c] = acc[0];
+    if constexpr (LUT) {
+        // samples j = 0 .. 2^L - 1 into rows c * 2^L + j: masks from polynomial 0, bodies from polynomial 1
+        const int L = p.log2_outputs;
+        for (int e = tid; e < NTT_N << L; e += PAIR_THREADS) {
+            const int j = e >> 10, x = e & (NTT_N - 1);
+            const size_t row = (c << L) + j;
+            if (rank == 0) p.out_a[row * NTT_N + x] = lut_tail_a(acc, j, x);
+            else if (x == 0) p.out_b[row] = acc[j];
+        }
+    } else {
+        for (int x = tid; x < NTT_N; x += PAIR_THREADS) {
+            if (p.accum_out) p.accum_out[(c * 2 + rank) * NTT_N + x] = acc[x];
+            if (p.extract) {
+                // sample extraction (tlwe_gpu.mako:63-82; blind_rotate.mako:213-224): a from polynomial 0, b from polynomial 1
+                if (rank == 0) p.out_a[c * NTT_N + x] = x == 0 ? acc[0] : (i32)(0u - (u32)acc[NTT_N - x]);
+                else if (x == 0) p.out_b[c] = acc[0];
+            }
         }
     }
     // nothing is in flight towards this CTA (it has waited for every exchange) and nothing it sent is unreceived

@@ -165,6 +165,25 @@ class Engine:
                    int(mu), _ptr(bk_int), n, _ptr(out_a), _ptr(out_b), B)
         return out_a, out_b
 
+    def bootstrap_lut_extract(self, x1, x2, c, s1, s2, tv, log2_outputs, bk_int):
+        """The programmable bootstrap of x = (0,c) + s1*x1 + s2*x2 (x2 may be None) with test vector `tv`: (1024,) int32
+        for the whole batch or (B, 1024) for one per ciphertext.  Returns the 2^L extracted samples of every ciphertext,
+        a (B * 2^L, 1024) and b (B * 2^L,), sample j of ciphertext c in row c * 2^L + j (nb_bootstrap_lut_extract)."""
+        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
+        a2 = b2 = None
+        if x2 is not None:
+            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
+        tv = self._dense(tv, torch.int32)
+        B = b1.numel()
+        n = a1.shape[-1]
+        stride = 0 if tv.dim() == 1 else N
+        assert tv.shape[-1] == N and (stride == 0 or tv.numel() == B * N), (tuple(tv.shape), B)
+        rows = B << int(log2_outputs)
+        out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
+        self._call('nb_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
+                   _ptr(tv), stride, int(log2_outputs), _ptr(bk_int), n, _ptr(out_a), _ptr(out_b), B)
+        return out_a, out_b
+
     def bootstrap_extract2(self, job_a, job_b, mu, bk_int):
         """Two bootstraps in one launch.  job = (x1, x2, c, s1, s2) as for bootstrap_extract.
         Returns two extracted samples (views of one (2B, 1024) / (2B,) allocation)."""

@@ -5,7 +5,8 @@ the number that predicts its run time; use this to judge an arithmetic change be
 The default kernel is the one the benchmark's workload launches: the throughput shape with the FP64 step
 (`br_fft_step`, BrFft); its FP64 instructions (DADD / DMUL / DFMA, 2 cycles per warp-instruction on an H100 SXM SM
 sub-partition) are counted in the `fp64` column.  The NTT throughput shape is
-`--kernel blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0`.
+`--kernel blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0EEELb0E`.  Every shape has a gate instantiation (`...Lb0E`
+after the shape) and a lookup-table one (`...Lb1E`, kernels.cuh: LUT); give enough of the name to select one.
 
     python tools/sass_stats.py [--kernel blind_rotate_kernel] [--by-func] [--lib path/to/lib.so]
 
@@ -89,10 +90,11 @@ def enclosing_functions(path):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--lib', default=os.path.join(ROOT, 'nufhe_b200', 'csrc', 'libnufhe_b200.so'))
-    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb1ELb1',
-                    help='substring of the mangled kernel name (default: the 2-ciphertext shape with the FP64 step; the '
-                         'NTT one is blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0, the wide shape '
-                         'blind_rotate_kernelINS_5BrCfgILi1ELi256)')
+    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb1ELb1EEELb0E',
+                    help='substring of the mangled kernel name (default: the gate kernel of the 2-ciphertext shape with '
+                         'the FP64 step; the NTT one is blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0EEELb0E, the '
+                         'wide shape blind_rotate_kernelINS_5BrCfgILi1ELi256ELi2ELb0ELb0EEELb0E, the pair shape '
+                         'blind_rotate_pair_kernelILb1ELb0E)')
     ap.add_argument('--by-func', action='store_true', help='also split each phase by innermost ff.cuh / br_phases function')
     ap.add_argument('--opcodes', action='store_true', help='per-step histogram of instruction forms (carry-out variants split)')
     ap.add_argument('--json', action='store_true', help='print one JSON object with the per-step totals (used by bench.py)')
