@@ -1,7 +1,8 @@
 /*
  * nufhe_b200.h -- C ABI of libnufhe_b200.so, the H100 (sm_90a) engine for the gate-bootstrapping hot
- * path of nucypher/nufhe, and for programmable bootstrapping (lookup tables on small encrypted integers,
- * nb_bootstrap_lut_extract).
+ * path of nucypher/nufhe, for programmable bootstrapping (lookup tables on small encrypted integers,
+ * nb_bootstrap_lut_extract), and for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
+ * device from a seed (nb_seeded_uniform_i32).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -173,6 +174,14 @@ int nb_lwe_dot(nb_ctx *ctx, int32_t *out, const int32_t *a, const int32_t *key, 
 int nb_make_keyswitch_key(nb_ctx *ctx, int32_t *ks_a, int32_t *ks_b, float *ks_cv, const int32_t *in_key,
                           const int32_t *out_key, const int32_t *noises_a, const int32_t *noises_b, size_t in_size,
                           size_t n, int t, int log2_base, float noise_variance);
+
+/* ---- seeded masks of compressed keys and ciphertexts (DESIGN.md section 10; no reference counterpart):
+ * out[i] = word (first + i) of the ChaCha20 keystream (seed_host: 8 words, nonce), i < count, as int32.
+ * The stream is the RFC 8439 block function in the original 64-bit-counter layout (state words 12-13 the block
+ * counter, 14-15 the nonce); word w is word w % 16 of block w / 16, so `first` may start mid-block.  seed_host is a
+ * HOST pointer.  NB_EINVAL for a NULL seed or output and for first + count past 2^64. */
+int nb_seeded_uniform_i32(nb_ctx *ctx, const uint32_t *seed_host, uint64_t nonce, uint64_t first, int32_t *out,
+                          size_t count);
 
 #ifdef __cplusplus
 }

@@ -41,6 +41,10 @@ from .lut import (
     bootstrap_lut,
     check_noise,
     )
+from .compressed import (
+    CompressedLweSampleArray,
+    CompressedCloudKey,
+    )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

@@ -52,6 +52,7 @@ SIGNATURES = {
     'nb_tgsw_mac': [_vp, _vp, _vp, _vp, _sz, _int, _int],
     'nb_lwe_dot': [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _sz],
     'nb_make_keyswitch_key': [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _int, _int, ctypes.c_float],
+    'nb_seeded_uniform_i32': [_vp, _vp, ctypes.c_uint64, ctypes.c_uint64, _vp, _sz],
 }
 _RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p, 'nb_build_info': ctypes.c_char_p}
 

@@ -4,6 +4,7 @@ import torch
 from .api_low_level import (
     NuFHEParameters, NuFHESecretKey, NuFHECloudKey, encrypt, decrypt, encrypt_int, decrypt_int, empty_ciphertext)
 from .lwe import LweSampleArray, lwe_copy, lwe_add_to
+from .compressed import CompressedLweSampleArray, CompressedCloudKey
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -96,7 +97,11 @@ class Context:
     def make_secret_key(self, **params):
         return NuFHESecretKey.from_rng(self.thread, NuFHEParameters(**params), self.rng)
 
-    def make_cloud_key(self, secret_key: NuFHESecretKey):
+    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False):
+        """compressed=True returns a CompressedCloudKey (about 12 times smaller to store or send); its `decompress()`
+        gives the NuFHECloudKey that make_virtual_machine takes."""
+        if compressed:
+            return CompressedCloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
         return NuFHECloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
 
     def make_key_pair(self, **params):
@@ -104,15 +109,16 @@ class Context:
         cloud_key = self.make_cloud_key(secret_key)
         return secret_key, cloud_key
 
-    def encrypt(self, secret_key: NuFHESecretKey, message):
-        return encrypt(self.thread, self.rng, secret_key, message)
+    def encrypt(self, secret_key: NuFHESecretKey, message, compressed=False):
+        """compressed=True returns a CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute)."""
+        return encrypt(self.thread, self.rng, secret_key, message, compressed=compressed)
 
     def decrypt(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray):
         return decrypt(self.thread, secret_key, ciphertext)
 
-    def encrypt_int(self, secret_key: NuFHESecretKey, values, bits):
+    def encrypt_int(self, secret_key: NuFHESecretKey, values, bits, compressed=False):
         """Integers in [0, 2^bits), bits = 1..3, for lookup tables (VirtualMachine.lut)."""
-        return encrypt_int(self.thread, self.rng, secret_key, values, bits)
+        return encrypt_int(self.thread, self.rng, secret_key, values, bits, compressed=compressed)
 
     def decrypt_int(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray, bits):
         return decrypt_int(self.thread, secret_key, ciphertext, bits)
@@ -124,6 +130,16 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return LweSampleArray.loads(file_or_bytestring, self.thread)
         return LweSampleArray.load(file_or_bytestring, self.thread)
+
+    def load_compressed_ciphertext(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return CompressedLweSampleArray.loads(file_or_bytestring, self.thread)
+        return CompressedLweSampleArray.load(file_or_bytestring, self.thread)
+
+    def load_compressed_cloud_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return CompressedCloudKey.loads(file_or_bytestring, self.thread)
+        return CompressedCloudKey.load(file_or_bytestring, self.thread)
 
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):

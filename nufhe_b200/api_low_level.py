@@ -157,14 +157,23 @@ def t32_to_bool(mu):
     return numpy.asarray(mu) > 0
 
 
-def encrypt(thr, rng, key: NuFHESecretKey, message):
-    """api_low_level.py:266-281"""
-    message = numpy.asarray(message)
-    result = empty_ciphertext(thr, key.params, message.shape)
-    mus = thr.to_device(numpy.ascontiguousarray(bool_to_t32(message)))
+def _encrypt_mus(thr, rng, key: NuFHESecretKey, shape, mus, compressed):
     noise = key.params.in_out_params.min_noise
+    if compressed:
+        from .compressed import CompressedLweSampleArray
+        return CompressedLweSampleArray.encrypt(thr, rng, key.params.in_out_params, mus.reshape(shape), noise,
+                                                key.lwe_key)
+    result = empty_ciphertext(thr, key.params, shape)
     lwe_encrypt(thr, rng, result, mus, noise, key.lwe_key)
     return result
+
+
+def encrypt(thr, rng, key: NuFHESecretKey, message, compressed=False):
+    """api_low_level.py:266-281.  compressed=True returns a CompressedLweSampleArray: the mask is regenerated from a
+    seed (nufhe_b200/compressed.py), so only the bodies and the seed are stored or sent."""
+    message = numpy.asarray(message)
+    mus = thr.to_device(numpy.ascontiguousarray(bool_to_t32(message)))
+    return _encrypt_mus(thr, rng, key, message.shape, mus, compressed)
 
 
 def decrypt(thr, key: NuFHESecretKey, ciphertext: LweSampleArray):
@@ -173,14 +182,13 @@ def decrypt(thr, key: NuFHESecretKey, ciphertext: LweSampleArray):
     return t32_to_bool(mus)
 
 
-def encrypt_int(thr, rng, key: NuFHESecretKey, values, bits):
-    """Encrypt integers in [0, 2^bits), bits = 1..3, for lookup tables (nufhe_b200/lut.py: m * 2^(31 - bits))."""
+def encrypt_int(thr, rng, key: NuFHESecretKey, values, bits, compressed=False):
+    """Encrypt integers in [0, 2^bits), bits = 1..3, for lookup tables (nufhe_b200/lut.py: m * 2^(31 - bits)).
+    compressed=True returns a CompressedLweSampleArray, as for encrypt()."""
     from .lut import encode_int
     values = numpy.asarray(values)
-    result = empty_ciphertext(thr, key.params, values.shape)
     mus = thr.to_device(numpy.ascontiguousarray(encode_int(values, bits)))
-    lwe_encrypt(thr, rng, result, mus, key.params.in_out_params.min_noise, key.lwe_key)
-    return result
+    return _encrypt_mus(thr, rng, key, values.shape, mus, compressed)
 
 
 def decrypt_int(thr, key: NuFHESecretKey, ciphertext: LweSampleArray, bits):

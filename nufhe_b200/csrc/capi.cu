@@ -751,4 +751,23 @@ int nb_make_keyswitch_key(nb_ctx *ctx, int32_t *ks_a, int32_t *ks_b, float *ks_c
     return launch_check(ctx, "make_keyswitch_key_kernel");
 }
 
+int nb_seeded_uniform_i32(nb_ctx *ctx, const uint32_t *seed_host, uint64_t nonce, uint64_t first, int32_t *out,
+                          size_t count)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!seed_host || !out) return fail(ctx, NB_EINVAL, "nb_seeded_uniform_i32: null argument");
+    if (count == 0) return NB_OK;
+    if ((uint64_t)count - 1 > UINT64_MAX - first)
+        return fail(ctx, NB_EINVAL, "nb_seeded_uniform_i32: first + count is past the end of the 2^64-word stream");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:seeded_uniform");
+    ChachaSeed seed;
+    memcpy(seed.w, seed_host, sizeof(seed.w));
+    const u64 blocks = ((first + ((u64)count - 1)) >> 4) - (first >> 4) + 1;
+    const u64 ctas = (blocks + SEEDED_THREADS - 1) / SEEDED_THREADS, cap = (u64)ctx->sm_count * 8;
+    seeded_uniform_kernel<<<(int)(ctas < cap ? ctas : cap), SEEDED_THREADS, 0, ctx->stream>>>(out, seed, nonce, first,
+                                                                                              (u64)count);
+    return launch_check(ctx, "seeded_uniform_kernel");
+}
+
 }  // extern "C"

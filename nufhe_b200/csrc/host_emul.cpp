@@ -7,6 +7,7 @@
 #include <vector>
 #include "tables.h"
 #include "lut_index.cuh"
+#include "chacha.cuh"
 
 using namespace nb;
 
@@ -355,6 +356,9 @@ void emul_lut_tail(const i32 *acc, int j, i32 *out_a, i32 *out_b)
     for (int x = 0; x < NTT_N; x++) out_a[x] = lut_tail_a(acc, j, x);
     *out_b = acc[NTT_N + j];
 }
+
+// The ChaCha20 block function of the seeded masks (chacha.cuh): out[16] = block `counter` of the stream (seed[8], nonce)
+void emul_chacha_block(const u32 *seed, u64 counter, u64 nonce, u32 *out) { chacha20_block(seed, counter, nonce, out); }
 
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)
 { for (size_t i = 0; i < n; i++) out[i] = ff_shl_var(in[i], s[i]); }

@@ -22,6 +22,7 @@
 #include "ntt_lane.cuh"
 #include "br_phases.cuh"
 #include "lut_index.cuh"
+#include "chacha.cuh"
 
 namespace nb {
 
@@ -1364,6 +1365,41 @@ __global__ void make_keyswitch_key_kernel(i32 *__restrict__ ks_a, i32 *__restric
             ks_b[row] = (i32)(message + (u32)noises_b[nrow] + acc);
             ks_cv[row] = noise_var;
         }
+    }
+}
+
+// ---- seeded masks (DESIGN.md section 10): out[i] = word (first + i) of the ChaCha20 stream (seed, nonce), i < count.
+// Each lane computes one 64-byte block; a warp's 32 blocks go through shared memory so that every store instruction of
+// the warp writes 32 consecutive words (the kernel is meant to be bound by these writes).  The row stride of 17 words
+// keeps the lane-per-block writes into shared memory free of bank conflicts.
+struct ChachaSeed { u32 w[8]; };
+
+constexpr int SEEDED_THREADS = 256;
+
+__global__ void __launch_bounds__(SEEDED_THREADS) seeded_uniform_kernel(i32 *__restrict__ out, ChachaSeed seed,
+                                                                        u64 nonce, u64 first, u64 count)
+{
+    __shared__ u32 stage[SEEDED_THREADS / 32][32 * 17];
+    const int lane = threadIdx.x & 31;
+    u32 *st = stage[threadIdx.x >> 5];
+    const u64 blk0 = first >> 4, head = first & 15;
+    const u64 blocks = ((first + (count - 1)) >> 4) - blk0 + 1;        // the caller rules out count = 0 and wrapping
+    const u64 warps = ((u64)gridDim.x * blockDim.x) >> 5;
+    for (u64 wb = (((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 32; wb < blocks; wb += warps * 32) {
+        if (wb + lane < blocks) {
+            u32 x[16];
+            chacha20_block(seed.w, blk0 + wb + lane, nonce, x);
+#pragma unroll
+            for (int j = 0; j < 16; j++) st[lane * 17 + j] = x[j];
+        }
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const int idx = j * 32 + lane;                              // word of the warp's 512-word window
+            const u64 w = wb * 16 + idx;                                // stream word - 16 * blk0
+            if (w >= head && w - head < count) out[w - head] = (i32)st[(idx >> 4) * 17 + (idx & 15)];
+        }
+        __syncwarp();
     }
 }
 

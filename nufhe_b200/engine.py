@@ -312,6 +312,19 @@ class Engine:
                    _ptr(self._dense(noises_b, torch.int32)), in_size, n, t, int(log2_base),
                    ctypes.c_float(float(noise_variance)))
 
+    def seeded_uniform(self, seed, nonce, shape, first=0):
+        """Uniform Torus32 values of `shape` (int32): words [first, first + prod(shape)) of the ChaCha20 stream
+        (seed, nonce) in C order (nb_seeded_uniform_i32).  `seed` holds 8 32-bit words (any integer dtype)."""
+        seed = numpy.ascontiguousarray(numpy.asarray(seed).astype(numpy.int64).astype(numpy.uint32).reshape(-1))
+        if seed.size != 8:
+            raise ValueError('a seed is 8 32-bit words, got %d' % seed.size)
+        out = self.empty(shape, torch.int32)
+        if out.numel() == 0:
+            return out
+        self._call('nb_seeded_uniform_i32', seed.ctypes.data_as(ctypes.c_void_p), ctypes.c_uint64(int(nonce)),
+                   ctypes.c_uint64(int(first)), _ptr(out), out.numel())
+        return out
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()

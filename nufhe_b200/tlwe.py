@@ -108,6 +108,13 @@ def tlwe_encrypt_zero(thr, rng, result: TLweSampleArray, noise: float, key: TLwe
     k = key.params.mask_size
     noises1 = rand_uniform_torus32(thr, rng, result.shape + (k, N))
     noises2 = rand_gaussian_torus32(thr, rng, 0, noise, result.shape + (N,))
+    tlwe_encrypt_zero_with_masks(thr, result, noises1, noises2, noise, key)
+
+
+def tlwe_encrypt_zero_with_masks(thr, result: TLweSampleArray, noises1, noises2, noise: float, key: TLweKey):
+    """tlwe_encrypt_zero with given masks `noises1` (shape + (k, N)) and body noises `noises2` (shape + (N,)); draws
+    nothing.  Compressed bootstrap keys pass masks expanded from a seed (nufhe_b200/compressed.py)."""
+    k = key.params.mask_size
     tr_key = thr.ntt_forward_i32(key.key.coeffs)                     # (k, N)
     tr_noise = thr.ntt_forward_i32(noises1)                          # shape + (k, N)
     prod = thr.ff_op(_native.FF_MUL, tr_noise, tr_key)               # key broadcast with period k*N
