@@ -1,8 +1,8 @@
 /*
  * nufhe_b200.h -- C ABI of libnufhe_b200.so, the H100 (sm_90a) engine for the gate-bootstrapping hot
  * path of nucypher/nufhe, for programmable bootstrapping (lookup tables on small encrypted integers,
- * nb_bootstrap_lut_extract), and for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
- * device from a seed (nb_seeded_uniform_i32).
+ * nb_bootstrap_lut_extract), for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
+ * device from a seed (nb_seeded_uniform_i32), and for public-key encryption (nb_pk_prepare, nb_pk_encrypt).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -182,6 +182,21 @@ int nb_make_keyswitch_key(nb_ctx *ctx, int32_t *ks_a, int32_t *ks_b, float *ks_c
  * HOST pointer.  NB_EINVAL for a NULL seed or output and for first + count past 2^64. */
 int nb_seeded_uniform_i32(nb_ctx *ctx, const uint32_t *seed_host, uint64_t nonce, uint64_t first, int32_t *out,
                           size_t count);
+
+/* ---- public-key encryption (DESIGN.md section 11; no reference counterpart).  A public key is m LWE encryptions of 0,
+ * a (m, n) int32 and b (m,) int32; encrypting B messages is (a, b) = R [A | b_pk] + (0, mu) with R binary (B, m).
+ * nb_pk_prepare lays W = [A | b | 1] (m x (n+2), columns padded to a multiple of 8) into 4 byte planes, plane p
+ * column-major: byte p of W[k][col] at ((p * npad + col) * m + k); `planes` holds nb_pk_planes_bytes(m, n) bytes
+ * (0 for an n the library rejects).
+ * nb_pk_encrypt: r_bits (B, m/32) uint32, bit i of row c = bit i % 32 of word (c, i / 32);
+ *     out_a[c] = sum_i r_ci A_i,  out_b[c] = mus[c] + sum_i r_ci b_i  (mod 2^32),
+ *     out_cv[c] = float(popcount(r_c)) * row_variance,
+ * one exact u8 x u8 -> s32 tensor-core GEMM (mma.sync m16n8k32).  NB_EINVAL for a NULL pointer, for m not a positive
+ * multiple of 32 or with m * 255 >= 2^31 (the sums would not be exact), and for n = 0; batch = 0 is a no-op. */
+size_t nb_pk_planes_bytes(size_t m, size_t n);
+int nb_pk_prepare(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t m, size_t n, uint8_t *planes);
+int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, size_t m, size_t n, const int32_t *mus,
+                  float row_variance, int32_t *out_a, int32_t *out_b, float *out_cv, size_t batch);
 
 #ifdef __cplusplus
 }

@@ -45,6 +45,11 @@ from .compressed import (
     CompressedLweSampleArray,
     CompressedCloudKey,
     )
+from .public_key import (
+    NuFHEPublicKey,
+    public_key_size,
+    public_encrypt,
+    )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

@@ -53,8 +53,11 @@ SIGNATURES = {
     'nb_lwe_dot': [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _sz, _sz],
     'nb_make_keyswitch_key': [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _int, _int, ctypes.c_float],
     'nb_seeded_uniform_i32': [_vp, _vp, ctypes.c_uint64, ctypes.c_uint64, _vp, _sz],
+    'nb_pk_planes_bytes': [_sz, _sz],
+    'nb_pk_prepare': [_vp, _vp, _vp, _sz, _sz, _vp],
+    'nb_pk_encrypt': [_vp, _vp, _vp, _sz, _sz, _vp, ctypes.c_float, _vp, _vp, _vp, _sz],
 }
-_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p, 'nb_build_info': ctypes.c_char_p}
+_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p, 'nb_build_info': ctypes.c_char_p}
 
 _lib = None
 

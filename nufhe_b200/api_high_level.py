@@ -5,6 +5,7 @@ from .api_low_level import (
     NuFHEParameters, NuFHESecretKey, NuFHECloudKey, encrypt, decrypt, encrypt_int, decrypt_int, empty_ciphertext)
 from .lwe import LweSampleArray, lwe_copy, lwe_add_to
 from .compressed import CompressedLweSampleArray, CompressedCloudKey
+from .public_key import NuFHEPublicKey
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -104,21 +105,26 @@ class Context:
             return CompressedCloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
         return NuFHECloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
 
+    def make_public_key(self, secret_key: NuFHESecretKey):
+        """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
+        return NuFHEPublicKey.from_secret_key(self.thread, self.rng, secret_key)
+
     def make_key_pair(self, **params):
         secret_key = self.make_secret_key(**params)
         cloud_key = self.make_cloud_key(secret_key)
         return secret_key, cloud_key
 
-    def encrypt(self, secret_key: NuFHESecretKey, message, compressed=False):
-        """compressed=True returns a CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute)."""
-        return encrypt(self.thread, self.rng, secret_key, message, compressed=compressed)
+    def encrypt(self, key, message, compressed=False):
+        """`key` is a NuFHESecretKey or a NuFHEPublicKey.  compressed=True (secret key only) returns a
+        CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute)."""
+        return encrypt(self.thread, self.rng, key, message, compressed=compressed)
 
     def decrypt(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray):
         return decrypt(self.thread, secret_key, ciphertext)
 
-    def encrypt_int(self, secret_key: NuFHESecretKey, values, bits, compressed=False):
-        """Integers in [0, 2^bits), bits = 1..3, for lookup tables (VirtualMachine.lut)."""
-        return encrypt_int(self.thread, self.rng, secret_key, values, bits, compressed=compressed)
+    def encrypt_int(self, key, values, bits, compressed=False):
+        """Integers in [0, 2^bits), bits = 1..3, for lookup tables (VirtualMachine.lut); `key` as for encrypt()."""
+        return encrypt_int(self.thread, self.rng, key, values, bits, compressed=compressed)
 
     def decrypt_int(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray, bits):
         return decrypt_int(self.thread, secret_key, ciphertext, bits)
@@ -140,6 +146,11 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return CompressedCloudKey.loads(file_or_bytestring, self.thread)
         return CompressedCloudKey.load(file_or_bytestring, self.thread)
+
+    def load_public_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHEPublicKey.loads(file_or_bytestring, self.thread)
+        return NuFHEPublicKey.load(file_or_bytestring, self.thread)
 
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):

@@ -157,7 +157,13 @@ def t32_to_bool(mu):
     return numpy.asarray(mu) > 0
 
 
-def _encrypt_mus(thr, rng, key: NuFHESecretKey, shape, mus, compressed):
+def _encrypt_mus(thr, rng, key, shape, mus, compressed):
+    from .public_key import NuFHEPublicKey, public_encrypt
+    if isinstance(key, NuFHEPublicKey):
+        if compressed:
+            raise ValueError("a public-key encryption cannot be compressed: its mask depends on the secret random "
+                             "matrix R, not on a seed that can be published")
+        return public_encrypt(thr, rng, key, mus.reshape(shape))
     noise = key.params.in_out_params.min_noise
     if compressed:
         from .compressed import CompressedLweSampleArray
@@ -168,9 +174,10 @@ def _encrypt_mus(thr, rng, key: NuFHESecretKey, shape, mus, compressed):
     return result
 
 
-def encrypt(thr, rng, key: NuFHESecretKey, message, compressed=False):
+def encrypt(thr, rng, key, message, compressed=False):
     """api_low_level.py:266-281.  compressed=True returns a CompressedLweSampleArray: the mask is regenerated from a
-    seed (nufhe_b200/compressed.py), so only the bodies and the seed are stored or sent."""
+    seed (nufhe_b200/compressed.py), so only the bodies and the seed are stored or sent.  `key` is a NuFHESecretKey or
+    a NuFHEPublicKey (nufhe_b200/public_key.py; not with compressed=True)."""
     message = numpy.asarray(message)
     mus = thr.to_device(numpy.ascontiguousarray(bool_to_t32(message)))
     return _encrypt_mus(thr, rng, key, message.shape, mus, compressed)
@@ -182,9 +189,9 @@ def decrypt(thr, key: NuFHESecretKey, ciphertext: LweSampleArray):
     return t32_to_bool(mus)
 
 
-def encrypt_int(thr, rng, key: NuFHESecretKey, values, bits, compressed=False):
+def encrypt_int(thr, rng, key, values, bits, compressed=False):
     """Encrypt integers in [0, 2^bits), bits = 1..3, for lookup tables (nufhe_b200/lut.py: m * 2^(31 - bits)).
-    compressed=True returns a CompressedLweSampleArray, as for encrypt()."""
+    compressed=True returns a CompressedLweSampleArray, as for encrypt(); `key` may be a NuFHEPublicKey."""
     from .lut import encode_int
     values = numpy.asarray(values)
     mus = thr.to_device(numpy.ascontiguousarray(encode_int(values, bits)))

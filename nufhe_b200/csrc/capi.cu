@@ -770,4 +770,53 @@ int nb_seeded_uniform_i32(nb_ctx *ctx, const uint32_t *seed_host, uint64_t nonce
     return launch_check(ctx, "seeded_uniform_kernel");
 }
 
+
+size_t nb_pk_planes_bytes(size_t m, size_t n)
+{
+    if (n == 0 || n > (1u << 30)) return 0;
+    return 4 * m * (size_t)pk_cols_padded((u32)n);
+}
+
+// m rows of [A | b] for an n-word LWE key: m a multiple of 32 (whole k-steps) and every plane sum, at most m * 255,
+// below 2^31 so that the s32 accumulators are exact
+static int pk_check_shape(nb_ctx *ctx, size_t m, size_t n, const char *what)
+{
+    if (m == 0 || m % 32 != 0 || (uint64_t)m * 255 >= (1ull << 31))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": m must be a positive multiple of 32 with m * 255 < 2^31");
+    if (n == 0 || n > (1u << 30)) return fail(ctx, NB_EINVAL, std::string(what) + ": bad LWE dimension");
+    return NB_OK;
+}
+
+int nb_pk_prepare(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t m, size_t n, uint8_t *planes)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!a || !b || !planes) return fail(ctx, NB_EINVAL, "nb_pk_prepare: null argument");
+    NB_TRY(pk_check_shape(ctx, m, n, "nb_pk_prepare"));
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:pk_prepare");
+    const size_t quads = (size_t)pk_cols_padded((u32)n) * (m / 4);
+    size_t blocks = (quads + 255) / 256, cap = (size_t)ctx->sm_count * 16;
+    pk_prepare_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(a, b, (u32)m, (u32)n, planes);
+    return launch_check(ctx, "pk_prepare_kernel");
+}
+
+int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, size_t m, size_t n, const int32_t *mus,
+                  float row_variance, int32_t *out_a, int32_t *out_b, float *out_cv, size_t batch)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!r_bits || !planes || !mus || !out_a || !out_b || !out_cv)
+        return fail(ctx, NB_EINVAL, "nb_pk_encrypt: null argument");
+    NB_TRY(pk_check_shape(ctx, m, n, "nb_pk_encrypt"));
+    if (batch == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:pk_encrypt");
+    const size_t rows_per_cta = (size_t)PK_WARPS * PK_MTILES * 16;
+    const size_t ctas = (batch + rows_per_cta - 1) / rows_per_cta;
+    if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_pk_encrypt: batch too large");
+    const dim3 grid((unsigned)ctas, pk_cols_padded((u32)n) / 8);
+    pk_encrypt_kernel<<<grid, PK_WARPS * 32, 0, ctx->stream>>>(r_bits, planes, (u32)m, (u32)n, mus, row_variance,
+                                                               out_a, out_b, out_cv, (u64)batch);
+    return launch_check(ctx, "pk_encrypt_kernel");
+}
+
 }  // extern "C"

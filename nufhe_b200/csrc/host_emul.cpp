@@ -8,6 +8,7 @@
 #include "tables.h"
 #include "lut_index.cuh"
 #include "chacha.cuh"
+#include "pk_layout.cuh"
 
 using namespace nb;
 
@@ -359,6 +360,94 @@ void emul_lut_tail(const i32 *acc, int j, i32 *out_a, i32 *out_b)
 
 // The ChaCha20 block function of the seeded masks (chacha.cuh): out[16] = block `counter` of the stream (seed[8], nonce)
 void emul_chacha_block(const u32 *seed, u64 counter, u64 nonce, u32 *out) { chacha20_block(seed, counter, nonce, out); }
+
+// Public-key encryption (pk_layout.cuh): pk_prepare_kernel's planes, then pk_encrypt_kernel's tile loop with a scalar
+// model of mma.sync.m16n8k32.row.col.s32.u8.u8.s32.  The model places each register byte by the fragment layout of the
+// PTX ISA (not by pk_layout.cuh), so a lane that feeds the wrong bits or plane bytes gives a wrong result here.
+static void mma_m16n8k32_u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4])
+{
+    u32 A[16][32], B[32][8];
+    for (int l = 0; l < 32; l++) {
+        const int g = l >> 2, t = l & 3;
+        for (int j = 0; j < 16; j++) {          // a_j: register j / 4, byte j % 4
+            const int row = g + ((j < 4 || (j >= 8 && j < 12)) ? 0 : 8), k = 4 * t + (j & 3) + (j >= 8 ? 16 : 0);
+            A[row][k] = (a[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
+        }
+        for (int j = 0; j < 8; j++) {           // b_j: register j / 4, byte j % 4
+            const int k = 4 * t + (j & 3) + (j >= 4 ? 16 : 0);
+            B[k][g] = (b[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
+        }
+    }
+    i32 D[16][8] = {};
+    for (int r = 0; r < 16; r++) {
+        bool any = false;
+        for (int k = 0; k < 32; k++) any |= A[r][k] != 0;
+        if (!any) continue;                     // (a zero row adds nothing)
+        for (int c2 = 0; c2 < 8; c2++) {
+            i32 s = 0;
+            for (int k = 0; k < 32; k++) s += (i32)(A[r][k] * B[k][c2]);
+            D[r][c2] = s;
+        }
+    }
+    for (int l = 0; l < 32; l++) {
+        const int g = l >> 2, t = l & 3;
+        for (int i = 0; i < 4; i++) c[l][i] += D[g + (i >= 2 ? 8 : 0)][2 * t + (i & 1)];
+    }
+}
+
+void emul_pk_encrypt(const u32 *r_bits, const i32 *a, const i32 *b, size_t m, size_t n, const i32 *mus,
+                     float row_variance, i32 *out_a, i32 *out_b, float *out_cv, size_t batch)
+{
+    const u32 npad = pk_cols_padded((u32)n), words = (u32)(m >> 5);
+    std::vector<uint8_t> planes((size_t)4 * npad * m);
+    for (u32 col = 0; col < npad; col++)
+        for (u32 k = 0; k < m; k++) {
+            const u32 w = pk_source_word(a, b, (u32)n, k, col);
+            for (int p = 0; p < 4; p++) planes[pk_plane_offset(p, col, k, (u32)m, npad)] = (uint8_t)(w >> (8 * p));
+        }
+    auto load32 = [&](u64 off) { u32 v; memcpy(&v, planes.data() + off, 4); return v; };
+    const u64 plane_stride = pk_plane_offset(1, 0, 0, (u32)m, npad);
+    for (u64 row0 = 0; row0 < batch; row0 += 16 * PK_MTILES)      // one warp
+        for (u32 col0 = 0; col0 < npad; col0 += 8) {
+            static i32 acc[4][PK_MTILES][32][4];
+            memset(acc, 0, sizeof(acc));
+            for (u32 ks = 0; ks < words; ks++) {
+                u32 bf[4][32][2], af[PK_MTILES][32][4];
+                for (int l = 0; l < 32; l++) {
+                    const int g = l >> 2, t = l & 3;
+                    const u64 bcol = pk_plane_offset(0, col0 + g, 0, (u32)m, npad);
+                    for (int p = 0; p < 4; p++)
+                        for (int h = 0; h < 2; h++) bf[p][l][h] = load32(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h));
+                    for (int mt = 0; mt < PK_MTILES; mt++) {
+                        u32 w[2];
+                        for (int hr = 0; hr < 2; hr++) {
+                            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
+                            w[hr] = r < batch ? r_bits[r * words + ks] : 0u;
+                        }
+                        af[mt][l][0] = pk_a_frag(w[0], t, 0);
+                        af[mt][l][1] = pk_a_frag(w[1], t, 0);
+                        af[mt][l][2] = pk_a_frag(w[0], t, 1);
+                        af[mt][l][3] = pk_a_frag(w[1], t, 1);
+                    }
+                }
+                for (int mt = 0; mt < PK_MTILES; mt++)
+                    for (int p = 0; p < 4; p++) mma_m16n8k32_u8(af[mt], bf[p], acc[p][mt]);
+            }
+            for (int l = 0; l < 32; l++) {
+                const int g = l >> 2, t = l & 3;
+                for (int mt = 0; mt < PK_MTILES; mt++)
+                    for (int i = 0; i < 4; i++) {
+                        const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
+                        const u32 col = col0 + pk_acc_col(t, i);
+                        if (row >= batch) continue;
+                        const u32 v = pk_combine(acc[0][mt][l][i], acc[1][mt][l][i], acc[2][mt][l][i], acc[3][mt][l][i]);
+                        if (col < n) out_a[row * n + col] = (i32)v;
+                        else if (col == n) out_b[row] = (i32)(v + (u32)mus[row]);
+                        else if (col == n + 1) out_cv[row] = (float)acc[0][mt][l][i] * row_variance;
+                    }
+            }
+        }
+}
 
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)
 { for (size_t i = 0; i < n; i++) out[i] = ff_shl_var(in[i], s[i]); }

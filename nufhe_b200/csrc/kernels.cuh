@@ -23,6 +23,7 @@
 #include "br_phases.cuh"
 #include "lut_index.cuh"
 #include "chacha.cuh"
+#include "pk_layout.cuh"
 
 namespace nb {
 
@@ -1401,6 +1402,99 @@ __global__ void __launch_bounds__(SEEDED_THREADS) seeded_uniform_kernel(i32 *__r
         }
         __syncwarp();
     }
+}
+
+// ---- public-key encryption (DESIGN.md section 11; index arithmetic in pk_layout.cuh).
+// nb_pk_prepare: the 4 byte planes of W = [A | b | 1] (m x n), one thread per (column, 4 consecutive k): it reads W
+// once and writes one 32-bit word to each plane.
+__global__ void pk_prepare_kernel(const i32 *__restrict__ a, const i32 *__restrict__ b, u32 m, u32 n,
+                                  uint8_t *__restrict__ planes)
+{
+    const u32 npad = pk_cols_padded(n), quads = m >> 2;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < (u64)npad * quads; i += (u64)gridDim.x * blockDim.x) {
+        const u32 col = (u32)(i / quads), k = (u32)(i % quads) * 4;
+        u32 w[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) w[j] = pk_source_word(a, b, n, k + j, col);
+#pragma unroll
+        for (int p = 0; p < 4; p++) {
+            u32 v = 0;
+#pragma unroll
+            for (int j = 0; j < 4; j++) v |= ((w[j] >> (8 * p)) & 0xFFu) << (8 * j);
+            *(u32 *)(planes + pk_plane_offset(p, col, k, m, npad)) = v;
+        }
+    }
+}
+
+__device__ __forceinline__ void pk_mma(i32 *c, const u32 *a, const u32 *b)
+{
+    asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// nb_pk_encrypt: one GEMM R (batch x m, packed bits) x W (m x npad, 4 byte planes).  CTA = PK_WARPS warps on the
+// same 8 columns (blockIdx.y), each warp PK_MTILES m16 tiles of rows.  Per k-step of 32 a lane loads the R word of its
+// 2 * PK_MTILES rows and 2 words of each plane, and issues the 4 planes' MMAs with the same A fragment, so the four
+// sums of one output word sit in one thread.  The planes (33 MB for the default key) stay in L2 across CTAs.
+__global__ void __launch_bounds__(PK_WARPS * 32) pk_encrypt_kernel(
+    const u32 *__restrict__ r_bits, const uint8_t *__restrict__ planes, u32 m, u32 n, const i32 *__restrict__ mus,
+    float row_variance, i32 *__restrict__ out_a, i32 *__restrict__ out_b, float *__restrict__ out_cv, u64 batch)
+{
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const u64 row0 = ((u64)blockIdx.x * PK_WARPS + (threadIdx.x >> 5)) * (16 * PK_MTILES);
+    if (row0 >= batch) return;
+    const u32 npad = pk_cols_padded(n), words = m >> 5, col0 = blockIdx.y * 8;
+    const uint8_t *bcol = planes + pk_plane_offset(0, col0 + g, 0, m, npad);
+    const u64 plane_stride = pk_plane_offset(1, 0, 0, m, npad);
+    const u32 *rrow[PK_MTILES][2];
+    bool rok[PK_MTILES][2];
+#pragma unroll
+    for (int mt = 0; mt < PK_MTILES; mt++)
+#pragma unroll
+        for (int hr = 0; hr < 2; hr++) {
+            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
+            rok[mt][hr] = r < batch;
+            rrow[mt][hr] = r_bits + (rok[mt][hr] ? r : 0) * words;
+        }
+    i32 acc[4][PK_MTILES][4];
+#pragma unroll
+    for (int p = 0; p < 4; p++)
+#pragma unroll
+        for (int mt = 0; mt < PK_MTILES; mt++)
+#pragma unroll
+            for (int i = 0; i < 4; i++) acc[p][mt][i] = 0;
+
+#pragma unroll 2
+    for (u32 ks = 0; ks < words; ks++) {
+        u32 bf[4][2];
+#pragma unroll
+        for (int p = 0; p < 4; p++)
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+                bf[p][h] = __ldg((const u32 *)(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h)));
+#pragma unroll
+        for (int mt = 0; mt < PK_MTILES; mt++) {
+            const u32 w0 = rok[mt][0] ? __ldg(rrow[mt][0] + ks) : 0u;     // row g of the tile
+            const u32 w1 = rok[mt][1] ? __ldg(rrow[mt][1] + ks) : 0u;     // row g + 8
+            const u32 af[4] = {pk_a_frag(w0, t, 0), pk_a_frag(w1, t, 0), pk_a_frag(w0, t, 1), pk_a_frag(w1, t, 1)};
+#pragma unroll
+            for (int p = 0; p < 4; p++) pk_mma(acc[p][mt], af, bf[p]);
+        }
+    }
+
+#pragma unroll
+    for (int mt = 0; mt < PK_MTILES; mt++)
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
+            const u32 col = col0 + pk_acc_col(t, i);
+            if (row >= batch) continue;
+            const u32 v = pk_combine(acc[0][mt][i], acc[1][mt][i], acc[2][mt][i], acc[3][mt][i]);
+            if (col < n) out_a[row * n + col] = (i32)v;
+            else if (col == n) out_b[row] = (i32)(v + (u32)mus[row]);
+            else if (col == n + 1) out_cv[row] = (float)acc[0][mt][i] * row_variance;   // the popcount of R's row
+        }
 }
 
 }  // namespace nb

@@ -325,6 +325,37 @@ class Engine:
                    ctypes.c_uint64(int(first)), _ptr(out), out.numel())
         return out
 
+    def pk_prepare(self, a, b):
+        """[A | b | 1] of a public key, a (m, n) and b (m,) int32, laid into the 4 byte planes that public_encrypt reads
+        (nb_pk_prepare): a uint8 tensor of nb_pk_planes_bytes(m, n) bytes."""
+        a = self._dense(a, torch.int32)
+        b = self._dense(b, torch.int32)
+        m, n = a.shape
+        if b.shape != (m,):
+            raise ValueError('public-key bodies of shape %s for %d rows' % (tuple(b.shape), m))
+        planes = self.empty((self.lib.nb_pk_planes_bytes(m, n),), torch.uint8)
+        self._call('nb_pk_prepare', _ptr(a), _ptr(b), m, n, _ptr(planes))
+        return planes
+
+    def public_encrypt(self, r_words, planes, m, n, mus, row_variance):
+        """Public-key encryption of the B = mus.numel() messages `mus` (int32) with the random binary matrix R given as
+        r_words (B, m/32) (bit i of row c = bit i % 32 of word (c, i // 32)) and `planes` from pk_prepare
+        (nb_pk_encrypt).  Returns a (B, n), b (B,) int32 and the variances (B,) float32."""
+        r_words = self._dense(r_words, torch.int32)
+        mus = self._dense(mus, torch.int32).reshape(-1)
+        planes = self._dense(planes, torch.uint8)
+        batch = mus.numel()
+        out_a, out_b = self.empty((batch, n), torch.int32), self.empty((batch,), torch.int32)
+        out_cv = self.empty((batch,), torch.float32)
+        if planes.numel() != self.lib.nb_pk_planes_bytes(m, n) or (m % 32 == 0 and r_words.numel() != batch * (m // 32)):
+            raise ValueError('public_encrypt: %d plane bytes and %d R words do not fit m = %d, n = %d, %d messages'
+                             % (planes.numel(), r_words.numel(), m, n, batch))
+        if batch == 0:
+            return out_a, out_b, out_cv
+        self._call('nb_pk_encrypt', _ptr(r_words), _ptr(planes), m, n, _ptr(mus), ctypes.c_float(float(row_variance)),
+                   _ptr(out_a), _ptr(out_b), _ptr(out_cv), batch)
+        return out_a, out_b, out_cv
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()
