@@ -2,7 +2,8 @@
  * nufhe_b200.h -- C ABI of libnufhe_b200.so, the H100 (sm_90a) engine for the gate-bootstrapping hot
  * path of nucypher/nufhe, for programmable bootstrapping (lookup tables on small encrypted integers,
  * nb_bootstrap_lut_extract), for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
- * device from a seed (nb_seeded_uniform_i32), and for public-key encryption (nb_pk_prepare, nb_pk_encrypt).
+ * device from a seed (nb_seeded_uniform_i32), for public-key encryption (nb_pk_prepare, nb_pk_encrypt), and for
+ * packing results into GLWE samples (nb_pack_digits, nb_ntt_mac, nb_pack_finish).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -197,6 +198,25 @@ size_t nb_pk_planes_bytes(size_t m, size_t n);
 int nb_pk_prepare(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t m, size_t n, uint8_t *planes);
 int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, size_t m, size_t n, const int32_t *mus,
                   float row_variance, int32_t *out_a, int32_t *out_b, float *out_cv, size_t batch);
+
+/* ---- result packing (DESIGN.md section 12; no reference counterpart).  B LWE samples under the n-word key become
+ * G = ceil(B / 1024) GLWE samples (k + 1 polynomials of N = 1024 coefficients): input c goes to group c / 1024, slot
+ * c % 1024.  The steps: nb_pack_digits, nb_ntt_forward_i32 of the digits, nb_ntt_mac with the spectra of the packing
+ * key, nb_ntt_inverse_i32, nb_pack_finish.
+ * nb_pack_digits: a (B, n) int32 -> digits (G, 2 n, N) int32; row 2 i + j of group g holds at coefficient p the digit j
+ *     of a[g N + p][i]: with w = a + 2^15 + 2^23 + 2^31 (mod 2^32), d_0 = (w >> 24) - 128, d_1 = ((w >> 16) & 255) - 128.
+ *     Empty slots of the last group are 0.  NB_EINVAL for a NULL pointer, n = 0 or n > 2^20, and G > 2047.
+ * nb_ntt_mac: out (G, U, N) = sum_{r < R} x (G, R, N) . key (R, U, N), element-wise products of plain-form (not
+ *     Montgomery) field elements, out canonical.  NB_EINVAL for a NULL pointer, R = 0, U = 0, R > 2^24 or U > 2^16.
+ * nb_pack_finish: c (G, k + 1, N) int32, the inverse transform of the MAC, and the bodies b (B,) int32 ->
+ *     out (G, k + 1, N) uint16: round_16(-c) for polynomials u < k, round_16(b[g N + p] - c) at coefficient p of the
+ *     body (b = 0 in empty slots), round_16(x) = (x + 2^15) >> 16 on the 32-bit x.  NB_EINVAL for a NULL pointer and
+ *     k < 1.
+ * batch / groups = 0 is a no-op for all three. */
+int nb_pack_digits(nb_ctx *ctx, const int32_t *a, size_t n, int32_t *digits, size_t batch);
+int nb_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *key, uint64_t *out, size_t rows, size_t outs,
+               size_t groups);
+int nb_pack_finish(nb_ctx *ctx, const int32_t *c, const int32_t *b, int mask_size, uint16_t *out, size_t batch);
 
 #ifdef __cplusplus
 }

@@ -50,6 +50,13 @@ from .public_key import (
     public_key_size,
     public_encrypt,
     )
+from .packing import (
+    NuFHEPackingSecretKey,
+    NuFHEPackingKey,
+    PackedLweSampleArray,
+    make_packing_keys,
+    pack,
+    )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

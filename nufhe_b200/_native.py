@@ -56,6 +56,9 @@ SIGNATURES = {
     'nb_pk_planes_bytes': [_sz, _sz],
     'nb_pk_prepare': [_vp, _vp, _vp, _sz, _sz, _vp],
     'nb_pk_encrypt': [_vp, _vp, _vp, _sz, _sz, _vp, ctypes.c_float, _vp, _vp, _vp, _sz],
+    'nb_pack_digits': [_vp, _vp, _sz, _vp, _sz],
+    'nb_ntt_mac': [_vp, _vp, _vp, _vp, _sz, _sz, _sz],
+    'nb_pack_finish': [_vp, _vp, _vp, _int, _vp, _sz],
 }
 _RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p, 'nb_build_info': ctypes.c_char_p}
 

@@ -6,6 +6,8 @@ from .api_low_level import (
 from .lwe import LweSampleArray, lwe_copy, lwe_add_to
 from .compressed import CompressedLweSampleArray, CompressedCloudKey
 from .public_key import NuFHEPublicKey
+from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
+                      decrypt_packed, decrypt_packed_int)
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -109,6 +111,11 @@ class Context:
         """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
         return NuFHEPublicKey.from_secret_key(self.thread, self.rng, secret_key)
 
+    def make_packing_keys(self, secret_key: NuFHESecretKey):
+        """(NuFHEPackingSecretKey, NuFHEPackingKey): the client keeps the first to decrypt packed results, the server
+        takes the second for `VirtualMachine.pack`."""
+        return make_packing_keys(self.thread, self.rng, secret_key)
+
     def make_key_pair(self, **params):
         secret_key = self.make_secret_key(**params)
         cloud_key = self.make_cloud_key(secret_key)
@@ -119,14 +126,21 @@ class Context:
         CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute)."""
         return encrypt(self.thread, self.rng, key, message, compressed=compressed)
 
-    def decrypt(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray):
+    def decrypt(self, secret_key, ciphertext):
+        """An LweSampleArray with its NuFHESecretKey, or a PackedLweSampleArray with its NuFHEPackingSecretKey
+        (TypeError for any other pairing)."""
+        if isinstance(secret_key, NuFHEPackingSecretKey) or isinstance(ciphertext, PackedLweSampleArray):
+            return decrypt_packed(self.thread, secret_key, ciphertext)
         return decrypt(self.thread, secret_key, ciphertext)
 
     def encrypt_int(self, key, values, bits, compressed=False):
         """Integers in [0, 2^bits), bits = 1..3, for lookup tables (VirtualMachine.lut); `key` as for encrypt()."""
         return encrypt_int(self.thread, self.rng, key, values, bits, compressed=compressed)
 
-    def decrypt_int(self, secret_key: NuFHESecretKey, ciphertext: LweSampleArray, bits):
+    def decrypt_int(self, secret_key, ciphertext, bits):
+        """As for decrypt(): a packed array goes with its NuFHEPackingSecretKey."""
+        if isinstance(secret_key, NuFHEPackingSecretKey) or isinstance(ciphertext, PackedLweSampleArray):
+            return decrypt_packed_int(self.thread, secret_key, ciphertext, bits)
         return decrypt_int(self.thread, secret_key, ciphertext, bits)
 
     def make_virtual_machine(self, cloud_key: NuFHECloudKey, perf_params: PerformanceParameters = None):
@@ -151,6 +165,21 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return NuFHEPublicKey.loads(file_or_bytestring, self.thread)
         return NuFHEPublicKey.load(file_or_bytestring, self.thread)
+
+    def load_packed_ciphertext(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return PackedLweSampleArray.loads(file_or_bytestring, self.thread)
+        return PackedLweSampleArray.load(file_or_bytestring, self.thread)
+
+    def load_packing_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHEPackingKey.loads(file_or_bytestring, self.thread)
+        return NuFHEPackingKey.load(file_or_bytestring, self.thread)
+
+    def load_packing_secret_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHEPackingSecretKey.loads(file_or_bytestring, self.thread)
+        return NuFHEPackingSecretKey.load(file_or_bytestring, self.thread)
 
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
@@ -223,6 +252,12 @@ class VirtualMachine:
         lwe_copy(self.thread, dest, x)          # both nb_lwe_affine, with broadcasting and variances
         lwe_add_to(self.thread, dest, y)
         return dest
+
+    def pack(self, packing_key: NuFHEPackingKey, ciphertexts: LweSampleArray):
+        """Pack results of any shape into GLWE samples, 4 bytes per bit to download (nufhe_b200/packing.py)."""
+        if packing_key.params != self.params:
+            raise ValueError('the packing key was made for other parameters than this virtual machine')
+        return pack(self.thread, packing_key, ciphertexts)
 
     def capture(self, circuit, reserve_batch=None):
         """Record `circuit()` -- any sequence of this VM's gates on device-resident ciphertexts -- into a CUDA graph;

@@ -819,4 +819,50 @@ int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, si
     return launch_check(ctx, "pk_encrypt_kernel");
 }
 
+int nb_pack_digits(nb_ctx *ctx, const int32_t *a, size_t n, int32_t *digits, size_t batch)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!a || !digits) return fail(ctx, NB_EINVAL, "nb_pack_digits: null argument");
+    if (n == 0 || n > (1u << 20)) return fail(ctx, NB_EINVAL, "nb_pack_digits: bad LWE dimension");
+    if (batch == 0) return NB_OK;
+    const size_t groups = (batch + PACK_N - 1) / PACK_N, tiles = groups * (PACK_N / PACK_TILE);
+    if (tiles > 65535) return fail(ctx, NB_EINVAL, "nb_pack_digits: more than 2047 groups in one call");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:pack_digits");
+    const dim3 grid((unsigned)((n + PACK_TILE - 1) / PACK_TILE), (unsigned)tiles);
+    pack_digits_kernel<<<grid, PACK_DIGITS_THREADS, 0, ctx->stream>>>(a, (u32)n, (u64)batch, digits);
+    return launch_check(ctx, "pack_digits_kernel");
+}
+
+int nb_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *key, uint64_t *out, size_t rows, size_t outs,
+               size_t groups)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!x || !key || !out) return fail(ctx, NB_EINVAL, "nb_ntt_mac: null argument");
+    if (rows == 0 || outs == 0 || rows > (1u << 24) || outs > (1u << 16))
+        return fail(ctx, NB_EINVAL, "nb_ntt_mac: rows must be in [1, 2^24] and outputs in [1, 2^16]");
+    if (groups == 0) return NB_OK;
+    const size_t ctas = groups * (PACK_N / MAC_POINTS);
+    if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_ntt_mac: too many groups");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:ntt_mac");
+    const dim3 grid((unsigned)ctas, (unsigned)((outs + MAC_OUTS - 1) / MAC_OUTS));
+    ntt_mac_kernel<<<grid, MAC_WARPS * 32, 0, ctx->stream>>>((const u64 *)x, (const u64 *)key, (u64 *)out, (u32)rows,
+                                                            (u32)outs);
+    return launch_check(ctx, "ntt_mac_kernel");
+}
+
+int nb_pack_finish(nb_ctx *ctx, const int32_t *c, const int32_t *b, int mask_size, uint16_t *out, size_t batch)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!c || !b || !out) return fail(ctx, NB_EINVAL, "nb_pack_finish: null argument");
+    if (mask_size < 1 || mask_size > (1 << 16)) return fail(ctx, NB_EINVAL, "nb_pack_finish: bad mask size");
+    if (batch == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:pack_finish");
+    const size_t total = (batch + PACK_N - 1) / PACK_N * (size_t)(mask_size + 1) * PACK_N;
+    pack_finish_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(c, b, (u32)mask_size, (u64)batch, out, (u64)total);
+    return launch_check(ctx, "pack_finish_kernel");
+}
+
 }  // extern "C"

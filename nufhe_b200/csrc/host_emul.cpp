@@ -9,6 +9,7 @@
 #include "lut_index.cuh"
 #include "chacha.cuh"
 #include "pk_layout.cuh"
+#include "pack_layout.cuh"
 
 using namespace nb;
 
@@ -448,6 +449,17 @@ void emul_pk_encrypt(const u32 *r_bits, const i32 *a, const i32 *b, size_t m, si
             }
         }
 }
+
+// Result packing (pack_layout.cuh): the digits of `count` mask words (out[2 c + j] = digit j of a[c]), the 16-bit mod
+// switch and its inverse, and the slot mapping of input c.
+void emul_pack_digits(const i32 *a, size_t count, i32 *out)
+{
+    for (size_t c = 0; c < count; c++)
+        for (int j = 0; j < PACK_LEVELS; j++) out[c * PACK_LEVELS + j] = pack_digit(a[c], j);
+}
+void emul_pack_round16(const u32 *x, size_t count, uint16_t *out) { for (size_t i = 0; i < count; i++) out[i] = pack_round16(x[i]); }
+void emul_pack_unround16(const uint16_t *x, size_t count, u32 *out) { for (size_t i = 0; i < count; i++) out[i] = pack_unround16(x[i]); }
+void emul_pack_slot(u64 c, u64 *group, u32 *slot) { *group = pack_group(c); *slot = pack_slot(c); }
 
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)
 { for (size_t i = 0; i < n; i++) out[i] = ff_shl_var(in[i], s[i]); }

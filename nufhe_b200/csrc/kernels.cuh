@@ -24,6 +24,7 @@
 #include "lut_index.cuh"
 #include "chacha.cuh"
 #include "pk_layout.cuh"
+#include "pack_layout.cuh"
 
 namespace nb {
 
@@ -1495,6 +1496,112 @@ __global__ void __launch_bounds__(PK_WARPS * 32) pk_encrypt_kernel(
             else if (col == n) out_b[row] = (i32)(v + (u32)mus[row]);
             else if (col == n + 1) out_cv[row] = (float)acc[0][mt][i] * row_variance;   // the popcount of R's row
         }
+}
+
+// ---- result packing (DESIGN.md section 12; slot mapping, digits and rounding in pack_layout.cuh).
+// nb_pack_digits: LWE masks a (batch, n) row-major -> digit polynomials (groups, n t, N), row i t + j of group g holding
+// digit j of a[g N + p][i] at coefficient p.  A transpose: a CTA stages a 32 x 32 tile (32 inputs x 32 mask words) in
+// shared memory, loads it along the mask (128 bytes per warp row) and stores it along the slots (128 bytes per warp
+// row of a digit polynomial).  The row stride of 33 words keeps the column reads free of bank conflicts.
+constexpr int PACK_TILE = 32;
+constexpr int PACK_DIGITS_THREADS = 256;
+
+__global__ void __launch_bounds__(PACK_DIGITS_THREADS) pack_digits_kernel(const i32 *__restrict__ a, u32 n, u64 batch,
+                                                                           i32 *__restrict__ out)
+{
+    __shared__ i32 tile[PACK_TILE][PACK_TILE + 1];
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const u32 i0 = blockIdx.x * PACK_TILE;
+    const u64 c0 = (u64)blockIdx.y * PACK_TILE;                  // 32 consecutive inputs, all in one group
+#pragma unroll
+    for (int r = ty; r < PACK_TILE; r += PACK_DIGITS_THREADS / 32) {
+        const u64 c = c0 + r;
+        const u32 i = i0 + tx;
+        tile[r][tx] = (c < batch && i < n) ? __ldcs(a + c * n + i) : 0;     // an empty slot has the digits of 0, i.e. 0
+    }
+    __syncthreads();
+    const u64 g = pack_group(c0);
+    const u32 p = pack_slot(c0) + tx;
+#pragma unroll 4
+    for (int q = ty; q < PACK_TILE * PACK_LEVELS; q += PACK_DIGITS_THREADS / 32) {
+        const u32 i = i0 + q / PACK_LEVELS;
+        const int j = q % PACK_LEVELS;
+        if (i < n) out[((g * n + i) * PACK_LEVELS + j) * PACK_N + p] = pack_digit(tile[tx][q / PACK_LEVELS], j);
+    }
+}
+
+// nb_ntt_mac: out (G, U, N) = sum_r x (G, R, N) . key (R, U, N) on plain-form field elements.  A CTA owns 64 points of
+// one group and up to 2 outputs; a lane 2 adjacent points (128-bit loads), each warp a slice r = warp, warp + 16, ...
+// of the sum.  The 128-bit products are summed exactly in five 32-bit limbs (mac128) and folded once per warp slice, as
+// ff_dot4 does; the 16 slices are added in shared memory.  The digit spectra x are read once with streaming loads, so
+// that the key spectra, which every CTA of a group reads, stay in L2.
+constexpr int MAC_WARPS = 16;
+constexpr int MAC_POINTS = 64;
+constexpr int MAC_OUTS = 2;
+
+__global__ void __launch_bounds__(MAC_WARPS * 32) ntt_mac_kernel(const u64 *__restrict__ x, const u64 *__restrict__ key,
+                                                                 u64 *__restrict__ out, u32 R, u32 U)
+{
+#if defined(__CUDA_ARCH__)          // (mac128 and the limb fold exist on the device only)
+    __shared__ u64 part[MAC_WARPS][MAC_OUTS][MAC_POINTS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const u64 g = blockIdx.x / (PACK_N / MAC_POINTS);
+    const u32 pt0 = (blockIdx.x % (PACK_N / MAC_POINTS)) * MAC_POINTS, pt = pt0 + 2 * lane;
+    const u32 u0 = blockIdx.y * MAC_OUTS, outs = U - u0 < (u32)MAC_OUTS ? U - u0 : (u32)MAC_OUTS;
+    u32 acc[MAC_OUTS][2][5];
+#pragma unroll
+    for (int o = 0; o < MAC_OUTS; o++)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int l = 0; l < 5; l++) acc[o][h][l] = 0;
+    const u64 *xg = x + g * R * PACK_N + pt;
+    const u64 *kg = key + (u64)u0 * PACK_N + pt;
+#pragma unroll 4
+    for (u32 r = warp; r < R; r += MAC_WARPS) {
+        const ulonglong2 xv = __ldcs((const ulonglong2 *)(xg + (u64)r * PACK_N));
+#pragma unroll
+        for (int o = 0; o < MAC_OUTS; o++) {
+            if (o < (int)outs) {
+                const ulonglong2 kv = __ldg((const ulonglong2 *)(kg + ((u64)r * U + o) * PACK_N));
+                mac128(xv.x, kv.x, acc[o][0][0], acc[o][0][1], acc[o][0][2], acc[o][0][3], acc[o][0][4]);
+                mac128(xv.y, kv.y, acc[o][1][0], acc[o][1][1], acc[o][1][2], acc[o][1][3], acc[o][1][4]);
+            }
+        }
+    }
+    // fold: 2^128 = -2^32 (mod p), and the carry limb counts at most one per term
+#pragma unroll
+    for (int o = 0; o < MAC_OUTS; o++)
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const u32 *c = acc[o][h];
+            part[warp][o][2 * lane + h] = ff_sub(ff_reduce_limbs(c[0], c[1], c[2], c[3]), (u64)c[4] << 32);
+        }
+    __syncthreads();
+    if (threadIdx.x < MAC_OUTS * MAC_POINTS) {
+        const int o = threadIdx.x / MAC_POINTS, q = threadIdx.x % MAC_POINTS;
+        if (o < (int)outs) {
+            u64 s = part[0][o][q];
+#pragma unroll
+            for (int w = 1; w < MAC_WARPS; w++) s = ff_add(s, part[w][o][q]);
+            out[(g * U + u0 + o) * PACK_N + pt0 + q] = ff_canon(s);     // (the folds leave [0, p])
+        }
+    }
+#endif
+}
+
+// nb_pack_finish: out (G, k+1, N) uint16 = round_16(-C) for the masks, round_16(b_c - C) at the slots of the body.
+__global__ void pack_finish_kernel(const i32 *__restrict__ c, const i32 *__restrict__ b, u32 k, u64 batch,
+                                   uint16_t *__restrict__ out, u64 total)
+{
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (u64)gridDim.x * blockDim.x) {
+        const u64 poly = i / PACK_N, g = poly / (k + 1);
+        const u32 u = (u32)(poly % (k + 1));
+        const u64 cidx = g * PACK_N + (i % PACK_N);
+        u32 v = 0u - (u32)c[i];
+        if (u == k && cidx < batch) v += (u32)b[cidx];
+        out[i] = pack_round16(v);
+    }
 }
 
 }  // namespace nb

@@ -356,6 +356,43 @@ class Engine:
                    _ptr(out_a), _ptr(out_b), _ptr(out_cv), batch)
         return out_a, out_b, out_cv
 
+    def pack_digits(self, a):
+        """LWE masks a (B, n) int32 -> digit polynomials (ceil(B / N), 2 n, N) int32: row 2 i + j of group g holds digit
+        j of a[g N + p][i] at coefficient p, 0 in the empty slots (nb_pack_digits)."""
+        a = self._dense(a, torch.int32)
+        batch, n = a.shape
+        out = self.empty(((batch + N - 1) // N, 2 * n, N), torch.int32)
+        if batch:
+            self._call('nb_pack_digits', _ptr(a), n, _ptr(out), batch)
+        return out
+
+    def ntt_mac(self, x, key):
+        """out (G, U, N) = sum_r x (G, R, N) . key (R, U, N) on plain-form field elements (nb_ntt_mac)."""
+        x = self._dense(x, torch.int64)
+        key = self._dense(key, torch.int64)
+        if x.dim() != 3 or key.dim() != 3 or x.shape[2] != N or key.shape[2] != N or x.shape[1] != key.shape[0]:
+            raise ValueError('ntt_mac: x %s and key %s are not (G, R, N) and (R, U, N)' % (tuple(x.shape), tuple(key.shape)))
+        groups, rows = x.shape[:2]
+        outs = key.shape[1]
+        out = self.empty((groups, outs, N), torch.int64)
+        if groups:
+            self._call('nb_ntt_mac', _ptr(x), _ptr(key), _ptr(out), rows, outs, groups)
+        return out
+
+    def pack_finish(self, c, b):
+        """c (G, k+1, N) int32 and the bodies b (B,) int32 -> (G, k+1, N) uint16: round_16(-c) for the masks,
+        round_16(b[g N + p] - c) at the slots of the body (nb_pack_finish)."""
+        c = self._dense(c, torch.int32)
+        b = self._dense(b, torch.int32).reshape(-1)
+        groups, k1 = c.shape[0], c.shape[1]
+        batch = b.numel()
+        if c.dim() != 3 or c.shape[2] != N or groups != (batch + N - 1) // N:
+            raise ValueError('pack_finish: %s polynomials for %d bodies' % (tuple(c.shape), batch))
+        out = self.empty(tuple(c.shape), torch.uint16)
+        if batch:
+            self._call('nb_pack_finish', _ptr(c), _ptr(b), k1 - 1, _ptr(out), batch)
+        return out
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()
