@@ -26,6 +26,7 @@
 #pragma once
 #include <cmath>
 #include "ntt_lane.cuh"
+#include "fft_layout.cuh"
 
 namespace nb {
 
@@ -1170,30 +1171,29 @@ template <class Cfg = BrDefault> NB_HD bool map_inv3(int tid, int &p, int &row, 
 // Negacyclic fold: a polynomial a of degree < 1024 becomes z_j = (a_j + i a_{j+512}) w^j, j < 512, w = e^{i pi / 1024};
 // its 512-point DFT (root e^{-2 pi i / 512}) is a evaluated at 512 roots of X^1024 + 1 that carry z^512 = i, so the
 // point-wise product of two such spectra is the spectrum of the negacyclic product.
-// The DFT is three radix-8 passes, decimation in frequency (natural order in, digit-reversed order out); the inverse
-// is the mirrored decimation-in-time network, so the MAC works point-wise and nothing is reordered:
-//     pass 1, task n0 < 64:          x[n0 + 64 m]                -> DFT8 over m, times W512^(n0 k1) -> x[n0 + 64 k1]
-//     pass 2, task (k1, n1 < 8):     x[64 k1 + n1 + 8 m]         -> DFT8, times W64^(n1 k2)        -> x[64 k1 + n1 + 8 k2]
-//     pass 3, task (k1, k2):         x[64 k1 + 8 k2 + m]         -> DFT8                            -> x[64 k1 + 8 k2 + k3]
-// leaving X[k1 + 8 k2 + 64 k3] at position 64 k1 + 8 k2 + k3.  A spectrum is 512 complex values in shared memory,
-// position x stored at x + x / 8 (one pad per 8) so that the 16-byte accesses of every pass are bank-conflict free.
+// The DFT is a radix 8 x 16 x 4 plan, decimation in frequency (natural order in, digit-reversed order out); the
+// inverse runs the mirrored passes, so the MAC works point-wise and nothing is reordered:
+//     pass 1, task n0 < 64:          x[n0 + 64 m]             -> DFT8 over m, times W512^(n0 k1) -> x[n0 + 64 k1]
+//     pass 2, task (k1, n2 < 4):     x[64 k1 + n2 + 4 m]      -> DFT16, times W64^(n2 k2)       -> x[64 k1 + n2 + 4 k2]
+//     pass 3, task (k1, k2):         x[64 k1 + 4 k2 + m]      -> DFT4                           -> x[64 k1 + 4 k2 + k3]
+// leaving X[k1 + 8 k2 + 128 k3] at position 64 k1 + 4 k2 + k3.  Pass 3 is fused with the MAC and the first inverse
+// pass: a thread holds the 4 points of group g = 16 k1 + k2 of all 4 digit spectra, transforms them, and for one
+// output spectrum at a time multiplies with the key, runs the inverse DFT4 and stores.  A step is five
+// barrier-separated phases: fwd1, fwd2, pass 3, inv2, inv1.  Shared-memory positions and thread maps: fft_layout.cuh.
 // Every floating-point operation is an explicit, correctly rounded add / mul / fma (__dadd_rn & co. are never
 // contracted by the compiler), in the order the error bound of DESIGN.md section 3 assumes; the host emulation
 // (csrc/host_emul.cpp, no FMA contraction) computes the same bits.
 struct cplx {
     double re, im;
 };
-constexpr int FFT_M = 512;                          // complex points per spectrum
-constexpr int FFT_SPEC_CPLX = FFT_M + FFT_M / 8;    // padded spectrum in shared memory
-NB_HD int fft_pad(int x) { return x + (x >> 3); }
 // Engine bootstrap-key row, FP64 part: 16 spectra [(m = (mi * 2 + j) * 2 + mo) * 2 + h][512] (h = 0: k_lo, 1: k_hi),
-// unpadded, complex doubles; it follows the NTT planes of the same row.
+// unpadded, complex doubles, each in the order of fft_key_pos; it follows the NTT planes of the same row.
 constexpr int BK_FFT_SPECTRA = 16;
 constexpr int BK_FFT_U64 = BK_FFT_SPECTRA * FFT_M * 2;
 static_assert(BK_ROW_U64 == BK_NTT_U64 + BK_FFT_U64, "key row layout");
 // tables (tables.h: FftTables), complex, concatenated: twist w^j (512), pass-1 twiddles W512^(n0 k1) [n0][k1] (512),
-// pass-2 twiddles W64^(n1 k2) [n1][k2] (64), untwist conj(w^j) / 512 (512)
-constexpr int FFT_TAB_TWIST = 0, FFT_TAB_TW1 = 512, FFT_TAB_TW2 = 1024, FFT_TAB_UNTWIST = 1088, FFT_TAB_CPLX = 1600;
+// untwist conj(w^j) / 512 (512).  The pass-2 twiddles are compile-time constants (fft_w64).
+constexpr int FFT_TAB_TWIST = 0, FFT_TAB_TW1 = 512, FFT_TAB_UNTWIST = 1024, FFT_TAB_CPLX = 1536;
 
 #if defined(__CUDA_ARCH__)
 NB_HD double d_add(double a, double b) { return __dadd_rn(a, b); }
@@ -1239,36 +1239,70 @@ NB_HD cplx c_mac(cplx acc, cplx a, cplx b)
 {
     return {d_fma(-a.im, b.im, d_fma(a.re, b.re, acc.re)), d_fma(a.im, b.re, d_fma(a.re, b.im, acc.im))};
 }
+// times -i (forward) / +i (inverse): exact
+template <bool INV> NB_HD cplx c_mul_mi(cplx a) { return INV ? cplx{-a.im, a.re} : cplx{a.im, -a.re}; }
+// times e^{-+ i pi / 4} = (1 -+ i) sqrt(1/2): one addition and one product per component with the rounded constant
+template <bool INV> NB_HD cplx c_mul_w8(cplx a)
+{
+    constexpr double S = 0.70710678118654752440;
+    return INV ? cplx{d_mul(d_sub(a.re, a.im), S), d_mul(d_add(a.re, a.im), S)} : cplx{d_mul(d_add(a.re, a.im), S), d_mul(d_sub(a.im, a.re), S)};
+}
+
+// W64^e = e^{-2 pi i e / 64}: cos (2 pi r / 64), r <= 16, evaluated in long double and rounded once (as the tables),
+// the quadrant e / 16 applied exactly (swap and sign).  Evaluated at compile time: the twiddles of pass 2 are operands
+// from the constant bank, not loads into registers.
+NB_HD constexpr cplx fft_w64(int e)
+{
+    constexpr double c[17] = {1, 0.99518472667219693, 0.98078528040323043, 0.95694033573220882, 0.92387953251128674,
+                              0.88192126434835505, 0.83146961230254524, 0.77301045336273699, 0.70710678118654757,
+                              0.63439328416364549, 0.55557023301960218, 0.47139673682599764, 0.38268343236508978,
+                              0.29028467725446239, 0.19509032201612828, 0.098017140329560604, 0};
+    const int q = (e >> 4) & 3, r = e & 15;
+    const double re = c[r], im = -c[16 - r];
+    return q == 0 ? cplx{re, im} : q == 1 ? cplx{im, -re} : q == 2 ? cplx{-re, -im} : cplx{-im, re};
+}
+// y[k] *= W64^(N2 k) (forward) / its conjugate (inverse), k = 1 .. 15
+template <int N2, bool INV> NB_HD void fft_w64_twiddle(cplx *y)
+{
+    static_for<1, 16>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        constexpr cplx w = fft_w64(N2 * k);
+        y[k] = INV ? c_mul_conj(y[k], w) : c_mul(y[k], w);
+    });
+}
+// the same for a run-time n2 (warp-uniform in the step: fft_pass2_task); n2 = 0 multiplies by 1
+template <bool INV> NB_HD void fft_w64_twiddle(int n2, cplx *y)
+{
+    switch (n2) {
+    case 0: break;
+    case 1: fft_w64_twiddle<1, INV>(y); break;
+    case 2: fft_w64_twiddle<2, INV>(y); break;
+    default: fft_w64_twiddle<3, INV>(y); break;
+    }
+}
 
 // 8-point DFT in place, natural order in and out: y[k] = sum_m y[m] e^{-+ 2 pi i m k / 8} (INV: the + sign), as three
 // radix-2 decimation-in-frequency layers.  Multiplications by -+i are exact (swap and sign); by e^{-+ i pi / 4} one
 // addition and one product per component with the rounded constant sqrt(1/2).
 template <bool INV> NB_HD void dft8(cplx *y)
 {
-    constexpr double S = 0.70710678118654752440;
-    auto mul_mi = [](cplx a) -> cplx { return INV ? cplx{-a.im, a.re} : cplx{a.im, -a.re}; };       // times -i (fwd) / +i (inv)
     cplx t[8];
     static_for<0, 4>([&](auto M) {
         constexpr int m = decltype(M)::value;
         t[m] = c_add(y[m], y[m + 4]);
         t[m + 4] = c_sub(y[m], y[m + 4]);
     });
-    // t[4 + m] *= W8^m, W8 = e^{-+ i pi / 4}
-    {
-        const cplx a = t[5];           // (re + im) S - i (re - im) S  (fwd);  (re - im) S + i (re + im) S  (inv)
-        t[5] = INV ? cplx{d_mul(d_sub(a.re, a.im), S), d_mul(d_add(a.re, a.im), S)} : cplx{d_mul(d_add(a.re, a.im), S), d_mul(d_sub(a.im, a.re), S)};
-        t[6] = mul_mi(t[6]);
-        const cplx b = t[7];           // W8^3 = -+ i W8
-        const cplx c = INV ? cplx{d_mul(d_sub(b.re, b.im), S), d_mul(d_add(b.re, b.im), S)} : cplx{d_mul(d_add(b.re, b.im), S), d_mul(d_sub(b.im, b.re), S)};
-        t[7] = mul_mi(c);
-    }
+    // t[4 + m] *= W8^m, W8 = e^{-+ i pi / 4}; W8^3 = -+ i W8
+    t[5] = c_mul_w8<INV>(t[5]);
+    t[6] = c_mul_mi<INV>(t[6]);
+    t[7] = c_mul_mi<INV>(c_mul_w8<INV>(t[7]));
     cplx u[8];
     static_for<0, 2>([&](auto H) {
         constexpr int h = 4 * decltype(H)::value;
         u[h + 0] = c_add(t[h + 0], t[h + 2]);
         u[h + 1] = c_add(t[h + 1], t[h + 3]);
         u[h + 2] = c_sub(t[h + 0], t[h + 2]);
-        u[h + 3] = mul_mi(c_sub(t[h + 1], t[h + 3]));
+        u[h + 3] = c_mul_mi<INV>(c_sub(t[h + 1], t[h + 3]));
     });
     // last layer; outputs of the DIF network are bit-reversed: position p holds y[brev3(p)]
     y[0] = c_add(u[0], u[1]); y[4] = c_sub(u[0], u[1]);
@@ -1277,9 +1311,48 @@ template <bool INV> NB_HD void dft8(cplx *y)
     y[3] = c_add(u[6], u[7]); y[7] = c_sub(u[6], u[7]);
 }
 
+// 16-point DFT in place, natural order in and out: one radix-2 decimation-in-frequency layer (pairs m, m + 8), the
+// twiddles W16^(-+m) on the differences, and a DFT8 on the sums (even outputs) and one on the differences (odd
+// outputs).  W16^4 = -+i is exact, W16^2 and W16^6 = -+i W16^2 take c_mul_w8, W16^1, W16^3 and W16^5 = -+i W16^1,
+// W16^7 = -+i W16^3 one product and one fma per component with the rounded constants cos(pi / 8), sin(pi / 8).
+template <bool INV> NB_HD void dft16(cplx *y)
+{
+    constexpr double C = 0.92387953251128675613, S = 0.38268343236508977173;
+    constexpr cplx W1 = {C, INV ? S : -S}, W3 = {S, INV ? C : -C};
+    cplx a[8], b[8];
+    static_for<0, 8>([&](auto M) {
+        constexpr int m = decltype(M)::value;
+        a[m] = c_add(y[m], y[m + 8]);
+        b[m] = c_sub(y[m], y[m + 8]);
+    });
+    b[1] = c_mul(b[1], W1);
+    b[2] = c_mul_w8<INV>(b[2]);
+    b[3] = c_mul(b[3], W3);
+    b[4] = c_mul_mi<INV>(b[4]);
+    b[5] = c_mul_mi<INV>(c_mul(b[5], W1));
+    b[6] = c_mul_mi<INV>(c_mul_w8<INV>(b[6]));
+    b[7] = c_mul_mi<INV>(c_mul(b[7], W3));
+    dft8<INV>(a);
+    dft8<INV>(b);
+    static_for<0, 8>([&](auto K) {
+        constexpr int k = decltype(K)::value;
+        y[2 * k] = a[k];
+        y[2 * k + 1] = b[k];
+    });
+}
+
+// 4-point DFT in place, natural order in and out: two radix-2 layers, the multiplication by -+i exact
+template <bool INV> NB_HD void dft4(cplx *y)
+{
+    const cplx a = c_add(y[0], y[2]), b = c_sub(y[0], y[2]), c = c_add(y[1], y[3]);
+    const cplx d = c_mul_mi<INV>(c_sub(y[1], y[3]));
+    y[0] = c_add(a, c); y[2] = c_sub(a, c);
+    y[1] = c_add(b, d); y[3] = c_sub(b, d);
+}
+
 // pass 1 (forward): x[m'] = real coefficient n0 + 64 m', m' < 16 (exact small integers as doubles); fold, twist,
-// DFT8 over m, twiddle, store
-NB_HD void fft_fwd1(int n0, const double *x, cplx *spec, const cplx *tab)
+// DFT8 over m, twiddle, store at position n0 + 64 k1 of spectrum sp
+NB_HD void fft_fwd1(int n0, const double *x, cplx *sp, const cplx *tab)
 {
     cplx y[8];
     static_for<0, 8>([&](auto M) {
@@ -1288,61 +1361,46 @@ NB_HD void fft_fwd1(int n0, const double *x, cplx *spec, const cplx *tab)
         y[m] = {d_fma(x[m], w.re, -d_mul(x[m + 8], w.im)), d_fma(x[m], w.im, d_mul(x[m + 8], w.re))};
     });
     dft8<false>(y);
-    st_cplx(spec + fft_pad(n0), y[0]);
+    st_cplx(sp + fft_pass1_x(n0, 0), y[0]);
     static_for<1, 8>([&](auto K) {
         constexpr int k = decltype(K)::value;
-        st_cplx(spec + fft_pad(n0 + 64 * k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k)));
+        st_cplx(sp + fft_pass1_x(n0, k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k)));
     });
 }
-// pass 2 (forward), task (k1, n1)
-NB_HD void fft_fwd2(int k1, int n1, cplx *spec, const cplx *tab)
+// pass 2 (forward): the 16 points 64 k1 + n2 + 4 m of spectrum sp -> DFT16, times W64^(n2 k2)
+NB_HD void fft_fwd2(int k1, int n2, cplx *sp)
+{
+    cplx y[16];
+    static_for<0, 16>([&](auto M) { y[decltype(M)::value] = ld_cplx(sp + fft_pass2_x(k1, n2, decltype(M)::value)); });
+    dft16<false>(y);
+    fft_w64_twiddle<false>(n2, y);
+    static_for<0, 16>([&](auto K) { st_cplx(sp + fft_pass2_x(k1, n2, decltype(K)::value), y[decltype(K)::value]); });
+}
+// pass 3 (forward only, the key spectra): group g of spectrum sp, in place
+NB_HD void fft_fwd3(int g, cplx *sp)
+{
+    cplx y[4];
+    static_for<0, 4>([&](auto I) { y[decltype(I)::value] = ld_cplx(sp + fft_pass3_x(g, decltype(I)::value)); });
+    dft4<false>(y);
+    static_for<0, 4>([&](auto I) { st_cplx(sp + fft_pass3_x(g, decltype(I)::value), y[decltype(I)::value]); });
+}
+// pass 2 (inverse), mirrored
+NB_HD void fft_inv2(int k1, int n2, cplx *sp)
+{
+    cplx y[16];
+    static_for<0, 16>([&](auto M) { y[decltype(M)::value] = ld_cplx(sp + fft_pass2_x(k1, n2, decltype(M)::value)); });
+    fft_w64_twiddle<true>(n2, y);
+    dft16<true>(y);
+    static_for<0, 16>([&](auto M) { st_cplx(sp + fft_pass2_x(k1, n2, decltype(M)::value), y[decltype(M)::value]); });
+}
+// pass 1 (inverse): x[m'] = the (unrounded) real coefficient n0 + 64 m', m' < 16, of spectrum sp
+NB_HD void fft_inv1(int n0, const cplx *sp, const cplx *tab, double *x)
 {
     cplx y[8];
-    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(spec + fft_pad(64 * k1 + n1 + 8 * decltype(M)::value)); });
-    dft8<false>(y);
-    st_cplx(spec + fft_pad(64 * k1 + n1), y[0]);
+    y[0] = ld_cplx(sp + fft_pass1_x(n0, 0));
     static_for<1, 8>([&](auto K) {
         constexpr int k = decltype(K)::value;
-        st_cplx(spec + fft_pad(64 * k1 + n1 + 8 * k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW2 + n1 * 8 + k)));
-    });
-}
-// pass 3 (forward), task (k1, k2)
-NB_HD void fft_fwd3(int k1, int k2, cplx *spec)
-{
-    cplx y[8];
-    cplx *s = spec + fft_pad(64 * k1 + 8 * k2);        // the 8 positions are contiguous (one pad per 8)
-    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(s + decltype(M)::value); });
-    dft8<false>(y);
-    static_for<0, 8>([&](auto K) { st_cplx(s + decltype(K)::value, y[decltype(K)::value]); });
-}
-// the inverse passes, mirrored
-NB_HD void fft_inv3(int k1, int k2, cplx *spec)
-{
-    cplx y[8];
-    cplx *s = spec + fft_pad(64 * k1 + 8 * k2);
-    static_for<0, 8>([&](auto M) { y[decltype(M)::value] = ld_cplx(s + decltype(M)::value); });
-    dft8<true>(y);
-    static_for<0, 8>([&](auto K) { st_cplx(s + decltype(K)::value, y[decltype(K)::value]); });
-}
-NB_HD void fft_inv2(int k1, int n1, cplx *spec, const cplx *tab)
-{
-    cplx y[8];
-    y[0] = ld_cplx(spec + fft_pad(64 * k1 + n1));
-    static_for<1, 8>([&](auto K) {
-        constexpr int k = decltype(K)::value;
-        y[k] = c_mul_conj(ld_cplx(spec + fft_pad(64 * k1 + n1 + 8 * k)), ld_cplx_tab(tab + FFT_TAB_TW2 + n1 * 8 + k));
-    });
-    dft8<true>(y);
-    static_for<0, 8>([&](auto M) { st_cplx(spec + fft_pad(64 * k1 + n1 + 8 * decltype(M)::value), y[decltype(M)::value]); });
-}
-// pass 1 (inverse): x[m'] = the (unrounded) real coefficient n0 + 64 m', m' < 16
-NB_HD void fft_inv1(int n0, const cplx *spec, const cplx *tab, double *x)
-{
-    cplx y[8];
-    y[0] = ld_cplx(spec + fft_pad(n0));
-    static_for<1, 8>([&](auto K) {
-        constexpr int k = decltype(K)::value;
-        y[k] = c_mul_conj(ld_cplx(spec + fft_pad(n0 + 64 * k)), ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k));
+        y[k] = c_mul_conj(ld_cplx(sp + fft_pass1_x(n0, k)), ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k));
     });
     dft8<true>(y);
     static_for<0, 8>([&](auto M) {
@@ -1353,8 +1411,8 @@ NB_HD void fft_inv1(int n0, const cplx *spec, const cplx *tab, double *x)
     });
 }
 
-// ---- the FP64 step of a CTA of CT ciphertexts on 128 CT threads; spectra [ct * 4 + s][FFT_SPEC_CPLX], s = mi * 2 + j
-// before the MAC and s = mo * 2 + h after it.
+// ---- the FP64 step of a CTA of 2 ciphertexts on 256 threads: spectra fft_spec(ct, s), s = mi * 2 + j before the MAC
+// and s = mo * 2 + h after it.
 // fwd1: task (pm = ct * 2 + mi, n0): the rotated coefficients serve both digit polynomials (as phase_fwd1_both_digits)
 template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, cplx *spec_all, const cplx *tab, const int *rot_a)
 {
@@ -1370,7 +1428,6 @@ template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, c
         const i32 c = ROTATE ? rotate_minus_one(acc, idx, ar, flip) : acc[idx];
         t[j1] = (u32)c + (0x80000000u + (1u << 21));
     });
-    cplx *spec = spec_all + pm * 2 * FFT_SPEC_CPLX;
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif
@@ -1378,68 +1435,71 @@ template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, c
         const int sh = 22 - 10 * j;
         double x[16];
         static_for<0, 16>([&](auto J) { x[decltype(J)::value] = (double)((int)((t[decltype(J)::value] >> sh) & 1023u) - 512); });
-        fft_fwd1(n0, x, spec + j * FFT_SPEC_CPLX, tab);
+        fft_fwd1(n0, x, spec_all + fft_pass1_spec(task, j), tab);
     }
 }
-// fwd2 / fwd3 / inv3 / inv2: task x < 256 CT = (spectrum s = x / 64, a = (x / 8) % 8, b = x % 8)
-NB_HD void fft_phase_fwd2(int x, cplx *spec_all, const cplx *tab) { fft_fwd2((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX, tab); }
-NB_HD void fft_phase_fwd3(int x, cplx *spec_all) { fft_fwd3((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX); }
-NB_HD void fft_phase_inv3(int x, cplx *spec_all) { fft_inv3((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX); }
-NB_HD void fft_phase_inv2(int x, cplx *spec_all, const cplx *tab) { fft_inv2((x >> 3) & 7, x & 7, spec_all + (x >> 6) * FFT_SPEC_CPLX, tab); }
-
-// MAC at point P (< 512) of every ciphertext of the CTA: out[mo][h] = sum_d D_d K[d][mo][h]; the key values are loaded
-// once for all CT ciphertexts, the outputs overwrite the digit spectra at the same point (the thread holds them)
-template <int CT> NB_HD void fft_mac_point(int P, cplx *spec_all, const cplx *key)
+// fwd2 / inv2: one 16-point task per thread (fft_pass2_task)
+NB_HD void fft_phase_fwd2(int tid, cplx *spec_all)
 {
-    cplx dg[CT][4];
-    static_for<0, CT>([&](auto C) {
-        static_for<0, 4>([&](auto D) {
-            dg[decltype(C)::value][decltype(D)::value] = ld_cplx(spec_all + (decltype(C)::value * 4 + decltype(D)::value) * FFT_SPEC_CPLX + fft_pad(P));
-        });
-    });
-    static_for<0, 4>([&](auto S) {
-        constexpr int mo = decltype(S)::value >> 1, h = decltype(S)::value & 1;      // output spectrum mo * 2 + h
-        cplx k[4];
-#ifdef NB_FFT_KEY_L1_BOUND
-        // TIMING EXPERIMENT ONLY (wrong results): every key load hits the same 2 KB of the row -- what the step would
-        // take if the key stream cost nothing (DESIGN.md section 4, FP64 step breakdown)
-        const int kp = P & 15;
-#else
-        const int kp = P;
-#endif
-        static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(key + ((decltype(D)::value * 2 + mo) * 2 + h) * FFT_M + kp); });
-        static_for<0, CT>([&](auto C) {
-            constexpr int c = decltype(C)::value;
-            cplx o = {d_mul(dg[c][0].re, k[0].re), d_mul(dg[c][0].re, k[0].im)};
-            o = {d_fma(-dg[c][0].im, k[0].im, o.re), d_fma(dg[c][0].im, k[0].re, o.im)};
-            static_for<1, 4>([&](auto D) { o = c_mac(o, dg[c][decltype(D)::value], k[decltype(D)::value]); });
-            st_cplx(spec_all + (c * 4 + mo * 2 + h) * FFT_SPEC_CPLX + fft_pad(P), o);
-        });
-    });
+    const FftPass2 t = fft_pass2_task(tid);
+    fft_fwd2(t.k1, t.n2, spec_all + fft_spec(t.ct, t.s));
 }
-template <int CT, int THREADS> NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
+NB_HD void fft_phase_inv2(int tid, cplx *spec_all)
 {
+    const FftPass2 t = fft_pass2_task(tid);
+    fft_inv2(t.k1, t.n2, spec_all + fft_spec(t.ct, t.s));
+}
+
+// pass 3, fused: group fft_pass3_group(tid / 2) of ciphertext tid & 1 (fft_pass3_pos): the forward DFT4 of the 4 digit spectra, then for each output
+// spectrum s = mo * 2 + h the MAC out = sum_d D_d K[d][mo][h] at the 4 points and the inverse DFT4; the outputs
+// overwrite the digit spectra at the same positions (the thread holds all of them).
+NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
+{
+    const int j = tid >> 1;
+    cplx dg[4][4];
+    static_for<0, 4>([&](auto D) {
+        static_for<0, 4>([&](auto I) { dg[decltype(D)::value][decltype(I)::value] = ld_cplx(spec_all + fft_pass3_pos(tid, decltype(D)::value, decltype(I)::value)); });
+        dft4<false>(dg[decltype(D)::value]);
+    });
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif
-    for (int P = tid; P < FFT_M; P += THREADS) fft_mac_point<CT>(P, spec_all, key);
+    for (int s = 0; s < 4; s++) {
+        cplx o[4];
+        static_for<0, 4>([&](auto K3) {
+            constexpr int k3 = decltype(K3)::value;
+#ifdef NB_FFT_KEY_L1_BOUND
+            // TIMING EXPERIMENT ONLY (wrong results): every key load hits the same 2 KB of the row -- what the step
+            // would take if the key stream cost nothing (DESIGN.md section 4, FP64 step breakdown)
+            const int kj = j & 15;
+#else
+            const int kj = j;
+#endif
+            cplx k[4];
+            static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(key + fft_key_pos(4 * decltype(D)::value + s, kj, k3)); });
+            cplx v = {d_mul(dg[0][k3].re, k[0].re), d_mul(dg[0][k3].re, k[0].im)};
+            v = {d_fma(-dg[0][k3].im, k[0].im, v.re), d_fma(dg[0][k3].im, k[0].re, v.im)};
+            static_for<1, 4>([&](auto D) { v = c_mac(v, dg[decltype(D)::value][k3], k[decltype(D)::value]); });
+            o[k3] = v;
+        });
+        dft4<true>(o);
+        static_for<0, 4>([&](auto I) { st_cplx(spec_all + fft_pass3_pos(tid, s, decltype(I)::value), o[decltype(I)::value]); });
+    }
 }
 // inv1: task (pp = ct * 2 + mo, n0): both key halves of output polynomial mo, rounded and recombined mod 2^32.
 // ACCUMULATE: acc += result, else acc = result.
 template <bool ACCUMULATE> NB_HD void fft_phase_inv1(int task, i32 *acc_all, const cplx *spec_all, const cplx *tab)
 {
     const int n0 = task & 63, pp = task >> 6;
-    const int ct = pp >> 1, mo = pp & 1;
-    const cplx *spec = spec_all + (ct * 4 + mo * 2) * FFT_SPEC_CPLX;
     u32 r[16];
     {
         double x[16];
-        fft_inv1(n0, spec, tab, x);
+        fft_inv1(n0, spec_all + fft_pass1_spec(task, 0), tab, x);
         static_for<0, 16>([&](auto J) { r[decltype(J)::value] = (u32)d_rint_lo32(x[decltype(J)::value]); });
     }
     {
         double x[16];
-        fft_inv1(n0, spec + FFT_SPEC_CPLX, tab, x);
+        fft_inv1(n0, spec_all + fft_pass1_spec(task, 1), tab, x);
         static_for<0, 16>([&](auto J) { r[decltype(J)::value] += (u32)d_rint_lo32(x[decltype(J)::value]) << 16; });
     }
     i32 *acc = acc_all + pp * NTT_N;

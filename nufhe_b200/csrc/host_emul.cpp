@@ -234,7 +234,7 @@ void emul_phase_step_wide2(i32 *acc_io, const u64 *bk_ref_row, const int *rot)
 
 // ---- the FP64 step (br_phases.cuh: FP64 step) ----
 // key spectra of one polynomial from its centred integer coefficients k[1024], as bk_spectra_kernel computes them:
-// spec[h][512] unpadded (h = 0: k_lo, 1: k_hi)
+// spec[h][512] unpadded in the order of fft_key_pos (h = 0: k_lo, 1: k_hi)
 static void fft_key_spectra(const long long *k, cplx *spec, const FftTables &F)
 {
     std::vector<cplx> w(2 * FFT_SPEC_CPLX);
@@ -246,9 +246,11 @@ static void fft_key_spectra(const long long *k, cplx *spec, const FftTables &F)
         fft_fwd1(n0, lo, w.data(), F.tab.data());
         fft_fwd1(n0, hi, w.data() + FFT_SPEC_CPLX, F.tab.data());
     }
-    for (int h = 0; h < 2; h++) for (int t = 0; t < 64; t++) fft_fwd2(t >> 3, t & 7, w.data() + h * FFT_SPEC_CPLX, F.tab.data());
-    for (int h = 0; h < 2; h++) for (int t = 0; t < 64; t++) fft_fwd3(t >> 3, t & 7, w.data() + h * FFT_SPEC_CPLX);
-    for (int h = 0; h < 2; h++) for (int P = 0; P < FFT_M; P++) spec[h * FFT_M + P] = w[h * FFT_SPEC_CPLX + fft_pad(P)];
+    for (int h = 0; h < 2; h++) for (int t = 0; t < 32; t++) fft_fwd2(t & 7, t >> 3, w.data() + h * FFT_SPEC_CPLX);
+    for (int h = 0; h < 2; h++) for (int g = 0; g < FFT_M / 4; g++) fft_fwd3(g, w.data() + h * FFT_SPEC_CPLX);
+    for (int h = 0; h < 2; h++)
+        for (int j = 0; j < FFT_M / 4; j++)
+            for (int k3 = 0; k3 < 4; k3++) spec[fft_key_pos(h, j, k3)] = w[h * FFT_SPEC_CPLX + fft_pass3_x(fft_pass3_group(j), k3)];
 }
 
 // the FP64 part of one engine key row from the reference row (Montgomery, natural order): -1 if a coefficient is not a
@@ -302,11 +304,9 @@ int emul_fft_step(i32 *acc_io, const u64 *bk_ref_row, const int *rot, int nct)
     for (int tid = 0; tid < TH; tid++) {
         if (rot) fft_phase_fwd1<true>(tid, acc.data(), w.data(), tab, rots); else fft_phase_fwd1<false>(tid, acc.data(), w.data(), tab, rots);
     }
-    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_fwd2(x, w.data(), tab);
-    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_fwd3(x, w.data());
-    for (int tid = 0; tid < TH; tid++) fft_phase_mac<Cfg::CT, TH>(tid, w.data(), key.data());
-    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_inv3(x, w.data());
-    for (int x = 0; x < 256 * Cfg::CT; x++) fft_phase_inv2(x, w.data(), tab);
+    for (int tid = 0; tid < TH; tid++) fft_phase_fwd2(tid, w.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_mac(tid, w.data(), key.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_inv2(tid, w.data());
     for (int tid = 0; tid < TH; tid++) {
         if (rot) fft_phase_inv1<true>(tid, acc.data(), w.data(), tab); else fft_phase_inv1<false>(tid, acc.data(), w.data(), tab);
     }
@@ -325,24 +325,52 @@ void emul_fft_product(const double *dig, const long long *key, double *out)
     std::vector<cplx> ks(BK_FFT_SPECTRA * FFT_M, cplx{0, 0});
     for (int d = 0; d < 4; d++) fft_key_spectra(key + d * NTT_N, ks.data() + (d * 2 + 0) * 2 * FFT_M, F);   // mo = 0
     std::vector<cplx> w(BrFft::POLYS * FFT_SPEC_CPLX, cplx{0, 0});
-    for (int d = 0; d < 4; d++)
-        for (int n0 = 0; n0 < 64; n0++) {
-            double x[16];
-            for (int j = 0; j < 16; j++) x[j] = dig[d * NTT_N + 64 * j + n0];
-            fft_fwd1(n0, x, w.data() + d * FFT_SPEC_CPLX, tab);
+    // ciphertext 0 of the CTA: the tasks that belong to it, in the kernel's thread maps
+    for (int tid = 0; tid < 128; tid++) {               // fwd1: digit polynomials mi * 2 + 0 / 1, mi = tid / 64
+        const int n0 = tid & 63, mi = tid >> 6;
+        double xa[16], xb[16];
+        for (int j = 0; j < 16; j++) {
+            xa[j] = dig[(mi * 2 + 0) * NTT_N + 64 * j + n0];
+            xb[j] = dig[(mi * 2 + 1) * NTT_N + 64 * j + n0];
         }
-    for (int x = 0; x < 64 * 4; x++) fft_phase_fwd2(x, w.data(), tab);
-    for (int x = 0; x < 64 * 4; x++) fft_phase_fwd3(x, w.data());
-    for (int P = 0; P < FFT_M; P++) fft_mac_point<1>(P, w.data(), ks.data());
-    for (int x = 0; x < 64 * 2; x++) fft_phase_inv3(x, w.data());       // spectra 0, 1: mo = 0, h = 0 / 1
-    for (int x = 0; x < 64 * 2; x++) fft_phase_inv2(x, w.data(), tab);
-    for (int h = 0; h < 2; h++)
-        for (int n0 = 0; n0 < 64; n0++) {
-            double x[16];
-            fft_inv1(n0, w.data() + h * FFT_SPEC_CPLX, tab, x);
-            for (int j = 0; j < 16; j++) out[h * NTT_N + 64 * j + n0] = x[j];
+        fft_fwd1(n0, xa, w.data() + fft_pass1_spec(tid, 0), tab);
+        fft_fwd1(n0, xb, w.data() + fft_pass1_spec(tid, 1), tab);
+    }
+    for (int tid = 0; tid < 128; tid++) fft_phase_fwd2(tid, w.data());
+    for (int tid = 0; tid < 256; tid += 2) fft_phase_mac(tid, w.data(), ks.data());
+    for (int tid = 0; tid < 128; tid++) fft_phase_inv2(tid, w.data());
+    for (int n0 = 0; n0 < 64; n0++) {                   // inv1 of output polynomial mo = 0: both key halves
+        double xl[16], xh[16];
+        fft_inv1(n0, w.data() + fft_pass1_spec(n0, 0), tab, xl);
+        fft_inv1(n0, w.data() + fft_pass1_spec(n0, 1), tab, xh);
+        for (int j = 0; j < 16; j++) {
+            out[0 * NTT_N + 64 * j + n0] = xl[j];
+            out[1 * NTT_N + 64 * j + n0] = xh[j];
         }
+    }
 }
+
+// The shared-memory accesses of the FP64 step (fft_layout.cuh), for the bank-conflict test: the offsets, in 16-byte
+// units from the start of the spectra, that thread tid of a BrFft CTA reads or writes in phase `phase` (0: fwd1 / inv1,
+// 1: fwd2 / inv2, 2: pass 3), one per warp-instruction, in program order.  Returns the count.
+int emul_fft_smem_offsets(int phase, int tid, int *out)
+{
+    int n = 0;
+    if (phase == 0) {
+        for (int k = 0; k < 8; k++)
+            for (int h = 0; h < 2; h++) out[n++] = fft_pass1_pos(tid, h, k);
+    } else if (phase == 1) {
+        const FftPass2 t = fft_pass2_task(tid);
+        for (int m = 0; m < 16; m++) out[n++] = fft_pass2_pos(t, m);
+    } else if (phase == 2) {
+        for (int s = 0; s < 4; s++)
+            for (int i = 0; i < 4; i++) out[n++] = fft_pass3_pos(tid, s, i);
+    }
+    return n;
+}
+// pass 3's key loads: the offset, in complex values from the FP64 part of the row, of key spectrum ks at output k3 of
+// the group of thread tid
+int emul_fft_key_offset(int tid, int ks, int k3) { return fft_key_pos(ks, tid >> 1, k3); }
 
 // The programmable bootstrap's index functions (lut_index.cuh): the rounded mod-switch, the initial accumulator
 // polynomial X^(2N - barb) * tv, and the sample extracted at index j from an accumulator (2, 1024).

@@ -306,13 +306,13 @@ __global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ 
         fft_fwd1(n0, hi, spec[1], tab);
     }
     __syncthreads();
-    for (int h = 0; h < 2; h++) fft_fwd2(n0 >> 3, n0 & 7, spec[h], tab);
+    fft_fwd2(n0 & 7, (n0 >> 3) & 3, spec[n0 >> 5]);      // 2 x 32 tasks (h, n2, k1)
     __syncthreads();
-    for (int h = 0; h < 2; h++) fft_fwd3(n0 >> 3, n0 & 7, spec[h]);
+    for (int t = n0; t < 2 * FFT_M / 4; t += 64) fft_fwd3(t & 127, spec[t >> 7]);
     __syncthreads();
-    cplx *out = reinterpret_cast<cplx *>(bk_int + row * BK_ROW_U64 + BK_NTT_U64) + (size_t)m * 2 * FFT_M;
+    cplx *out = reinterpret_cast<cplx *>(bk_int + row * BK_ROW_U64 + BK_NTT_U64);
     for (int P = n0; P < FFT_M; P += 64)
-        for (int h = 0; h < 2; h++) out[h * FFT_M + P] = spec[h][fft_pad(P)];
+        for (int h = 0; h < 2; h++) out[fft_key_pos(m * 2 + h, P & 127, P >> 7)] = spec[h][fft_pass3_x(fft_pass3_group(P & 127), P >> 7)];
 }
 
 // mod-switch to [0, 2N) (numeric_functions_gpu.py:55-71)
@@ -532,29 +532,37 @@ NB_D void br2_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *
     }
 }
 
-// The FP64 step (br_phases.cuh: FP64 step): the same seven barrier-separated phases as br2_step, on spectra of 512
-// complex doubles instead of NTT work polynomials; bk_row: the whole engine key row (its FP64 part is read)
-template <bool ROTATE, class Cfg>
-NB_D void br_fft_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *rot, int tid, const cplx *__restrict__ tab)
+// The thread index, read again (volatile, so not hoisted out of the step loop): every address of the FP64 step's phases
+// is a per-thread base plus constants, and without this the compiler keeps all five phases' bases live across the
+// whole loop -- about 70 bytes more spill at 128 registers.
+NB_D int fft_step_tid()
 {
+    int t;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    return t;
+}
+
+// The FP64 step (br_phases.cuh: FP64 step): five barrier-separated phases on spectra of 512 complex doubles, one task
+// per thread in each; bk_row: the whole engine key row (its FP64 part is read)
+template <bool ROTATE, class Cfg>
+NB_D void br_fft_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *rot, int /* tid */, const cplx *__restrict__ tab)
+{
+    static_assert(Cfg::CT == FFT_CT && Cfg::THREADS == 256, "the FP64 step's thread maps (fft_layout.cuh)");
     cplx *spec = reinterpret_cast<cplx *>(s.w);
-    fft_phase_fwd1<ROTATE>(tid, s.acc, spec, tab, rot);          // 128 CT tasks: (ct, mi, n0), both digits
+    int tid = fft_step_tid();
+    fft_phase_fwd1<ROTATE>(tid, s.acc, spec, tab, rot);          // (ct, mi, n0), both digits
     __syncthreads();
-#pragma unroll 1
-    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_fwd2(x, spec, tab);
+    tid = fft_step_tid();
+    fft_phase_fwd2(tid, spec);                              // (ct, n2, s, k1): DFT16, W64 twiddles
     __syncthreads();
-#pragma unroll 1
-    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_fwd3(x, spec);
+    tid = fft_step_tid();
+    fft_phase_mac(tid, spec, reinterpret_cast<const cplx *>(bk_row + BK_NTT_U64));   // (j, ct): DFT4, MAC, inverse DFT4
     __syncthreads();
-    fft_phase_mac<Cfg::CT, Cfg::THREADS>(tid, spec, reinterpret_cast<const cplx *>(bk_row + BK_NTT_U64));
+    tid = fft_step_tid();
+    fft_phase_inv2(tid, spec);                              // (ct, n2, s, k1)
     __syncthreads();
-#pragma unroll 1
-    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_inv3(x, spec);
-    __syncthreads();
-#pragma unroll 1
-    for (int x = tid; x < 256 * Cfg::CT; x += Cfg::THREADS) fft_phase_inv2(x, spec, tab);
-    __syncthreads();
-    fft_phase_inv1<ROTATE>(tid, s.acc, spec, tab);                // 128 CT tasks: (ct, mo, n0), both key halves
+    tid = fft_step_tid();
+    fft_phase_inv1<ROTATE>(tid, s.acc, spec, tab);                // (ct, mo, n0), both key halves
 }
 
 NB_D unsigned ld_acquire_u32(const unsigned *p)

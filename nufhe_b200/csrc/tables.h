@@ -59,8 +59,6 @@ struct FftTables {
         }
         for (int n0 = 0; n0 < 64; n0++)
             for (int k = 0; k < 8; k++) tab[FFT_TAB_TW1 + n0 * 8 + k] = e(-(long double)((n0 * k) % 512) / 512);
-        for (int n1 = 0; n1 < 8; n1++)
-            for (int k = 0; k < 8; k++) tab[FFT_TAB_TW2 + n1 * 8 + k] = e(-(long double)((n1 * k) % 64) / 64);
     }
 };
 

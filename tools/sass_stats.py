@@ -12,8 +12,10 @@ after the shape) and a lookup-table one (`...Lb1E`, kernels.cuh: LUT); give enou
 
 Each SASS instruction is attributed (through nvdisasm's inline chains, the library is built with -lineinfo)
 to the line of `br2_step` (or `br_fft_step`) in kernels.cuh that called it, i.e. to a phase.  Counts are static: fwd1 / fwd2 /
-fwd3 are multiplied by their two sweeps per step (the `it` loops are not unrolled), the MAC by its two row
-iterations, and code inside the warp-uniform `switch (g)` of fwd2 / inv2 counts a quarter -- see `per step`.
+fwd3 of the NTT step are multiplied by their two sweeps per step (the `it` loops are not unrolled), the MAC by its
+two row iterations, and code inside the warp-uniform `switch (g)` of fwd2 / inv2 counts a quarter; the FP64 step
+runs each of its five phases once per thread, with a real loop of four iterations inside pass 3
+-- see `per step`.
 """
 import argparse
 import collections
@@ -51,9 +53,9 @@ def pipe_of(op):
 
 COST = {'IMAD.WIDE(+R64)': 4, 'IMAD.WIDE(+RZ)': 4}
 STEP_MULT = {'phase_fwd1': 2, 'phase_fwd2': 2, 'phase_fwd3': 2, 'phase_mac': 2,
-             # the FP64 step (2 ciphertexts on 256 threads): two tasks per thread in the four middle passes and two MAC
-             # points (loops not unrolled); fwd1's digit loop is weighted by `twice_lines`
-             'fft_phase_fwd2': 2, 'fft_phase_fwd3': 2, 'fft_phase_inv3': 2, 'fft_phase_inv2': 2, 'fft_phase_mac': 2}
+             # the FP64 step (2 ciphertexts on 256 threads): one task per thread in each of its five phases; pass 3's
+             # output-spectrum loop (fft_phase_mac) is weighted by `four_lines`
+             'fft_phase_fwd1': 1, 'fft_phase_fwd2': 1, 'fft_phase_mac': 1, 'fft_phase_inv2': 1, 'fft_phase_inv1': 1}
 
 
 def instruction_form(op, rest):
@@ -141,18 +143,24 @@ def main():
     bpath = os.path.join(ROOT, 'nufhe_b200', 'csrc', 'br_phases.cuh')
     case_lines = {i for i, l in enumerate(open(bpath).read().splitlines(), 1) if re.match(r'\s*(case \d+|default):', l)}
 
-    # lines of br_phases.cuh inside the digit loop of phase_fwd1_both_digits (a real loop, two iterations per step)
-    twice_lines = set()
+    # lines of br_phases.cuh inside the digit loop of phase_fwd1_both_digits (a real loop, two iterations per step),
+    # and inside the output-spectrum loop of the FP64 step's pass 3 (four iterations)
     bsrc0 = open(bpath).read().splitlines()
-    for i, l in enumerate(bsrc0, 1):
-        if 'for (int j = 0; j < 2; j++)' in l:
-            depth, j = 0, i
-            while True:
-                depth += bsrc0[j - 1].count('{') - bsrc0[j - 1].count('}')
-                twice_lines.add(j)
-                if depth <= 0 and j > i:
-                    break
-                j += 1
+
+    def loop_lines(header):
+        lines = set()
+        for i, l in enumerate(bsrc0, 1):
+            if header in l:
+                depth, j = 0, i
+                while True:
+                    depth += bsrc0[j - 1].count('{') - bsrc0[j - 1].count('}')
+                    lines.add(j)
+                    if depth <= 0 and j > i:
+                        break
+                    j += 1
+        return lines
+    twice_lines = loop_lines('for (int j = 0; j < 2; j++)')
+    four_lines = loop_lines('for (int s = 0; s < 4; s++)')
 
     # lines of br_phases.cuh inside an `if (canon_needed(...)) { ... }` block: the rare path of the deferred
     # canonicalisation (taken with probability ~2^-28 per task) -- not part of the executed step
@@ -219,6 +227,8 @@ def main():
         w = 0.25 if any(path.endswith('br_phases.cuh') and line in case_lines for path, line in chain) else 1
         if any(path.endswith('br_phases.cuh') and line in twice_lines for path, line in chain):
             w *= 2
+        if any(path.endswith('br_phases.cuh') and line in four_lines for path, line in chain):
+            w *= 4
         if any(path.endswith('br_phases.cuh') and line in rare_lines for path, line in chain):
             counts['rare:' + phase][pipe] += w
             continue
