@@ -218,6 +218,35 @@ int nb_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *key, uint64_t *ou
                size_t groups);
 int nb_pack_finish(nb_ctx *ctx, const int32_t *c, const int32_t *b, int mask_size, uint16_t *out, size_t batch);
 
+/* ---- tree-based programmable bootstrapping (DESIGN.md section 13; no reference counterpart).  A lookup table on D
+ * digits is evaluated one digit at a time: the LWE outputs of one level become GLWE test vectors under the bootstrap
+ * key's GLWE key S (k polynomials of N = 1024), which the next level blind-rotates by the next digit.
+ * The tree key T: n t = 2 n rows, row i t + j a GLWE encryption under S of the constant s_i g_j (g = 2^24, 2^16), as
+ * masks (n, t, k, N) and bodies (n, t, N) int32.
+ * nb_tree_prepare lays T ((n t) x (k+1) N, rows padded with zeros to kpad = n t rounded up to 32) into 4 byte planes,
+ *     plane p column-major: byte p of T[row][col] at ((p * (k+1) N + col) * kpad + row); `planes` holds
+ *     nb_tree_planes_bytes(n, k) bytes (0 for sizes the library rejects).
+ * nb_tree_keyswitch: a (R, n) int32 LWE masks -> out (R, k+1, N) int32, V = sum_ij d_ij(a_r) T_ij mod 2^32 with the
+ *     signed digits d_ij of nb_pack_digits (round_16(a_i) = d_i0 g_0 + d_i1 g_1), one exact s8 x u8 -> s32
+ *     tensor-core GEMM (mma.sync m16n8k32) per byte plane.
+ * nb_tree_assemble: v (count, 2^bits, k+1, N) and the LWE bodies b (count, 2^bits) -> tv (count, k+1, N),
+ *     tv_u = sum_m X^(o_m) (1 + X + ... + X^(box - 1)) G_m,u (negacyclic, mod 2^32), box = N >> bits,
+ *     o_m = m box - box / 2, G_m,u = -v_m,u for u < k and b_m X^0 - v_m,k for u = k.
+ * NB_EINVAL for a NULL pointer, n = 0 or kpad * 128 * 255 >= 2^31 (the sums would not be exact), a mask size outside
+ * 1..16 and bits outside 1..2; rows / count = 0 is a no-op. */
+size_t nb_tree_planes_bytes(size_t n, int mask_size);
+int nb_tree_prepare(nb_ctx *ctx, const int32_t *masks, const int32_t *body, size_t n, int mask_size, uint8_t *planes);
+int nb_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *planes, size_t n, int mask_size, int32_t *out,
+                      size_t rows);
+int nb_tree_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, int mask_size, int32_t *tv,
+                     size_t count);
+/* The programmable bootstrap of one LWE input (in_a (B, n), in_b (B,)) with a per-ciphertext GLWE test vector
+ * tv (B, 2, 1024) (k = 1, the fused kernel's parameter set): the accumulator starts as X^(2N - barb) * (tv_0, tv_1)
+ * instead of (0, X^(2N - barb) * tv), L = 0.  Output: out_a (B, 1024), out_b (B,).  NB_EINVAL for a NULL pointer;
+ * batch = 0 is a no-op. */
+int nb_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
+                                  const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch);
+
 #ifdef __cplusplus
 }
 #endif

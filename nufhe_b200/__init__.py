@@ -57,6 +57,11 @@ from .packing import (
     make_packing_keys,
     pack,
     )
+from .tree_lut import (
+    NuFHETreeKey,
+    TreeLookupTable,
+    lut_tree,
+    )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

@@ -59,8 +59,15 @@ SIGNATURES = {
     'nb_pack_digits': [_vp, _vp, _sz, _vp, _sz],
     'nb_ntt_mac': [_vp, _vp, _vp, _vp, _sz, _sz, _sz],
     'nb_pack_finish': [_vp, _vp, _vp, _int, _vp, _sz],
+    'nb_tree_planes_bytes': [_sz, _int],
+    'nb_tree_prepare': [_vp, _vp, _vp, _sz, _int, _vp],
+    'nb_tree_keyswitch': [_vp, _vp, _vp, _sz, _int, _vp, _sz],
+    'nb_tree_assemble': [_vp, _vp, _vp, _int, _int, _vp, _sz],
+    'nb_bootstrap_glwe_lut_extract': [_vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz],
 }
-_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p, 'nb_build_info': ctypes.c_char_p}
+_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
+             'nb_tree_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p,
+             'nb_build_info': ctypes.c_char_p}
 
 _lib = None
 

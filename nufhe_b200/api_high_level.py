@@ -8,6 +8,7 @@ from .compressed import CompressedLweSampleArray, CompressedCloudKey
 from .public_key import NuFHEPublicKey
 from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
                       decrypt_packed, decrypt_packed_int)
+from .tree_lut import NuFHETreeKey, TreeLookupTable, lut_tree
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -100,12 +101,16 @@ class Context:
     def make_secret_key(self, **params):
         return NuFHESecretKey.from_rng(self.thread, NuFHEParameters(**params), self.rng)
 
-    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False):
+    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False):
         """compressed=True returns a CompressedCloudKey (about 12 times smaller to store or send); its `decompress()`
-        gives the NuFHECloudKey that make_virtual_machine takes."""
-        if compressed:
-            return CompressedCloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
-        return NuFHECloudKey.from_rng(self.thread, secret_key.params, self.rng, secret_key)
+        gives the NuFHECloudKey that make_virtual_machine takes.  tree_key=True returns (cloud key, NuFHETreeKey), the
+        key of VirtualMachine.lut_tree; its draws follow all of the cloud key's, so the cloud key is the same either
+        way."""
+        cls = CompressedCloudKey if compressed else NuFHECloudKey
+        cloud_key, tgsw_key = cls.from_rng_with_tgsw_key(self.thread, secret_key.params, self.rng, secret_key)
+        if not tree_key:
+            return cloud_key
+        return cloud_key, NuFHETreeKey.from_secret_key(self.thread, self.rng, secret_key, tgsw_key)
 
     def make_public_key(self, secret_key: NuFHESecretKey):
         """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
@@ -181,6 +186,11 @@ class Context:
             return NuFHEPackingSecretKey.loads(file_or_bytestring, self.thread)
         return NuFHEPackingSecretKey.load(file_or_bytestring, self.thread)
 
+    def load_tree_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHETreeKey.loads(file_or_bytestring, self.thread)
+        return NuFHETreeKey.load(file_or_bytestring, self.thread)
+
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
             return NuFHESecretKey.loads(file_or_bytestring, self.thread)
@@ -243,6 +253,31 @@ class VirtualMachine:
         bootstrap_lut(self.thread, dest, self.cloud_key.bootstrap_key, self.cloud_key.keyswitch_key, table, x, y,
                       shift, perf_params=self.perf_params)
         return dest if table.outputs > 1 else dest[0]
+
+    def make_tree_lut(self, tables, bits, digits, out='int'):
+        """A lookup table on `digits` encrypted digits of `bits` bits (nufhe_b200/tree_lut.py: TreeLookupTable):
+        tables of shape (F,) + (2^bits,) * digits, or (2^bits,) * digits for one function, indexed
+        [f, d_{D-1}, ..., d_0].  Raises ValueError for bits outside {1, 2} and for D < 2 or above what the noise
+        allows (tree_lut.max_digits: 4 at bits = 2)."""
+        return TreeLookupTable(self.thread, self.params, tables, bits, digits, out=out)
+
+    def lut_tree(self, tree_key, table, digits, dest=None):
+        """f(d_{D-1}, ..., d_0) for the digit ciphertexts `digits` (highest first): one ciphertext, or a list of F for a
+        table of F functions.  D levels of bootstraps; `tree_key` is the NuFHETreeKey made with this VM's cloud key
+        (TypeError for anything else).  To record it with `capture`, reserve table.reserve_batch(batch)."""
+        if not isinstance(tree_key, NuFHETreeKey):
+            raise TypeError('lut_tree needs a NuFHETreeKey (ctx.make_cloud_key(sk, tree_key=True)), got %s'
+                            % type(tree_key).__name__)
+        if tree_key.params != self.params:
+            raise ValueError('the tree key was made for other parameters than this virtual machine')
+        if dest is None:
+            shape = result_shape(*[get_shape(d) for d in digits])
+            dest = [self.empty_ciphertext(shape) for _ in range(table.functions)]
+        elif isinstance(dest, LweSampleArray):
+            dest = [dest]
+        lut_tree(self.thread, dest, self.cloud_key.bootstrap_key, self.cloud_key.keyswitch_key, tree_key, table,
+                 digits, perf_params=self.perf_params)
+        return dest[0] if table.single else dest
 
     def int_add(self, x, y, dest=None):
         """x + y of two integer ciphertexts without a bootstrap (the caller keeps the sum below 2^bits)."""

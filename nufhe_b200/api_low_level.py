@@ -103,13 +103,19 @@ class NuFHECloudKey:
     @classmethod
     def from_rng(cls, thr, params: NuFHEParameters, rng, secret_key: NuFHESecretKey,
                  perf_params: PerformanceParametersForDevice = None):
+        return cls.from_rng_with_tgsw_key(thr, params, rng, secret_key, perf_params)[0]
+
+    @classmethod
+    def from_rng_with_tgsw_key(cls, thr, params: NuFHEParameters, rng, secret_key: NuFHESecretKey,
+                               perf_params: PerformanceParametersForDevice = None):
+        """(cloud key, TGswKey): the TGSW key, which from_rng discards, is what a tree key is made with."""
         if perf_params is None:
             perf_params = PerformanceParameters(params).for_device(thr.device_params)
         tgsw_key = TGswKey.from_rng(thr, params.tgsw_params, rng)
         bk = BootstrapKey.from_rng(thr, rng, secret_key.lwe_key, tgsw_key, perf_params)
         ks = LweKeyswitchKey.from_tgsw_key(
             thr, rng, params.ks_decomp_length, params.ks_log2_base, secret_key.lwe_key, tgsw_key)
-        return cls(params, bk, ks)
+        return cls(params, bk, ks), tgsw_key
 
     def dump(self, file_obj):
         pickle.dump(self.params, file_obj)

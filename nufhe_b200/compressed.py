@@ -161,6 +161,11 @@ class CompressedCloudKey:
     @classmethod
     def from_rng(cls, thr, params, rng, secret_key):
         """Key generation in the order: TGSW key, seed, bootstrap-key body noises, key-switch noises_b."""
+        return cls.from_rng_with_tgsw_key(thr, params, rng, secret_key)[0]
+
+    @classmethod
+    def from_rng_with_tgsw_key(cls, thr, params, rng, secret_key):
+        """(compressed cloud key, TGswKey), as NuFHECloudKey.from_rng_with_tgsw_key."""
         lwe_key = secret_key.lwe_key
         tgsw_key = TGswKey.from_rng(thr, params.tgsw_params, rng)
         seed = draw_seed(rng)
@@ -184,7 +189,7 @@ class CompressedCloudKey:
         ks = LweSampleArray.empty(thr, lwe_key.params, (in_size, t, base))
         make_lwe_keyswitch_key(thr, ks, in_key.key, lwe_key.key, _ks_masks(thr, seed, in_size, t, base, n_out),
                                noises_b, params.ks_log2_base, noise)
-        return cls(params, seed, bk_body, _variance(tl.min_noise), ks.b.contiguous(), _variance(noise))
+        return cls(params, seed, bk_body, _variance(tl.min_noise), ks.b.contiguous(), _variance(noise)), tgsw_key
 
     def decompress(self, thr):
         """The NuFHECloudKey: masks regenerated on the device, the bootstrap key transformed as at key generation."""

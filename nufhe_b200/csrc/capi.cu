@@ -536,6 +536,19 @@ int nb_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *i
     return launch_blind_rotate(ctx, p);
 }
 
+int nb_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
+                                  const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
+    if (!ctx || !in_a || !in_b || !tv || !bk_int || !out_a || !out_b)
+        return fail(ctx, NB_EINVAL, "nb_bootstrap_glwe_lut_extract: null argument");
+    BlindRotateArgs p{};
+    p.in1_a = in_a; p.in1_b = in_b; p.c = 0; p.s1 = 1; p.s2 = 0;
+    p.tv = tv; p.tv_stride = 2 * (size_t)NTT_N; p.log2_outputs = 0;
+    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
+    return launch_blind_rotate(ctx, p);
+}
+
 int nb_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
                           const int32_t *a2_b, int32_t a_c, int32_t a_s1, int32_t a_s2, const int32_t *b1_a,
                           const int32_t *b1_b, const int32_t *b2_a, const int32_t *b2_b, int32_t b_c, int32_t b_s1,
@@ -863,6 +876,69 @@ int nb_pack_finish(nb_ctx *ctx, const int32_t *c, const int32_t *b, int mask_siz
     const size_t total = (batch + PACK_N - 1) / PACK_N * (size_t)(mask_size + 1) * PACK_N;
     pack_finish_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(c, b, (u32)mask_size, (u64)batch, out, (u64)total);
     return launch_check(ctx, "pack_finish_kernel");
+}
+
+size_t nb_tree_planes_bytes(size_t n, int mask_size)
+{
+    if (n == 0 || n > (1u << 20) || mask_size < 1 || mask_size > 16) return 0;
+    return 4 * (size_t)tree_k_padded((u32)n) * (size_t)(mask_size + 1) * PACK_N;
+}
+
+// n t digit rows: every plane sum, at most kpad * 128 * 255, must stay below 2^31 for the s32 accumulators to be exact
+static int tree_check_shape(nb_ctx *ctx, size_t n, int mask_size, const char *what)
+{
+    if (n == 0 || n > (1u << 20) || (uint64_t)tree_k_padded((u32)n) * 128 * 255 >= (1ull << 31))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": n t (padded to 32) * 128 * 255 must be below 2^31");
+    if (mask_size < 1 || mask_size > 16) return fail(ctx, NB_EINVAL, std::string(what) + ": bad mask size");
+    return NB_OK;
+}
+
+int nb_tree_prepare(nb_ctx *ctx, const int32_t *masks, const int32_t *body, size_t n, int mask_size, uint8_t *planes)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!masks || !body || !planes) return fail(ctx, NB_EINVAL, "nb_tree_prepare: null argument");
+    NB_TRY(tree_check_shape(ctx, n, mask_size, "nb_tree_prepare"));
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:tree_prepare");
+    const size_t quads = (size_t)(mask_size + 1) * PACK_N * (tree_k_padded((u32)n) / 4);
+    const size_t blocks = (quads + 255) / 256, cap = (size_t)ctx->sm_count * 16;
+    tree_prepare_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(masks, body, (u32)n,
+                                                                                      (u32)mask_size, planes);
+    return launch_check(ctx, "tree_prepare_kernel");
+}
+
+int nb_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *planes, size_t n, int mask_size, int32_t *out,
+                      size_t rows)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!a || !planes || !out) return fail(ctx, NB_EINVAL, "nb_tree_keyswitch: null argument");
+    NB_TRY(tree_check_shape(ctx, n, mask_size, "nb_tree_keyswitch"));
+    if (rows == 0) return NB_OK;
+    const size_t rows_per_cta = (size_t)TREE_WARPS * TREE_MTILES * 16;
+    const size_t ctas = (rows + rows_per_cta - 1) / rows_per_cta;
+    if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_tree_keyswitch: too many rows");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:tree_keyswitch");
+    const u32 cols = (u32)(mask_size + 1) * PACK_N;
+    const dim3 grid((unsigned)ctas, cols / (8 * TREE_NTILES));
+    tree_keyswitch_kernel<<<grid, TREE_WARPS * 32, 0, ctx->stream>>>(a, planes, (u32)n, cols, out, (u64)rows);
+    return launch_check(ctx, "tree_keyswitch_kernel");
+}
+
+int nb_tree_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, int mask_size, int32_t *tv,
+                     size_t count)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!v || !b || !tv) return fail(ctx, NB_EINVAL, "nb_tree_assemble: null argument");
+    if (bits < 1 || bits > 2) return fail(ctx, NB_EINVAL, "nb_tree_assemble: bits must be 1 or 2");
+    if (mask_size < 1 || mask_size > 16) return fail(ctx, NB_EINVAL, "nb_tree_assemble: bad mask size");
+    if (count == 0) return NB_OK;
+    const size_t ctas = count * (size_t)(mask_size + 1);
+    if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_tree_assemble: too many test vectors");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:tree_assemble");
+    tree_assemble_kernel<<<(unsigned)ctas, TREE_ASM_THREADS, 0, ctx->stream>>>(v, b, bits, (u32)mask_size, tv);
+    return launch_check(ctx, "tree_assemble_kernel");
 }
 
 }  // extern "C"

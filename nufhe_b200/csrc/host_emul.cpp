@@ -10,6 +10,7 @@
 #include "chacha.cuh"
 #include "pk_layout.cuh"
 #include "pack_layout.cuh"
+#include "tree_layout.cuh"
 
 using namespace nb;
 
@@ -488,6 +489,117 @@ void emul_pack_digits(const i32 *a, size_t count, i32 *out)
 void emul_pack_round16(const u32 *x, size_t count, uint16_t *out) { for (size_t i = 0; i < count; i++) out[i] = pack_round16(x[i]); }
 void emul_pack_unround16(const uint16_t *x, size_t count, u32 *out) { for (size_t i = 0; i < count; i++) out[i] = pack_unround16(x[i]); }
 void emul_pack_slot(u64 c, u64 *group, u32 *slot) { *group = pack_group(c); *slot = pack_slot(c); }
+
+// Tree-based programmable bootstrapping (tree_layout.cuh).  emul_tree_keyswitch: tree_prepare_kernel's planes, then
+// tree_keyswitch_kernel's tile loop with a scalar model of mma.sync.m16n8k32.row.col.s32.s8.u8.s32 that places each
+// register byte by the PTX ISA's fragment layout (A bytes signed, B bytes unsigned).
+static void mma_m16n8k32_s8u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4])
+{
+    i32 A[16][32];
+    u32 B[32][8];
+    for (int l = 0; l < 32; l++) {
+        const int g = l >> 2, t = l & 3;
+        for (int j = 0; j < 16; j++) {
+            const int row = g + ((j < 4 || (j >= 8 && j < 12)) ? 0 : 8), k = 4 * t + (j & 3) + (j >= 8 ? 16 : 0);
+            A[row][k] = (int8_t)((a[l][j >> 2] >> (8 * (j & 3))) & 0xFF);
+        }
+        for (int j = 0; j < 8; j++) {
+            const int k = 4 * t + (j & 3) + (j >= 4 ? 16 : 0);
+            B[k][g] = (b[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
+        }
+    }
+    i32 D[16][8] = {};
+    for (int r = 0; r < 16; r++) {
+        bool any = false;
+        for (int k = 0; k < 32; k++) any |= A[r][k] != 0;
+        if (!any) continue;
+        for (int c2 = 0; c2 < 8; c2++) {
+            i32 s = 0;
+            for (int k = 0; k < 32; k++) s += A[r][k] * (i32)B[k][c2];
+            D[r][c2] = s;
+        }
+    }
+    for (int l = 0; l < 32; l++) {
+        const int g = l >> 2, t = l & 3;
+        for (int i = 0; i < 4; i++) c[l][i] += D[g + (i >= 2 ? 8 : 0)][2 * t + (i & 1)];
+    }
+}
+
+void emul_tree_keyswitch(const i32 *a, const i32 *masks, const i32 *body, size_t n, int k, i32 *out, size_t rows)
+{
+    const u32 kpad = tree_k_padded((u32)n), cols = (u32)(k + 1) * PACK_N, ksteps = kpad >> 5;
+    std::vector<uint8_t> planes((size_t)4 * kpad * cols);
+    for (u32 col = 0; col < cols; col++)
+        for (u32 kk = 0; kk < kpad; kk++) {
+            const u32 w = tree_key_word(masks, body, (u32)n, (u32)k, kk, col);
+            for (int p = 0; p < 4; p++) planes[tree_plane_offset(p, col, kk, kpad, cols)] = (uint8_t)(w >> (8 * p));
+        }
+    auto load32 = [&](u64 off) { u32 v; memcpy(&v, planes.data() + off, 4); return v; };
+    const u64 plane_stride = tree_plane_offset(1, 0, 0, kpad, cols);
+    std::vector<i32> acc((size_t)4 * TREE_MTILES * 32 * 4);
+    auto A = [&](int p, int mt) { return reinterpret_cast<i32 (*)[4]>(&acc[((size_t)p * TREE_MTILES + mt) * 128]); };
+    for (u64 row0 = 0; row0 < rows; row0 += 16 * TREE_MTILES)      // one warp
+        for (u32 col0 = 0; col0 < cols; col0 += 8) {                 // one n8 tile
+            std::fill(acc.begin(), acc.end(), 0);
+            for (u32 ks = 0; ks < ksteps; ks++) {
+                u32 bf[4][32][2], af[TREE_MTILES][32][4];
+                for (int l = 0; l < 32; l++) {
+                    const int g = l >> 2, t = l & 3;
+                    const u64 bcol = tree_plane_offset(0, col0 + g, 0, kpad, cols);
+                    for (int p = 0; p < 4; p++)
+                        for (int h = 0; h < 2; h++) bf[p][l][h] = load32(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h));
+                    const u32 i0 = 16 * ks + 4 * t;
+                    for (int mt = 0; mt < TREE_MTILES; mt++) {
+                        i32 w[2][4];
+                        for (int hr = 0; hr < 2; hr++) {
+                            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
+                            for (int q = 0; q < 4; q++) w[hr][q] = (r < rows && i0 + q < n) ? a[r * n + i0 + q] : 0;
+                        }
+                        af[mt][l][0] = tree_a_frag(w[0][0], w[0][1]);
+                        af[mt][l][1] = tree_a_frag(w[1][0], w[1][1]);
+                        af[mt][l][2] = tree_a_frag(w[0][2], w[0][3]);
+                        af[mt][l][3] = tree_a_frag(w[1][2], w[1][3]);
+                    }
+                }
+                for (int mt = 0; mt < TREE_MTILES; mt++)
+                    for (int p = 0; p < 4; p++) mma_m16n8k32_s8u8(af[mt], bf[p], A(p, mt));
+            }
+            for (int l = 0; l < 32; l++) {
+                const int g = l >> 2, t = l & 3;
+                for (int mt = 0; mt < TREE_MTILES; mt++)
+                    for (int i = 0; i < 4; i++) {
+                        const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
+                        if (row >= rows) continue;
+                        const u32 col = col0 + pk_acc_col(t, i);
+                        out[row * cols + col] = (i32)pk_combine(A(0, mt)[l][i], A(1, mt)[l][i], A(2, mt)[l][i], A(3, mt)[l][i]);
+                    }
+            }
+        }
+}
+
+// emul_tree_assemble: tree_assemble_kernel's arithmetic, one (test vector, polynomial) after the other, with a serial
+// prefix sum
+void emul_tree_assemble(const i32 *v, const i32 *b, int bits, int k, i32 *tv, size_t count)
+{
+    const int M = 1 << bits;
+    std::vector<u32> z(PACK_N), ps(PACK_N + 1);
+    for (size_t t = 0; t < count; t++)
+        for (int u = 0; u <= k; u++) {
+            for (int x = 0; x < PACK_N; x++) {
+                u32 s = 0;
+                for (int m = 0; m < M; m++) {
+                    bool neg;
+                    const int d = tree_shift_index(tree_offset(m, bits), x, &neg);
+                    const u32 gv = tree_glwe_coef(v + ((t * M + m) * (k + 1) + u) * PACK_N, b[t * M + m], u == k, d);
+                    s += neg ? 0u - gv : gv;
+                }
+                z[x] = s;
+            }
+            ps[0] = 0;
+            for (int x = 0; x < PACK_N; x++) ps[x + 1] = ps[x] + z[x];
+            for (int x = 0; x < PACK_N; x++) tv[(t * (k + 1) + u) * PACK_N + x] = (i32)tree_window_coef(ps.data(), PACK_N >> bits, x);
+        }
+}
 
 void emul_ff_shl_var(const u64 *in, const int *s, u64 *out, size_t n)
 { for (size_t i = 0; i < n; i++) out[i] = ff_shl_var(in[i], s[i]); }

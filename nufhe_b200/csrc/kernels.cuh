@@ -25,6 +25,7 @@
 #include "chacha.cuh"
 #include "pk_layout.cuh"
 #include "pack_layout.cuh"
+#include "tree_layout.cuh"
 
 namespace nb {
 
@@ -360,7 +361,7 @@ struct BlindRotateArgs {
     // are rounded to multiples of 2^log2_outputs, and samples are extracted at indices j = 0 .. 2^log2_outputs - 1
     // into rows c * 2^log2_outputs + j of out_a / out_b (lut_index.cuh)
     const i32 *tv;
-    size_t tv_stride;       // 0: one test vector for the batch, NTT_N: one per ciphertext
+    size_t tv_stride;       // 0: one test vector for the batch, NTT_N: one per ciphertext, 2 NTT_N: one GLWE per ciphertext
     int log2_outputs;
 };
 constexpr int BR_SCHED_HEADER = 32;      // the ticket counter has a 128-byte line of its own
@@ -425,11 +426,14 @@ NB_D int lut_rotation(const BlindRotateArgs &p, size_t c, int i)
     return modswitch_lut((i32)xa, p.log2_outputs);
 }
 
+// tv_stride 2N: one GLWE test vector (mask, body) per ciphertext (nb_bootstrap_glwe_lut_extract), whose mask
+// polynomial starts the accumulator's mask instead of 0
 NB_D i32 lut_initial_acc(const BlindRotateArgs &p, size_t c, int mi, int x)
 {
-    if (mi == 0) return 0;
+    const bool glwe = p.tv_stride == 2 * NTT_N;
+    if (mi == 0 && !glwe) return 0;
     const u32 xb = (u32)p.c + (u32)p.s1 * (u32)p.in1_b[c] + (p.in2_b ? (u32)p.s2 * (u32)p.in2_b[c] : 0u);
-    return lut_head_coef(p.tv + c * p.tv_stride, modswitch_lut((i32)xb, p.log2_outputs), x);
+    return lut_head_coef(p.tv + c * p.tv_stride + (glwe ? mi * NTT_N : 0), modswitch_lut((i32)xb, p.log2_outputs), x);
 }
 
 template <bool LUT> NB_D int br_rotation(const BlindRotateArgs &p, size_t c, int i)
@@ -1610,6 +1614,156 @@ __global__ void pack_finish_kernel(const i32 *__restrict__ c, const i32 *__restr
         if (u == k && cidx < batch) v += (u32)b[cidx];
         out[i] = pack_round16(v);
     }
+}
+
+// ---- tree-based programmable bootstrapping (DESIGN.md section 13; layout and index arithmetic in tree_layout.cuh).
+// nb_tree_prepare: the 4 byte planes of the tree key T (n t rows padded to kpad, (k+1) N columns), one thread per
+// (column, 4 consecutive rows): it reads 4 key words and writes one 32-bit word to each plane.
+__global__ void tree_prepare_kernel(const i32 *__restrict__ masks, const i32 *__restrict__ body, u32 n, u32 k,
+                                    uint8_t *__restrict__ planes)
+{
+    const u32 kpad = tree_k_padded(n), cols = (k + 1) * PACK_N, quads = kpad >> 2;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < (u64)cols * quads; i += (u64)gridDim.x * blockDim.x) {
+        const u32 col = (u32)(i / quads), kk = (u32)(i % quads) * 4;
+        u32 w[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) w[j] = tree_key_word(masks, body, n, k, kk + j, col);
+#pragma unroll
+        for (int p = 0; p < 4; p++) {
+            u32 v = 0;
+#pragma unroll
+            for (int j = 0; j < 4; j++) v |= ((w[j] >> (8 * p)) & 0xFFu) << (8 * j);
+            *(u32 *)(planes + tree_plane_offset(p, col, kk, kpad, cols)) = v;
+        }
+    }
+}
+
+__device__ __forceinline__ void tree_mma(i32 *c, const u32 *a, const u32 *b)
+{
+    asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// nb_tree_keyswitch: V (rows x cols) = D (rows x kpad, signed digits of the masks) x T (4 byte planes), the pk_encrypt
+// tiling with TREE_NTILES n8 tiles per CTA: per k-step of 32 a lane reads 4 mask words of each of its 2 * TREE_MTILES
+// rows, forms their digits in registers (tree_a_frag) and issues every plane and column tile with the same A fragment,
+// so the four plane sums of one output word sit in one thread.  Every plane sum is at most kpad * 128 * 255 < 2^31.
+__global__ void __launch_bounds__(TREE_WARPS * 32) tree_keyswitch_kernel(
+    const i32 *__restrict__ a, const uint8_t *__restrict__ planes, u32 n, u32 cols, i32 *__restrict__ out, u64 rows)
+{
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const u64 row0 = ((u64)blockIdx.x * TREE_WARPS + (threadIdx.x >> 5)) * (16 * TREE_MTILES);
+    if (row0 >= rows) return;
+    const u32 kpad = tree_k_padded(n), ksteps = kpad >> 5, col0 = blockIdx.y * (8 * TREE_NTILES);
+    const u64 plane_stride = tree_plane_offset(1, 0, 0, kpad, cols);
+    const uint8_t *bcol = planes + tree_plane_offset(0, col0 + g, 0, kpad, cols);
+    const i32 *arow[TREE_MTILES][2];
+    bool rok[TREE_MTILES][2];
+#pragma unroll
+    for (int mt = 0; mt < TREE_MTILES; mt++)
+#pragma unroll
+        for (int hr = 0; hr < 2; hr++) {
+            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
+            rok[mt][hr] = r < rows;
+            arow[mt][hr] = a + (rok[mt][hr] ? r : 0) * n;
+        }
+    i32 acc[4][TREE_MTILES][TREE_NTILES][4];
+#pragma unroll
+    for (int p = 0; p < 4; p++)
+#pragma unroll
+        for (int mt = 0; mt < TREE_MTILES; mt++)
+#pragma unroll
+            for (int nt = 0; nt < TREE_NTILES; nt++)
+#pragma unroll
+                for (int i = 0; i < 4; i++) acc[p][mt][nt][i] = 0;
+
+    for (u32 ks = 0; ks < ksteps; ks++) {
+        u32 bf[TREE_NTILES][4][2];
+#pragma unroll
+        for (int nt = 0; nt < TREE_NTILES; nt++)
+#pragma unroll
+            for (int p = 0; p < 4; p++)
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+                    bf[nt][p][h] = __ldg((const u32 *)(bcol + (u64)8 * nt * kpad + p * plane_stride + 32 * ks + pk_frag_k(t, h)));
+        const u32 i0 = 16 * ks + 4 * t;      // mask words i0, i0 + 1 feed half 0, i0 + 2, i0 + 3 half 1
+#pragma unroll
+        for (int mt = 0; mt < TREE_MTILES; mt++) {
+            i32 w[2][4];
+#pragma unroll
+            for (int hr = 0; hr < 2; hr++)
+#pragma unroll
+                for (int q = 0; q < 4; q++) w[hr][q] = (rok[mt][hr] && i0 + q < n) ? __ldg(arow[mt][hr] + i0 + q) : 0;
+            const u32 af[4] = {tree_a_frag(w[0][0], w[0][1]), tree_a_frag(w[1][0], w[1][1]),
+                               tree_a_frag(w[0][2], w[0][3]), tree_a_frag(w[1][2], w[1][3])};
+#pragma unroll
+            for (int nt = 0; nt < TREE_NTILES; nt++)
+#pragma unroll
+                for (int p = 0; p < 4; p++) tree_mma(acc[p][mt][nt], af, bf[nt][p]);
+        }
+    }
+
+#pragma unroll
+    for (int mt = 0; mt < TREE_MTILES; mt++)
+#pragma unroll
+        for (int nt = 0; nt < TREE_NTILES; nt++)
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
+                if (row >= rows) continue;
+                const u32 col = col0 + 8 * nt + pk_acc_col(t, i);
+                out[row * cols + col] = (i32)pk_combine(acc[0][mt][nt][i], acc[1][mt][nt][i], acc[2][mt][nt][i],
+                                                        acc[3][mt][nt][i]);
+            }
+}
+
+// nb_tree_assemble: one CTA per (test vector, polynomial u).  Z_u = sum_m X^(o_m) G_m,u in shared memory, its
+// exclusive prefix sums (4 coefficients per thread, a warp scan, then the warp totals), then every coefficient of
+// Q_P Z_u as the difference of two prefix sums.  All sums wrap mod 2^32, which is exact.
+constexpr int TREE_ASM_THREADS = 256;
+static_assert(TREE_ASM_THREADS * 4 == PACK_N, "tree_assemble_kernel: 4 coefficients per thread");
+
+__global__ void __launch_bounds__(TREE_ASM_THREADS) tree_assemble_kernel(const i32 *__restrict__ v,
+                                                                          const i32 *__restrict__ b, int bits, u32 k,
+                                                                          i32 *__restrict__ tv)
+{
+    __shared__ u32 z[PACK_N];
+    __shared__ u32 ps[PACK_N + 1];
+    __shared__ u32 warp_sum[TREE_ASM_THREADS / 32];
+    const u64 t = blockIdx.x / (k + 1);
+    const u32 u = blockIdx.x % (k + 1);
+    const int M = 1 << bits, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int x = tid; x < PACK_N; x += TREE_ASM_THREADS) {
+        u32 s = 0;
+        for (int m = 0; m < M; m++) {
+            bool neg;
+            const int d = tree_shift_index(tree_offset(m, bits), x, &neg);
+            const u32 gv = tree_glwe_coef(v + ((t * M + m) * (k + 1) + u) * PACK_N, b[t * M + m], u == k, d);
+            s += neg ? 0u - gv : gv;
+        }
+        z[x] = s;
+    }
+    __syncthreads();
+    u32 loc[4], run = 0;
+#pragma unroll
+    for (int q = 0; q < 4; q++) { loc[q] = run; run += z[4 * tid + q]; }
+    u32 incl = run;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const u32 y = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += y;
+    }
+    if (lane == 31) warp_sum[warp] = incl;
+    __syncthreads();
+    u32 base = incl - run;
+    for (int w = 0; w < warp; w++) base += warp_sum[w];
+#pragma unroll
+    for (int q = 0; q < 4; q++) ps[4 * tid + q] = base + loc[q];
+    if (tid == TREE_ASM_THREADS - 1) ps[PACK_N] = base + run;
+    __syncthreads();
+    i32 *out = tv + (t * (k + 1) + u) * PACK_N;
+    for (int x = tid; x < PACK_N; x += TREE_ASM_THREADS) out[x] = (i32)tree_window_coef(ps, PACK_N >> bits, x);
 }
 
 }  // namespace nb

@@ -393,6 +393,58 @@ class Engine:
             self._call('nb_pack_finish', _ptr(c), _ptr(b), k1 - 1, _ptr(out), batch)
         return out
 
+    def tree_prepare(self, masks, body):
+        """The tree key's masks (n, t, k, N) and bodies (n, t, N) int32 laid into the 4 byte planes that tree_keyswitch
+        reads (nb_tree_prepare): a uint8 tensor of nb_tree_planes_bytes(n, k) bytes."""
+        masks = self._dense(masks, torch.int32)
+        body = self._dense(body, torch.int32)
+        n, t, k, n_poly = masks.shape
+        if t != 2 or n_poly != N or tuple(body.shape) != (n, t, N):
+            raise ValueError('tree_prepare: masks %s and bodies %s are not (n, 2, k, N) and (n, 2, N)'
+                             % (tuple(masks.shape), tuple(body.shape)))
+        planes = self.empty((self.lib.nb_tree_planes_bytes(n, k),), torch.uint8)
+        self._call('nb_tree_prepare', _ptr(masks), _ptr(body), n, k, _ptr(planes))
+        return planes
+
+    def tree_keyswitch(self, a, planes, mask_size):
+        """LWE masks a (R, n) int32 -> V (R, k+1, N) int32, V = sum_ij d_ij(a) T_ij mod 2^32 (nb_tree_keyswitch)."""
+        a = self._dense(a, torch.int32)
+        planes = self._dense(planes, torch.uint8)
+        rows, n = a.shape
+        if planes.numel() != self.lib.nb_tree_planes_bytes(n, int(mask_size)):
+            raise ValueError('tree_keyswitch: %d plane bytes do not fit n = %d, k = %d' % (planes.numel(), n, mask_size))
+        out = self.empty((rows, mask_size + 1, N), torch.int32)
+        if rows:
+            self._call('nb_tree_keyswitch', _ptr(a), _ptr(planes), n, int(mask_size), _ptr(out), rows)
+        return out
+
+    def tree_assemble(self, v, b, bits):
+        """v (T, 2^bits, k+1, N) and bodies b (T, 2^bits) int32 -> test vectors (T, k+1, N) (nb_tree_assemble)."""
+        v = self._dense(v, torch.int32)
+        b = self._dense(b, torch.int32)
+        if v.dim() != 4 or v.shape[1] != 1 << int(bits) or v.shape[3] != N or tuple(b.shape) != tuple(v.shape[:2]):
+            raise ValueError('tree_assemble: v %s and b %s do not fit %d-bit digits'
+                             % (tuple(v.shape), tuple(b.shape), bits))
+        count, _, k1, _ = v.shape
+        out = self.empty((count, k1, N), torch.int32)
+        if count:
+            self._call('nb_tree_assemble', _ptr(v), _ptr(b), int(bits), k1 - 1, _ptr(out), count)
+        return out
+
+    def bootstrap_glwe_lut_extract(self, x, tv, bk_int):
+        """The programmable bootstrap of x = (a (B, n), b (B,)) with per-ciphertext GLWE test vectors tv (B, 2, N):
+        returns the extracted samples a (B, N), b (B,) (nb_bootstrap_glwe_lut_extract)."""
+        a, b = self._dense(x[0], torch.int32), self._dense(x[1], torch.int32)
+        tv = self._dense(tv, torch.int32)
+        B = b.numel()
+        n = a.shape[-1]
+        if tuple(tv.shape) != (B, 2, N) or a.numel() != B * n:
+            raise ValueError('bootstrap_glwe_lut_extract: tv %s for %d ciphertexts' % (tuple(tv.shape), B))
+        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
+        self._call('nb_bootstrap_glwe_lut_extract', _ptr(a), _ptr(b), _ptr(tv), _ptr(bk_int), n, _ptr(out_a),
+                   _ptr(out_b), B)
+        return out_a, out_b
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()

@@ -88,10 +88,13 @@ class NuFHEPackingSecretKey:
                 and torch.equal(self.key.cpu(), other.key.cpu()))
 
 
-class NuFHEPackingKey:
-    """The server's half: params, the 256-bit seed of the masks, the bodies (n, t, N) int32 (4.1 MB for the default
-    parameters) and the variance of their noise.  `spectra(thr)` -- the NTT of all n t (k+1) key polynomials, 16.4 MB
-    for k = 1 -- is built once per engine and cached on the object."""
+class _GadgetKey:
+    """n t seeded GLWE encryptions of the constants s_i g_j (s the LWE key, g_j = PACK_GADGET[j]) under a GLWE key:
+    params, the 256-bit seed of the masks (ChaCha20 stream (seed, NONCE)), the bodies (n, t, N) int32 and the variance
+    of their noise.  The packing key and the tree key (nufhe_b200/tree_lut.py) are two distinct subclasses."""
+    NONCE = None
+    TAG = None
+    NAME = None
 
     def __init__(self, params, seed, body, variance: float):
         self.params = params
@@ -101,20 +104,19 @@ class NuFHEPackingKey:
         tl, k, N = _glwe(params)
         want = (params.in_out_params.size, PACK_LEVELS, N)
         if tuple(body.shape) != want:
-            raise ValueError('a packing key for these parameters has body shape %s, got %s' % (want, tuple(body.shape)))
-        self._spectra = None
+            raise ValueError('a %s for these parameters has body shape %s, got %s' % (self.NAME, want, tuple(body.shape)))
 
     @classmethod
-    def from_secret_key(cls, thr, rng, secret_key, packing_secret_key: NuFHEPackingSecretKey):
-        """K_ij = GLWE_{S_p}(s_i g_j) with seeded masks: draws the seed, then the Gaussian body noises (n, t, N)."""
+    def _encrypt(cls, thr, rng, secret_key, glwe_key):
+        """K_ij = GLWE_{glwe_key}(s_i g_j) with seeded masks: draws the seed, then the Gaussian body noises (n, t, N)."""
         params = secret_key.params
         tl, k, N = _glwe(params)
         n = params.in_out_params.size
         seed = draw_seed(rng)
         noises = rand_gaussian_torus32(thr, rng, 0, tl.min_noise, (n, PACK_LEVELS, N))
         samples = TLweSampleArray.empty(thr, tl, (n, PACK_LEVELS))
-        key = TLweKey(tl, IntPolynomialArray(packing_secret_key.key))
-        tlwe_encrypt_zero_with_masks(thr, samples, _masks(thr, seed, params), noises, tl.min_noise, key)
+        key = TLweKey(tl, IntPolynomialArray(glwe_key))
+        tlwe_encrypt_zero_with_masks(thr, samples, _masks(thr, seed, params, cls.NONCE), noises, tl.min_noise, key)
         body = samples.a.coeffs[..., k, :].contiguous()
         g = torch.tensor(PACK_GADGET, dtype=torch.int64, device=body.device)
         msg = secret_key.lwe_key.key.to(body.device).to(torch.int64)[:, None] * g[None, :]      # (n, t): s_i g_j
@@ -123,19 +125,10 @@ class NuFHEPackingKey:
 
     def masks(self, thr):
         """The masks A (n, t, k, N), regenerated from the seed."""
-        return _masks(thr, self.seed, self.params)
-
-    def spectra(self, thr):
-        """NTT of the key polynomials K_iju as (n t, k + 1, N) field elements, row i t + j: what nb_ntt_mac reads."""
-        if self._spectra is None or self._spectra[0] is not thr:
-            tl, k, N = _glwe(self.params)
-            polys = torch.cat([self.masks(thr), self.body.to(thr.device)[:, :, None, :]], dim=2)   # (n, t, k+1, N)
-            spec = thr.ntt_forward_i32(polys.contiguous()).reshape(-1, k + 1, N)
-            self._spectra = (thr, spec)
-        return self._spectra[1]
+        return _masks(thr, self.seed, self.params, self.NONCE)
 
     def dump(self, file_obj):
-        pickle.dump(_PACKING_KEY_TAG, file_obj)
+        pickle.dump(self.TAG, file_obj)
         pickle.dump(self.params, file_obj)
         pickle.dump(self.seed, file_obj)
         pickle.dump(self.body.cpu().numpy(), file_obj)
@@ -148,7 +141,7 @@ class NuFHEPackingKey:
 
     @classmethod
     def load(cls, file_obj, thr):
-        _check_tag(file_obj, _PACKING_KEY_TAG)
+        _check_tag(file_obj, cls.TAG)
         params = pickle.load(file_obj)
         seed = pickle.load(file_obj)
         body = thr.to_device(pickle.load(file_obj))
@@ -164,9 +157,36 @@ class NuFHEPackingKey:
                 and torch.equal(self.body.cpu(), other.body.cpu()) and self.variance == other.variance)
 
 
-def _masks(thr, seed, params):
+class NuFHEPackingKey(_GadgetKey):
+    """The server's half: params, the 256-bit seed of the masks, the bodies (n, t, N) int32 (4.1 MB for the default
+    parameters) and the variance of their noise.  `spectra(thr)` -- the NTT of all n t (k+1) key polynomials, 16.4 MB
+    for k = 1 -- is built once per engine and cached on the object."""
+    NONCE = NONCE_PACKING_KEY
+    TAG = _PACKING_KEY_TAG
+    NAME = 'packing key'
+
+    def __init__(self, params, seed, body, variance: float):
+        super().__init__(params, seed, body, variance)
+        self._spectra = None
+
+    @classmethod
+    def from_secret_key(cls, thr, rng, secret_key, packing_secret_key: NuFHEPackingSecretKey):
+        """K_ij = GLWE_{S_p}(s_i g_j) with seeded masks: draws the seed, then the Gaussian body noises (n, t, N)."""
+        return cls._encrypt(thr, rng, secret_key, packing_secret_key.key)
+
+    def spectra(self, thr):
+        """NTT of the key polynomials K_iju as (n t, k + 1, N) field elements, row i t + j: what nb_ntt_mac reads."""
+        if self._spectra is None or self._spectra[0] is not thr:
+            tl, k, N = _glwe(self.params)
+            polys = torch.cat([self.masks(thr), self.body.to(thr.device)[:, :, None, :]], dim=2)   # (n, t, k+1, N)
+            spec = thr.ntt_forward_i32(polys.contiguous()).reshape(-1, k + 1, N)
+            self._spectra = (thr, spec)
+        return self._spectra[1]
+
+
+def _masks(thr, seed, params, nonce=NONCE_PACKING_KEY):
     tl, k, N = _glwe(params)
-    return thr.seeded_uniform(seed, NONCE_PACKING_KEY, (params.in_out_params.size, PACK_LEVELS, k, N))
+    return thr.seeded_uniform(seed, nonce, (params.in_out_params.size, PACK_LEVELS, k, N))
 
 
 class PackedLweSampleArray:
