@@ -117,44 +117,6 @@ def test_full_size_batches_decrypt_to_truth_table(eng, keys, dev_keys, batch):
     assert (keys.decrypt((eng.to_host(ma), eng.to_host(mb))) == numpy.where(bits[0], bits[1], bits[2])).all()
 
 
-def test_all_cta_shapes_give_the_same_bits(keys, monkeypatch):
-    """The fused bootstrap has four shapes: 2 ciphertexts per 256 threads (throughput, with the FP64 step or, forced,
-    the NTT step), 1 ciphertext per 256 threads (inverse phases split over thread pairs), 1 ciphertext per 512 threads
-    (forward phases split as well; batches up to 1.5 ciphertexts per SM) and 1 ciphertext per cluster of two
-    256-thread CTAs on two SMs (partial sums of the MAC exchanged through distributed shared memory, in both exchange
-    variants; batches whose clusters all fit).  Force each shape for the same inputs, including a ragged batch and one
-    larger than a wave (time-sliced, or clusters queued by the hardware); all must equal the oracle and each other."""
-    from nufhe_b200.engine import Engine
-    rng = G.rs(480)
-    shapes = {'default': ('0', '0', '0', '1', '1'),          # the throughput shape with the FP64 step (integral key)
-              'default_ntt': ('0', '0', '0', '1', '0'),      # the throughput shape with the NTT step
-              'wide': ('1000000', '0', '0', '1', '1'), 'wide2': ('1000000', '1000000', '0', '1', '1'),
-              'pair': ('0', '0', '1000000', '1', '1'),       # exchange by st.async + mbarrier (the default)
-              'pair_barrier': ('0', '0', '1000000', '0', '1')}  # exchange by plain remote stores + barrier.cluster
-    for B in (1, 5, 301):
-        bits_a, bits_b = rng.randint(0, 2, B).astype(bool), rng.randint(0, 2, B).astype(bool)
-        a, b = keys.encrypt(bits_a), keys.encrypt(bits_b)
-        want = O.gate_binary('nand', a, b, keys.bk, keys.ks) if B <= 5 else None
-        outs = {}
-        for name, (wide_max, wide2_max, pair_max, pair_async, fft) in shapes.items():
-            monkeypatch.setenv('NUFHE_B200_FFT', fft)
-            monkeypatch.setenv('NUFHE_B200_WIDE_MAX', wide_max)
-            monkeypatch.setenv('NUFHE_B200_WIDE2_MAX', wide2_max)
-            monkeypatch.setenv('NUFHE_B200_PAIR_MAX', pair_max)
-            monkeypatch.setenv('NUFHE_B200_PAIR_ASYNC', pair_async)
-            eng = Engine()
-            dk = (eng.bk_prepare(eng.to_device(keys.bk)),
-                  (eng.to_device(keys.ks_a), eng.to_device(keys.ks_b), eng.to_device(keys.ks_cv)))
-            ext, out = gpu_gate(eng, dk, 'nand', a, b)
-            outs[name] = (ext, out)
-            if want is not None:
-                assert (out[0] == want[0]).all() and (out[1] == want[1]).all(), (B, name)
-            assert (keys.decrypt(out) == ~(bits_a & bits_b)).all()
-        for name in ('default_ntt', 'wide', 'wide2', 'pair', 'pair_barrier'):
-            for x, y in zip(outs['default'], outs[name]):
-                assert (x[0] == y[0]).all() and (x[1] == y[1]).all(), (B, name)
-
-
 # ---- BASELINE.md section 4 parity set --------------------------------------------------------------------------
 
 def test_nand32_and_mux_match_reference_closures(eng, keys, dev_keys, golden):
@@ -277,6 +239,21 @@ assert (eng.to_host(ra) == want[0]).all() and (eng.to_host(rb) == want[1]).all()
 x = numpy.random.RandomState(5).randint(-2**31, 2**31, (64, 1024)).astype(numpy.int32)
 f = eng.ntt_forward_i32(eng.to_device(x))
 assert (eng.to_host(eng.ntt_inverse_i32(f)) == x).all()
+# the LUT instantiations and the second job of extract2, against the oracle at n = 25
+sys.path.insert(0, %(root)r + '/tests')
+import fused_ref as F
+bk25 = eng.bk_prepare(eng.to_device(keys.bk[:25]))
+dev = lambda x: (eng.to_device(x[0]), eng.to_device(x[1]))
+same = lambda got, want: all((eng.to_host(g) == w).all() for g, w in zip(got, want))
+x1, x2, x3 = [(G.torus32(rng, (B, 25)), G.torus32(rng, (B,))) for _ in range(3)]
+tv = G.torus32(rng, (B, 1024))
+assert same(eng.bootstrap_lut_extract(dev(x1), dev(x2), 12345678, 2, -3, eng.to_device(tv), 2, bk25),
+            F.bootstrap_lut_extract(x1, x2, 12345678, 2, -3, tv, 2, keys.bk))
+tv2 = G.torus32(rng, (B, 2, 1024))
+assert same(eng.bootstrap_glwe_lut_extract(dev(x1), eng.to_device(tv2), bk25), F.bootstrap_glwe_lut_extract(x1, tv2, keys.bk))
+ja, jb = (x1, x2, O.phase_to_t32(-1, 8), 1, 1), (x3, x1, O.phase_to_t32(1, 8) + 4321, -1, 3)
+u1, u2 = eng.bootstrap_extract2((dev(x1), dev(x2)) + ja[2:], (dev(x3), dev(x1)) + jb[2:], O.MU, bk25)
+assert same(u1 + u2, F.bootstrap_extract(*ja, O.MU, keys.bk) + F.bootstrap_extract(*jb, O.MU, keys.bk))
 print('rare path ok')
 '''
 
@@ -286,7 +263,9 @@ def test_canonicalisation_rare_path_forced(wide_max):
     """NUFHE_B200_FORCE_RARE_PATH=1 lowers the trigger of the deferred canonicalisation so that EVERY task of fwd1,
     inv1 and the MAC runs its fix-up code (normally 2^-32 per element); results must not change.  Runs in a fresh
     process because the trigger is a __constant__ set when the context is created.  The throughput shape runs the
-    FP64 step on the (integral) gate key unless NUFHE_B200_FFT=0 keeps its NTT step, which has the fix-up code."""
+    FP64 step on the (integral) gate key unless NUFHE_B200_FFT=0 keeps its NTT step, which has the fix-up code.  Besides
+    the gate, the script runs the separately compiled LUT instantiations (L = 2 with per-ciphertext test vectors, and a
+    GLWE test vector) and extract2 with distinct job operands at an odd job batch, at n = 25 against the oracle."""
     import os
     import subprocess
     import sys

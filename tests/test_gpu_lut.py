@@ -1,11 +1,12 @@
 """Programmable bootstrapping on the GPU: nb_bootstrap_lut_extract against the gate path and the oracle's composition
-of the reference's steps, in every CTA shape, and lookup tables end to end through the VirtualMachine."""
+of the reference's steps, and lookup tables end to end through the VirtualMachine."""
 import numpy
 import pytest
 import torch
 
 import gen_inputs as G
 from oracle import oracle as O
+from fused_ref import oracle_lut
 
 pytestmark = pytest.mark.gpu
 N = 1024
@@ -25,22 +26,6 @@ def keys():
 @pytest.fixture(scope='module')
 def dev_keys(eng, keys):
     return eng.bk_prepare(eng.to_device(keys.bk)), tuple(eng.to_device(x) for x in keys.ks)
-
-
-def oracle_lut(a, b, tv, L, bk):
-    """The reference's composition for x = (a, b): t32_to_phase (2N / 2^L) * 2^L, X^(2N - barb) * tv, trivial
-    accumulator, blind rotation, then per output j a rotation by X^(2N - j) and the extraction; rows c * 2^L + j."""
-    B, K = b.size, 1 << L
-    barb = (O.t32_to_phase(b, (2 * N) >> L).astype(numpy.int64) << L).astype(numpy.int32)
-    bara = (O.t32_to_phase(a, (2 * N) >> L).astype(numpy.int64) << L).astype(numpy.int32)
-    tvs = numpy.ascontiguousarray(numpy.broadcast_to(tv.reshape(-1, N), (B, N)))
-    acc = O.tlwe_noiseless_trivial(O.shift_torus_polynomial(tvs[:, None, :], barb, invert_powers=True)[:, 0])
-    acc = O.blind_rotate(acc, bk, bara)
-    out_a, out_b = numpy.empty((B, K, N), numpy.int32), numpy.empty((B, K), numpy.int32)
-    for j in range(K):
-        src = O.shift_torus_polynomial(acc, numpy.full(B, 2 * N - j, numpy.int32)) if j else acc
-        out_a[:, j], out_b[:, j] = O.tlwe_extract_lwe_samples(src)
-    return out_a.reshape(B * K, N), out_b.reshape(B * K)
 
 
 def _random_lwe(rng, B):
@@ -100,41 +85,6 @@ def test_bad_arguments_are_rejected(eng, dev_keys):
     with pytest.raises(ValueError, match='stride'):
         eng._call('nb_bootstrap_lut_extract', x[0].data_ptr(), x[1].data_ptr(), None, None, 0, 1, 0, tv.data_ptr(), 512,
                   0, bk_int.data_ptr(), O.LWE_N, x[0].data_ptr(), x[1].data_ptr(), 2)
-
-
-def test_all_cta_shapes_give_the_same_bits(keys, monkeypatch):
-    """Every shape of the fused bootstrap (forced as in test_gpu_gates.py) at B = 1, 5, 301, L = 0 and 2, per-ciphertext
-    test vectors: all shapes agree with each other, and with the oracle for B <= 5."""
-    from nufhe_b200.engine import Engine
-    rng = G.rs(930)
-    shapes = {'default': ('0', '0', '0', '1', '1'), 'default_ntt': ('0', '0', '0', '1', '0'),
-              'wide': ('1000000', '0', '0', '1', '1'), 'wide2': ('1000000', '1000000', '0', '1', '1'),
-              'pair': ('0', '0', '1000000', '1', '1'), 'pair_barrier': ('0', '0', '1000000', '0', '1')}
-    cases = []
-    for B in (1, 5, 301):
-        for L in (0, 2):
-            x = _random_lwe(rng, B)
-            tv = rng.randint(-2**31, 2**31, size=(B, N), dtype=numpy.int64).astype(numpy.int32)
-            want = oracle_lut(x[0], x[1], tv, L, keys.bk) if B <= 5 else None
-            cases.append((B, L, x, tv, want))
-    outs = {}
-    for name, (wide_max, wide2_max, pair_max, pair_async, fft) in shapes.items():
-        monkeypatch.setenv('NUFHE_B200_FFT', fft)
-        monkeypatch.setenv('NUFHE_B200_WIDE_MAX', wide_max)
-        monkeypatch.setenv('NUFHE_B200_WIDE2_MAX', wide2_max)
-        monkeypatch.setenv('NUFHE_B200_PAIR_MAX', pair_max)
-        monkeypatch.setenv('NUFHE_B200_PAIR_ASYNC', pair_async)
-        eng = Engine()
-        bk_int = eng.bk_prepare(eng.to_device(keys.bk))
-        for B, L, x, tv, want in cases:
-            ga, gb = eng.bootstrap_lut_extract(_dev(eng, x), None, 0, 1, 0, eng.to_device(tv), L, bk_int)
-            got = (eng.to_host(ga), eng.to_host(gb))
-            outs[name, B, L] = got
-            if want is not None:
-                assert (got[0] == want[0]).all() and (got[1] == want[1]).all(), (name, B, L)
-    for (name, B, L), got in outs.items():
-        ref = outs['default', B, L]
-        assert (got[0] == ref[0]).all() and (got[1] == ref[1]).all(), (name, B, L)
 
 
 @pytest.fixture(scope='module')

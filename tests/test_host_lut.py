@@ -113,6 +113,43 @@ def test_modswitch_head_tail_match_the_oracle(emul):
         assert (got_a == want_a[0]).all() and got_b[0] == want_b[0], j
 
 
+def test_fused_ref_compositions_agree():
+    """The oracle compositions the GPU matrix checks against (tests/fused_ref.py) agree with each other at n = 25: the
+    LUT composition with the constant test vector mu is the gate bootstrap (also for the rounding ties of the L = 0
+    mod-switch), the GLWE composition with zero masks is the LUT composition, the extract2 rows are two gates, and the
+    explicit rotation of the gate's initial accumulator is the gate."""
+    import fused_ref as F
+    keys = O.OracleKeys(G.GATE_SEED, n=25)
+    rng = numpy.random.RandomState(8)
+    B, n = 12, 25
+    x1 = (G.torus32(rng, (B, n)), G.torus32(rng, (B,)))
+    x2 = (G.torus32(rng, (B, n)), G.torus32(rng, (B,)))
+    x1[1][:4] = [2**20, 2**20 - 1, -2**20, 2**31 - 2**20]            # ties of the rounding, with s1 = 1 and no x2
+    c, s1, s2 = 12345678, 1, -3
+    gate = F.bootstrap_extract(x1, None, c, s1, s2, O.MU, keys.bk)
+    lut0 = F.bootstrap_lut_extract(x1, None, c, s1, s2, numpy.full(N, O.MU, numpy.int32), 0, keys.bk)
+    assert (gate[0] == lut0[0]).all() and (gate[1] == lut0[1]).all()
+    gate2 = F.bootstrap_extract(x1, x2, c, s1, s2, -2**31, keys.bk)
+    lut2 = F.bootstrap_lut_extract(x1, x2, c, s1, s2, numpy.full(N, -2**31, numpy.int32), 0, keys.bk)
+    assert (gate2[0] == lut2[0]).all() and (gate2[1] == lut2[1]).all()
+    pair = F.bootstrap_extract2((x1, None, c, s1, s2), (x1, x2, c, s1, s2), O.MU, keys.bk)
+    assert (pair[0][:B] == gate[0]).all() and (pair[1][B:] == F.bootstrap_extract(x1, x2, c, s1, s2, O.MU, keys.bk)[1]).all()
+    tv = G.torus32(rng, (B, N))
+    a, b = F.prologue(x1, x2, c, s1, s2)
+    glwe = numpy.zeros((B, 2, N), numpy.int32)
+    glwe[:, 1] = tv
+    want = F.bootstrap_lut_extract((a, b), None, 0, 1, 0, tv, 0, keys.bk)
+    got = F.bootstrap_glwe_lut_extract((a, b), glwe, keys.bk)
+    assert (got[0] == want[0]).all() and (got[1] == want[1]).all()
+    # the gate's initial accumulator (0, X^(2N - barb) mu) rotated explicitly
+    barb = O.t32_to_phase(b, 2 * N)
+    acc = O.tlwe_noiseless_trivial(O.shift_torus_polynomial(numpy.full((B, 1, N), O.MU, numpy.int32), barb,
+                                                            invert_powers=True)[:, 0])
+    ea, eb, eacc = F.blind_rotate(acc, O.t32_to_phase(a, 2 * N), keys.bk)
+    gate3 = F.bootstrap_extract((a, b), None, 0, 1, 0, O.MU, keys.bk)
+    assert (ea == gate3[0]).all() and (eb == gate3[1]).all() and eacc.shape == (B, 2, N)
+
+
 def test_allowed_table_follows_the_sigma_formula():
     import nufhe_b200
     params = nufhe_b200.NuFHEParameters()
