@@ -25,6 +25,7 @@
 // barrier between phases), which lets the CPU-only test-suite check every index map against the oracle.
 #pragma once
 #include <cmath>
+#include <cstring>
 #include "ntt_lane.cuh"
 #include "fft_layout.cuh"
 
@@ -1191,19 +1192,25 @@ struct cplx {
 constexpr int BK_FFT_SPECTRA = 16;
 constexpr int BK_FFT_U64 = BK_FFT_SPECTRA * FFT_M * 2;
 static_assert(BK_ROW_U64 == BK_NTT_U64 + BK_FFT_U64, "key row layout");
-// tables (tables.h: FftTables), complex, concatenated: twist w^j (512), pass-1 twiddles W512^(n0 k1) [n0][k1] (512),
-// untwist conj(w^j) / 512 (512).  The pass-2 twiddles are compile-time constants (fft_w64).
-constexpr int FFT_TAB_TWIST = 0, FFT_TAB_TW1 = 512, FFT_TAB_UNTWIST = 1024, FFT_TAB_CPLX = 1536;
+// table (tables.h: FftTables), complex: the pass-1 twiddles merged with the n0 part of the twist,
+// T[k1][n0] = w^n0 W512^(n0 k1), stored [k1][n0] so that the consecutive n0 of a warp read consecutive 16-byte
+// elements.  The rest of the twist, w^(64 m), and the pass-2 twiddles are compile-time constants (fft_w64).
+constexpr int FFT_TAB_T1 = 0, FFT_TAB_CPLX = 512;
+NB_HD constexpr int fft_tab_t1(int k1, int n0) { return FFT_TAB_T1 + k1 * 64 + n0; }
 
 #if defined(__CUDA_ARCH__)
 NB_HD double d_add(double a, double b) { return __dadd_rn(a, b); }
 NB_HD double d_sub(double a, double b) { return __dsub_rn(a, b); }
 NB_HD double d_mul(double a, double b) { return __dmul_rn(a, b); }
 NB_HD double d_fma(double a, double b, double c) { return __fma_rn(a, b, c); }
+// a table load (through the L1) that the compiler can neither merge with the same load of another phase nor move across
+// a barrier: fwd1 and inv1 read the same table entries, and ptxas merges two read-only (.nc) loads of one address even
+// across barriers -- it then keeps fwd1's 8 values (32 registers) live through the whole step, and the step spills
 NB_HD cplx ld_cplx_tab(const cplx *p)
 {
-    const double2 t = __ldg(reinterpret_cast<const double2 *>(p));
-    return {t.x, t.y};
+    cplx t;
+    asm volatile("ld.global.v2.f64 {%0, %1}, [%2];" : "=d"(t.re), "=d"(t.im) : "l"(p));
+    return t;
 }
 NB_HD cplx ld_cplx(const cplx *p)
 {
@@ -1216,7 +1223,8 @@ NB_HD cplx ld_cplx_stream(const cplx *p)           // key spectra: read once per
     const double2 t = __ldcg(reinterpret_cast<const double2 *>(p));
     return {t.x, t.y};
 }
-NB_HD i32 d_rint_lo32(double x) { return (i32)__double2ll_rn(x); }
+NB_HD double d_from_words(u32 hi, u32 lo) { return __hiloint2double((int)hi, (int)lo); }
+NB_HD u32 d_lo_word(double x) { return (u32)__double2loint(x); }
 #else
 NB_HD double d_add(double a, double b) { return a + b; }
 NB_HD double d_sub(double a, double b) { return a - b; }
@@ -1226,8 +1234,29 @@ NB_HD cplx ld_cplx_tab(const cplx *p) { return *p; }
 NB_HD cplx ld_cplx(const cplx *p) { return *p; }
 NB_HD void st_cplx(cplx *p, cplx v) { *p = v; }
 NB_HD cplx ld_cplx_stream(const cplx *p) { return *p; }
-NB_HD i32 d_rint_lo32(double x) { return (i32)(u32)(uint64_t)std::llrint(x); }
+NB_HD double d_from_words(u32 hi, u32 lo)
+{
+    const uint64_t b = (uint64_t)hi << 32 | lo;
+    double x;
+    memcpy(&x, &b, sizeof x);
+    return x;
+}
+NB_HD u32 d_lo_word(double x)
+{
+    uint64_t b;
+    memcpy(&b, &x, sizeof b);
+    return (u32)b;
+}
 #endif
+// Conversions between doubles and integers without the conversion unit (I2F.F64 / F2I.F64, a quarter of the FP64
+// rate on sm_90), so the step stays on the FP64 pipe:
+// the digit u - 512 of u in [0, 1023]: the words 0x43300000 : u are the double 2^52 + u, and one exact subtraction
+// removes 2^52 + 512
+NB_HD double d_digit(u32 u) { return d_add(d_from_words(0x43300000u, u), -(0x1p52 + 512)); }
+// round(x) mod 2^32 for |x| < 2^51: x + 1.5 2^52 lies in [2^52, 2^53), where the spacing of doubles is 1, so the
+// correctly rounded sum is 1.5 2^52 + round(x) (to nearest, ties to even, as __double2ll_rn), and its low word is
+// round(x) mod 2^32 (the low word of 1.5 2^52 is 0)
+NB_HD i32 d_rint_lo32(double x) { return (i32)d_lo_word(d_add(x, 0x1.8p52)); }
 
 NB_HD cplx c_add(cplx a, cplx b) { return {d_add(a.re, b.re), d_add(a.im, b.im)}; }
 NB_HD cplx c_sub(cplx a, cplx b) { return {d_sub(a.re, b.re), d_sub(a.im, b.im)}; }
@@ -1350,22 +1379,36 @@ template <bool INV> NB_HD void dft4(cplx *y)
     y[1] = c_add(b, d); y[3] = c_sub(b, d);
 }
 
+// the 8 pass-1 table values of task n0: t1[k1] = T[k1][n0]; loaded once per phase and shared by both digits (fwd1)
+// or both key halves (inv1)
+NB_HD void fft_load_t1(int n0, const cplx *tab, cplx *t1)
+{
+    static_for<0, 8>([&](auto K) { t1[decltype(K)::value] = ld_cplx_tab(tab + fft_tab_t1(decltype(K)::value, n0)); });
+}
 // pass 1 (forward): x[m'] = real coefficient n0 + 64 m', m' < 16 (exact small integers as doubles); fold, twist,
-// DFT8 over m, twiddle, store at position n0 + 64 k1 of spectrum sp
-NB_HD void fft_fwd1(int n0, const double *x, cplx *sp, const cplx *tab)
+// DFT8 over m, twiddle, store at position n0 + 64 k1 of spectrum sp.  The twist w^(n0 + 64 m) is split: w^(64 m) =
+// e^{i pi m / 16} = conj(W64^(2 m)) is a constant per m (exact for m = 0, the (1 + i) sqrt(1/2) form for m = 4), and
+// w^n0, which commutes with the DFT8 over m, is part of the table T[k1][n0] = w^n0 W512^(n0 k1) applied after it.
+NB_HD void fft_fwd1_t(int n0, const double *x, cplx *sp, const cplx *t1)
 {
     cplx y[8];
-    static_for<0, 8>([&](auto M) {
+    y[0] = {x[0], x[8]};
+    y[4] = c_mul_w8<true>({x[4], x[12]});
+    static_for<1, 8>([&](auto M) {
         constexpr int m = decltype(M)::value;
-        const cplx w = ld_cplx_tab(tab + FFT_TAB_TWIST + n0 + 64 * m);
-        y[m] = {d_fma(x[m], w.re, -d_mul(x[m + 8], w.im)), d_fma(x[m], w.im, d_mul(x[m + 8], w.re))};
+        if constexpr (m != 4) y[m] = c_mul_conj({x[m], x[m + 8]}, fft_w64(2 * m));
     });
     dft8<false>(y);
-    st_cplx(sp + fft_pass1_x(n0, 0), y[0]);
-    static_for<1, 8>([&](auto K) {
+    static_for<0, 8>([&](auto K) {
         constexpr int k = decltype(K)::value;
-        st_cplx(sp + fft_pass1_x(n0, k), c_mul(y[k], ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k)));
+        st_cplx(sp + fft_pass1_x(n0, k), c_mul(y[k], t1[k]));
     });
+}
+NB_HD void fft_fwd1(int n0, const double *x, cplx *sp, const cplx *tab)
+{
+    cplx t1[8];
+    fft_load_t1(n0, tab, t1);
+    fft_fwd1_t(n0, x, sp, t1);
 }
 // pass 2 (forward): the 16 points 64 k1 + n2 + 4 m of spectrum sp -> DFT16, times W64^(n2 k2)
 NB_HD void fft_fwd2(int k1, int n2, cplx *sp)
@@ -1393,22 +1436,35 @@ NB_HD void fft_inv2(int k1, int n2, cplx *sp)
     dft16<true>(y);
     static_for<0, 16>([&](auto M) { st_cplx(sp + fft_pass2_x(k1, n2, decltype(M)::value), y[decltype(M)::value]); });
 }
-// pass 1 (inverse): x[m'] = the (unrounded) real coefficient n0 + 64 m', m' < 16, of spectrum sp
-NB_HD void fft_inv1(int n0, const cplx *sp, const cplx *tab, double *x)
+// pass 1 (inverse): x[m'] = the (unrounded) real coefficient n0 + 64 m', m' < 16, of spectrum sp.  Mirrored: conj(T)
+// before the inverse DFT8, the constants conj(w^(64 m)) / 512 = W64^(2 m) / 512 after it (the division is exact)
+NB_HD void fft_inv1_t(int n0, const cplx *sp, const cplx *t1, double *x)
 {
+    constexpr double R = 1.0 / 512, S = 0.70710678118654752440 / 512;
     cplx y[8];
-    y[0] = ld_cplx(sp + fft_pass1_x(n0, 0));
-    static_for<1, 8>([&](auto K) {
+    static_for<0, 8>([&](auto K) {
         constexpr int k = decltype(K)::value;
-        y[k] = c_mul_conj(ld_cplx(sp + fft_pass1_x(n0, k)), ld_cplx_tab(tab + FFT_TAB_TW1 + n0 * 8 + k));
+        y[k] = c_mul_conj(ld_cplx(sp + fft_pass1_x(n0, k)), t1[k]);
     });
     dft8<true>(y);
     static_for<0, 8>([&](auto M) {
         constexpr int m = decltype(M)::value;
-        const cplx v = c_mul(y[m], ld_cplx_tab(tab + FFT_TAB_UNTWIST + n0 + 64 * m));
+        cplx v;
+        if constexpr (m == 0) v = {d_mul(y[0].re, R), d_mul(y[0].im, R)};
+        else if constexpr (m == 4) v = {d_mul(d_add(y[4].re, y[4].im), S), d_mul(d_sub(y[4].im, y[4].re), S)};
+        else {
+            constexpr cplx w = fft_w64(2 * m);
+            v = c_mul(y[m], cplx{w.re * R, w.im * R});
+        }
         x[m] = v.re;
         x[m + 8] = v.im;
     });
+}
+NB_HD void fft_inv1(int n0, const cplx *sp, const cplx *tab, double *x)
+{
+    cplx t1[8];
+    fft_load_t1(n0, tab, t1);
+    fft_inv1_t(n0, sp, t1, x);
 }
 
 // ---- the FP64 step of a CTA of 2 ciphertexts on 256 threads: spectra fft_spec(ct, s), s = mi * 2 + j before the MAC
@@ -1428,14 +1484,16 @@ template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, c
         const i32 c = ROTATE ? rotate_minus_one(acc, idx, ar, flip) : acc[idx];
         t[j1] = (u32)c + (0x80000000u + (1u << 21));
     });
+    cplx t1[8];
+    fft_load_t1(n0, tab, t1);
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif
     for (int j = 0; j < 2; j++) {
         const int sh = 22 - 10 * j;
         double x[16];
-        static_for<0, 16>([&](auto J) { x[decltype(J)::value] = (double)((int)((t[decltype(J)::value] >> sh) & 1023u) - 512); });
-        fft_fwd1(n0, x, spec_all + fft_pass1_spec(task, j), tab);
+        static_for<0, 16>([&](auto J) { x[decltype(J)::value] = d_digit((t[decltype(J)::value] >> sh) & 1023u); });
+        fft_fwd1_t(n0, x, spec_all + fft_pass1_spec(task, j), t1);
     }
 }
 // fwd2 / inv2: one 16-point task per thread (fft_pass2_task)
@@ -1492,14 +1550,16 @@ template <bool ACCUMULATE> NB_HD void fft_phase_inv1(int task, i32 *acc_all, con
 {
     const int n0 = task & 63, pp = task >> 6;
     u32 r[16];
+    cplx t1[8];
+    fft_load_t1(n0, tab, t1);
     {
         double x[16];
-        fft_inv1(n0, spec_all + fft_pass1_spec(task, 0), tab, x);
+        fft_inv1_t(n0, spec_all + fft_pass1_spec(task, 0), t1, x);
         static_for<0, 16>([&](auto J) { r[decltype(J)::value] = (u32)d_rint_lo32(x[decltype(J)::value]); });
     }
     {
         double x[16];
-        fft_inv1(n0, spec_all + fft_pass1_spec(task, 1), tab, x);
+        fft_inv1_t(n0, spec_all + fft_pass1_spec(task, 1), t1, x);
         static_for<0, 16>([&](auto J) { r[decltype(J)::value] += (u32)d_rint_lo32(x[decltype(J)::value]) << 16; });
     }
     i32 *acc = acc_all + pp * NTT_N;

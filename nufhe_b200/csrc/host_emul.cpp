@@ -373,6 +373,20 @@ int emul_fft_smem_offsets(int phase, int tid, int *out)
 // the group of thread tid
 int emul_fft_key_offset(int tid, int ks, int k3) { return fft_key_pos(ks, tid >> 1, k3); }
 
+// The FP64 step's table as the library uploads it (tables.h: FftTables), FFT_TAB_CPLX complex values, and the index of
+// T[k1][n0] in it; returns FFT_TAB_CPLX
+int emul_fft_table(double *out)
+{
+    static FftTables F;
+    memcpy(out, F.tab.data(), F.tab.size() * sizeof(cplx));
+    return FFT_TAB_CPLX;
+}
+int emul_fft_tab_t1(int k1, int n0) { return fft_tab_t1(k1, n0); }
+// The conversion-free integer <-> double steps of the FP64 step (br_phases.cuh): the digit u - 512 built from the bits
+// of 2^52 + u, and round(x) mod 2^32 through the addition of 1.5 2^52
+double emul_fft_digit(unsigned u) { return d_digit(u); }
+int emul_fft_rint_lo32(double x) { return d_rint_lo32(x); }
+
 // The programmable bootstrap's index functions (lut_index.cuh): the rounded mod-switch, the initial accumulator
 // polynomial X^(2N - barb) * tv, and the sample extracted at index j from an accumulator (2, 1024).
 int emul_modswitch_lut(i32 x, int log2_outputs) { return modswitch_lut(x, log2_outputs); }

@@ -40,25 +40,21 @@ struct PhaseTables {
     }
 };
 
-// Tables of the FP64 step (br_phases.cuh: FFT_TAB_*), complex doubles.  Each value is cos / sin evaluated in long
+// Table of the FP64 step (br_phases.cuh: FFT_TAB_*), complex doubles.  Each value is cos / sin evaluated in long
 // double and rounded once to double, so every component is within 2^-53 (relative) of the exact value -- what the
-// error bound of DESIGN.md section 3 assumes.
+// error bound of DESIGN.md section 4 assumes.
 struct FftTables {
     std::vector<cplx> tab;
     FftTables() : tab(FFT_TAB_CPLX)
     {
         const long double pi = acosl(-1.0L);
-        auto e = [&](long double turns) {           // e^{2 pi i turns}
-            const long double a = 2 * pi * turns;
+        auto e = [&](int num) {                      // e^{2 pi i num / 2048}
+            const long double a = 2 * pi * (long double)(((num % 2048) + 2048) % 2048) / 2048;
             return cplx{(double)cosl(a), (double)sinl(a)};
         };
-        for (int j = 0; j < FFT_M; j++) {
-            tab[FFT_TAB_TWIST + j] = e((long double)j / 2048);                      // w^j, w = e^{i pi / 1024}
-            const cplx c = e(-(long double)j / 2048);                               // conj(w^j) / 512 (exact scaling)
-            tab[FFT_TAB_UNTWIST + j] = {c.re / 512, c.im / 512};
-        }
-        for (int n0 = 0; n0 < 64; n0++)
-            for (int k = 0; k < 8; k++) tab[FFT_TAB_TW1 + n0 * 8 + k] = e(-(long double)((n0 * k) % 512) / 512);
+        // T[k1][n0] = w^n0 W512^(n0 k1) = e^{2 pi i n0 (1 - 4 k1) / 2048}, w = e^{i pi / 1024}
+        for (int k1 = 0; k1 < 8; k1++)
+            for (int n0 = 0; n0 < 64; n0++) tab[fft_tab_t1(k1, n0)] = e(n0 * (1 - 4 * k1));
     }
 };
 

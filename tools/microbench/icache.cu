@@ -35,6 +35,17 @@ DEF(256, G256)
 DEF(512, G256 G256)
 DEF(1024, G1K)
 DEF(2048, G1K G1K)
+// 2 048 .. 3 072 instructions (32 - 48 KB of code) in steps of 128: where, around the 32 KB instruction cache, the
+// issue rate falls off
+#define G128 G64 G64
+DEF(2176, G1K G1K G128)
+DEF(2304, G1K G1K G256)
+DEF(2432, G1K G1K G256 G128)
+DEF(2560, G1K G1K G256 G256)
+DEF(2688, G1K G1K G256 G256 G128)
+DEF(2816, G1K G1K G256 G256 G256)
+DEF(2944, G1K G1K G256 G256 G256 G128)
+DEF(3072, G1K G1K G1K)
 DEF(4096, G4K)
 DEF(8192, G4K G4K)
 DEF(16384, G16K)
@@ -90,6 +101,19 @@ int main()
         run<32768, true>(w, out, dcyc);
         run<1024, true>(w, out, dcyc);
         run<256, true>(w, out, dcyc);
+    }
+    // the fine sweep around the size of the bootstrap's step loop (2 000 - 2 400 instructions), at the 2 and 4 warps
+    // per sub-partition that its 1 and 2 CTAs of 256 threads per SM give
+    for (int w : {2, 4}) {
+        run<2048, false>(w, out, dcyc);
+        run<2176, false>(w, out, dcyc);
+        run<2304, false>(w, out, dcyc);
+        run<2432, false>(w, out, dcyc);
+        run<2560, false>(w, out, dcyc);
+        run<2688, false>(w, out, dcyc);
+        run<2816, false>(w, out, dcyc);
+        run<2944, false>(w, out, dcyc);
+        run<3072, false>(w, out, dcyc);
     }
     return 0;
 }

@@ -18,12 +18,16 @@ def rnd32(shape):
     return torch.randint(-2**31, 2**31, shape, generator=g, dtype=torch.int64).to(torch.int32).cuda()
 
 
-def rnd_ff(shape):
-    # uniform 63-bit values are valid (possibly non-canonical) field inputs for a profile run
-    return torch.randint(0, 2**62, shape, generator=g, dtype=torch.int64).cuda()
+def integral_bk(shape):
+    # a bootstrap key whose polynomials are centred 32-bit integers, in the reference's form (NTT, Montgomery), as
+    # real keys are: nb_bk_prepare gives it spectra, so the launch below runs the FP64 step that bench.py times.  (A
+    # key of random field elements has no spectra and would time the NTT step.)
+    from oracle import oracle as O
+    raw = torch.randint(-2**31, 2**31, shape, generator=g, dtype=torch.int64).to(torch.int32).numpy()
+    return torch.from_numpy(O.bk_transform(raw).view('int64')).cuda()
 
 
-bk_int = eng.bk_prepare(rnd_ff((500, 2, 2, 2, 1024)))
+bk_int = eng.bk_prepare(integral_bk((500, 2, 2, 2, 1024)))
 ks = (rnd32((1024, 8, 4, 500)), rnd32((1024, 8, 4)), torch.zeros((1024, 8, 4), dtype=torch.float32).cuda())
 x1 = (rnd32((B, 500)), rnd32((B,)))
 x2 = (rnd32((B, 500)), rnd32((B,)))

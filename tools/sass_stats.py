@@ -89,6 +89,26 @@ def enclosing_functions(path):
     return names
 
 
+def step_loop(kernel_ins, loop_addrs, labels):
+    """The rotating step loop: from the target of its back-edge (the first backward branch after the last instruction of
+    a step phase) to that branch.  Returns its size and the static count of spill (LDL / STL) and FP64 conversion
+    (I2F.F64 / F2I.*F64) instructions inside it, or None if there is no such loop."""
+    if not loop_addrs:
+        return None
+    last = max(loop_addrs)
+    for addr, op, rest in kernel_ins:
+        if addr < last or not op.startswith('BRA'):
+            continue
+        t = re.search(r'\((\.L_x_\d+)\)', rest)
+        head = labels.get(t.group(1)) if t else None
+        if head is not None and head < addr:
+            body = [o for a, o, _ in kernel_ins if head <= a <= addr]
+            return {'head': head, 'back_edge': addr, 'bytes': addr + 16 - head, 'instructions': len(body),
+                    'ldl': sum(o.startswith('LDL') for o in body), 'stl': sum(o.startswith('STL') for o in body),
+                    'conversions': sum(o.startswith(('I2F.F64', 'F2I')) and 'F64' in o for o in body)}
+    return None
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--lib', default=os.path.join(ROOT, 'nufhe_b200', 'csrc', 'libnufhe_b200.so'))
@@ -192,8 +212,12 @@ def main():
     counts = collections.defaultdict(lambda: collections.Counter())
     byfunc = collections.defaultdict(lambda: collections.Counter())
     rx_line = re.compile(r'//## File "([^"]+)", line (\d+)')
-    rx_ins = re.compile(r'^\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)(.*)')
+    rx_ins = re.compile(r'^\s+/\*([0-9a-f]+)\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)(.*)')
     forms = collections.Counter()
+    loop_addrs = []           # addresses of the instructions of the rotating step loop's phases
+    kernel_ins = []           # (address, opcode, operands) of every instruction of the kernel
+    labels, pending_labels = {}, []
+    rx_label = re.compile(r'^(\.L_x_\d+):')
     for ln in text:
         if ln.startswith('.text.'):
             in_kernel = args.kernel in ln
@@ -208,11 +232,19 @@ def main():
                 chain_done = False
             chain.append((m.group(1), int(m.group(2))))
             continue
+        m = rx_label.match(ln)
+        if m:
+            pending_labels.append(m.group(1))
+            continue
         m = rx_ins.match(ln)
         if not m:
             continue
         chain_done = True
-        op = m.group(1)
+        addr, op, rest = int(m.group(1), 16), m.group(2), m.group(3)
+        kernel_ins.append((addr, op, rest))
+        for lab in pending_labels:
+            labels[lab] = addr
+        pending_labels = []
         pipe = pipe_of(op)
         phase = 'other'
         in_loop = False
@@ -224,6 +256,8 @@ def main():
                     in_loop = True
         if phase != 'other' and not in_loop:
             phase = 'plain:' + phase     # the non-rotating instantiation (nb_external_product)
+        if in_loop and phase != 'other':
+            loop_addrs.append(addr)
         w = 0.25 if any(path.endswith('br_phases.cuh') and line in case_lines for path, line in chain) else 1
         if any(path.endswith('br_phases.cuh') and line in twice_lines for path, line in chain):
             w *= 2
@@ -234,7 +268,7 @@ def main():
             continue
         counts[phase][pipe] += w
         if args.opcodes and phase.startswith(('phase_', 'fft_phase_')):
-            forms[instruction_form(op, m.group(2))] += w * (
+            forms[instruction_form(op, rest)] += w * (
                 1 if ('BrCfgILi1E' in args.kernel and phase.startswith('phase_fwd')) else STEP_MULT.get(phase, 1))
         if args.by_func and chain:
             inner = None
@@ -249,6 +283,7 @@ def main():
 
     # the wide shape (1 ciphertext on 256 threads) runs the forward phases in one sweep
     mult = dict(STEP_MULT, phase_fwd1=1, phase_fwd2=1, phase_fwd3=1) if 'BrCfgILi1E' in args.kernel else STEP_MULT
+    loop = step_loop(kernel_ins, loop_addrs, labels)
     if args.json:
         import json
         tot = collections.Counter()
@@ -258,7 +293,8 @@ def main():
                     tot[k] += v * mult.get(phase, 1)
         print(json.dumps({'kernel': args.kernel, 'per_thread_step': {k: tot[k] for k in ('alu', 'fma', 'fp64', 'lsu', 'uni', 'other')},
                           'per_thread_step_total': sum(tot.values()),
-                          'phases': {ph: sum(c.values()) * mult.get(ph, 1) for ph, c in counts.items() if ph.startswith(('phase_', 'fft_phase_'))}}))
+                          'phases': {ph: sum(c.values()) * mult.get(ph, 1) for ph, c in counts.items() if ph.startswith(('phase_', 'fft_phase_'))},
+                          'step_loop': loop}))
         return 0
     print('%-22s %7s %7s %7s %7s %7s %7s %8s' % ('phase (static)', 'alu', 'fma', 'fp64', 'lsu', 'uni', 'other', 'total'))
     tot = collections.Counter()
@@ -270,6 +306,10 @@ def main():
                 tot[k] += v * mult.get(phase, 1)
     print('%-22s %7d %7d %7d %7d %7d %7d %8d   (sweeps, MAC rows and switch weights applied)' % (
         'per step, per thread', tot['alu'], tot['fma'], tot['fp64'], tot['lsu'], tot['uni'], tot['other'], sum(tot.values())))
+    if loop:
+        print('step loop: %#x - back-edge %#x, %d bytes (%d instructions); static in the loop: %d LDL, %d STL (spill), '
+              '%d I2F.F64 / F2I.F64 (conversion)' % (loop['head'], loop['back_edge'], loop['bytes'], loop['instructions'],
+                                                       loop['ldl'], loop['stl'], loop['conversions']))
     if args.opcodes:
         # issue cost in SMSP cycles per warp-instruction (tools/microbench/pipes.cu): 2 on either integer
         # pipe, except IMAD.WIDE with a 64-bit addend: 4
