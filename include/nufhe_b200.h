@@ -80,6 +80,17 @@ int nb_ff_elementwise(nb_ctx *ctx, int op, const uint64_t *a, const uint64_t *b,
 size_t nb_bk_row_u64(void);
 int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t rows);
 
+/* ---- multi-bit bootstrap key (DESIGN.md section 14): key bits taken two at a time, group g = (s_2g, s_2g+1) has
+ * 3 reference rows, row 3 g + p - 1 encrypting [s_2g = b0 and s_2g+1 = b1] for p = b0 + 2 b1 = 1, 2, 3.
+ * Re-lays 3 * `groups` reference rows into nb_bk_multibit_row_u64() uint64 per row: the FP64 spectra of the 16-bit key
+ * halves only.  Synchronises the context's stream.  NB_EINVAL if a coefficient is not a centred 32-bit integer.
+ * The prepared range is registered on the context: nb_bootstrap_extract, nb_bootstrap_extract2,
+ * nb_bootstrap_lut_extract and nb_bootstrap_glwe_lut_extract given a pointer into it run the multi-bit blind rotation
+ * (n / 2 groups; n must be even), in the 2-ciphertext FP64 shape at every batch size; nb_blind_rotate and
+ * nb_external_product return NB_EUNSUPPORTED for it. */
+size_t nb_bk_multibit_row_u64(void);
+int nb_bk_prepare_multibit(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_mb, size_t groups);
+
 /* ---- tgsw_transformed_external_mul (tgsw.py:165-172): accum (B,2,1024) <- bk[row] (x) accum ---- */
 int nb_external_product(nb_ctx *ctx, int32_t *accum, const uint64_t *bk_int, size_t bk_row, size_t batch);
 

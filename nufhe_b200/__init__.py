@@ -45,6 +45,7 @@ from .compressed import (
     CompressedLweSampleArray,
     CompressedCloudKey,
     )
+from .bootstrap import MultiBitBootstrapKey
 from .public_key import (
     NuFHEPublicKey,
     public_key_size,

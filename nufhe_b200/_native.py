@@ -35,6 +35,8 @@ SIGNATURES = {
     'nb_ff_elementwise': [_vp, _int, _vp, _vp, _vp, _sz, _sz],
     'nb_bk_row_u64': [],
     'nb_bk_prepare': [_vp, _vp, _vp, _sz],
+    'nb_bk_multibit_row_u64': [],
+    'nb_bk_prepare_multibit': [_vp, _vp, _vp, _sz],
     'nb_external_product': [_vp, _vp, _vp, _sz, _sz],
     'nb_blind_rotate': [_vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _sz],
     'nb_bootstrap_extract': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _sz, _vp, _vp, _sz],
@@ -65,7 +67,7 @@ SIGNATURES = {
     'nb_tree_assemble': [_vp, _vp, _vp, _int, _int, _vp, _sz],
     'nb_bootstrap_glwe_lut_extract': [_vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _sz],
 }
-_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
+_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_bk_multibit_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
              'nb_tree_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p,
              'nb_build_info': ctypes.c_char_p}
 

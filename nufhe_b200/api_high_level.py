@@ -101,13 +101,16 @@ class Context:
     def make_secret_key(self, **params):
         return NuFHESecretKey.from_rng(self.thread, NuFHEParameters(**params), self.rng)
 
-    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False):
+    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False, multi_bit=1):
         """compressed=True returns a CompressedCloudKey (about 12 times smaller to store or send); its `decompress()`
         gives the NuFHECloudKey that make_virtual_machine takes.  tree_key=True returns (cloud key, NuFHETreeKey), the
         key of VirtualMachine.lut_tree; its draws follow all of the cloud key's, so the cloud key is the same either
-        way."""
+        way.  multi_bit=2 gives the cloud key a MultiBitBootstrapKey (key bits two at a time: half the CMux steps per
+        bootstrap, about 3x the key rows and more noise; DESIGN.md section 14); ValueError for parameters it cannot
+        take (tlwe_mask_size = 2, an odd LWE dimension) and for multi_bit outside {1, 2}."""
         cls = CompressedCloudKey if compressed else NuFHECloudKey
-        cloud_key, tgsw_key = cls.from_rng_with_tgsw_key(self.thread, secret_key.params, self.rng, secret_key)
+        cloud_key, tgsw_key = cls.from_rng_with_tgsw_key(self.thread, secret_key.params, self.rng, secret_key,
+                                                         multi_bit=multi_bit)
         if not tree_key:
             return cloud_key
         return cloud_key, NuFHETreeKey.from_secret_key(self.thread, self.rng, secret_key, tgsw_key)
@@ -216,6 +219,8 @@ class VirtualMachine:
         self.params = cloud_key.params
         self.cloud_key = cloud_key
         self.perf_params = perf_params
+        if getattr(cloud_key.bootstrap_key, 'multi_bit', 1) == 2 and not perf_params.single_kernel_bootstrap:
+            raise ValueError('a multi-bit bootstrap key runs on the fused kernel only (single_kernel_bootstrap=True)')
         # lay the bootstrap key out for the fused kernel once, at VM creation rather than at the first gate
         from .tgsw import engine_format, fused_kernel_supported
         if perf_params.single_kernel_bootstrap and fused_kernel_supported(cloud_key.bootstrap_key.bk_params):
@@ -259,7 +264,8 @@ class VirtualMachine:
         tables of shape (F,) + (2^bits,) * digits, or (2^bits,) * digits for one function, indexed
         [f, d_{D-1}, ..., d_0].  Raises ValueError for bits outside {1, 2} and for D < 2 or above what the noise
         allows (tree_lut.max_digits: 4 at bits = 2)."""
-        return TreeLookupTable(self.thread, self.params, tables, bits, digits, out=out)
+        return TreeLookupTable(self.thread, self.params, tables, bits, digits, out=out,
+                               multi_bit=getattr(self.cloud_key.bootstrap_key, 'multi_bit', 1))
 
     def lut_tree(self, tree_key, table, digits, dest=None):
         """f(d_{D-1}, ..., d_0) for the digit ciphertexts `digits` (highest first): one ciphertext, or a list of F for a

@@ -8,7 +8,7 @@ from .numeric_functions import phase_to_t32
 from .lwe import LweParams, LweKey, LweSampleArray, lwe_encrypt, lwe_decrypt, LweKeyswitchKey
 from .tgsw import TGswParams, TGswKey
 from .tlwe import TLweParams
-from .bootstrap import BootstrapKey
+from .bootstrap import BootstrapKey, MultiBitBootstrapKey, check_multi_bit
 from .performance import PerformanceParameters, PerformanceParametersForDevice
 
 
@@ -107,12 +107,15 @@ class NuFHECloudKey:
 
     @classmethod
     def from_rng_with_tgsw_key(cls, thr, params: NuFHEParameters, rng, secret_key: NuFHESecretKey,
-                               perf_params: PerformanceParametersForDevice = None):
-        """(cloud key, TGswKey): the TGSW key, which from_rng discards, is what a tree key is made with."""
+                               perf_params: PerformanceParametersForDevice = None, multi_bit=1):
+        """(cloud key, TGswKey): the TGSW key, which from_rng discards, is what a tree key is made with.
+        multi_bit=2 makes a MultiBitBootstrapKey in the bootstrap key's place (bootstrap.py)."""
+        check_multi_bit(params, multi_bit)
         if perf_params is None:
             perf_params = PerformanceParameters(params).for_device(thr.device_params)
         tgsw_key = TGswKey.from_rng(thr, params.tgsw_params, rng)
-        bk = BootstrapKey.from_rng(thr, rng, secret_key.lwe_key, tgsw_key, perf_params)
+        bk_cls = MultiBitBootstrapKey if multi_bit == 2 else BootstrapKey
+        bk = bk_cls.from_rng(thr, rng, secret_key.lwe_key, tgsw_key, perf_params)
         ks = LweKeyswitchKey.from_tgsw_key(
             thr, rng, params.ks_decomp_length, params.ks_log2_base, secret_key.lwe_key, tgsw_key)
         return cls(params, bk, ks), tgsw_key

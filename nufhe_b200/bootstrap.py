@@ -10,7 +10,7 @@ from .tlwe import (
     TLweSampleArray, tlwe_noiseless_trivial, tlwe_extract_lwe_samples, tlwe_shift_polynomials, tlwe_add_to, tlwe_copy)
 from .tgsw import (
     TGswKey, TransformedTGswSampleArray, TGswParams, TGswSampleArray,
-    tgsw_transform_samples, tgsw_encrypt_int, tgsw_transformed_external_mul, engine_format)
+    tgsw_transform_samples, tgsw_encrypt_int, tgsw_transformed_external_mul, engine_format, fused_kernel_supported)
 
 
 class BootstrapKey:
@@ -42,13 +42,76 @@ class BootstrapKey:
 
     @classmethod
     def load(cls, file_obj, thr):
+        """A BootstrapKey, or the MultiBitBootstrapKey whose pickle starts with its tag."""
         in_out_params = pickle.load(file_obj)
+        if isinstance(in_out_params, str):
+            if in_out_params != MULTI_BIT_TAG:
+                raise ValueError('not a bootstrap key: %r' % in_out_params)
+            in_out_params = pickle.load(file_obj)
+            return MultiBitBootstrapKey(in_out_params, MultiBitTGswSampleArray.load(file_obj, thr))
         tgsw = TransformedTGswSampleArray.load(file_obj, thr)
         return cls(in_out_params, tgsw)
 
     def __eq__(self, other):
         return (self.__class__ == other.__class__ and self.in_out_params == other.in_out_params
                 and self.tgsw == other.tgsw)
+
+
+MULTI_BIT_TAG = 'nufhe_b200.MultiBitBootstrapKey/1'
+
+
+def check_multi_bit(params, multi_bit):
+    """Raise for a `multi_bit` choice the key's parameters cannot take (`params`: NuFHEParameters)."""
+    if isinstance(multi_bit, bool) or not isinstance(multi_bit, int):
+        raise TypeError('multi_bit must be the integer 1 or 2, got %r' % (multi_bit,))
+    if multi_bit not in (1, 2):
+        raise ValueError('multi_bit must be 1 (one key bit per CMux step) or 2 (two), got %d' % multi_bit)
+    if multi_bit == 1:
+        return
+    if params.tgsw_params.tlwe_params.mask_size != 1 or not fused_kernel_supported(params.tgsw_params):
+        raise ValueError('multi-bit bootstrap keys run on the fused kernel only: tlwe_mask_size = 1, the default '
+                         'decomposition and N = 1024')
+    if params.in_out_params.size % 2:
+        raise ValueError('a multi-bit bootstrap key takes the key bits in pairs: the LWE dimension must be even, '
+                         'got %d' % params.in_out_params.size)
+
+
+def multi_bit_messages(key_bits):
+    """The (3n/2,) indicators a multi-bit key encrypts: row 3 g + p - 1 holds [s_2g = b0 and s_2g+1 = b1], p = b0 + 2 b1."""
+    s = key_bits.to(torch.int32).reshape(-1, 2)
+    s0, s1 = s[:, 0], s[:, 1]
+    return torch.stack([s0 * (1 - s1), (1 - s0) * s1, s0 * s1], dim=1).reshape(-1).contiguous()
+
+
+class MultiBitTGswSampleArray(TransformedTGswSampleArray):
+    """The rows of a multi-bit bootstrap key, (3n/2, k+1, l, k+1, N) in the reference's transformed wire format.
+    engine_format lays them out for the multi-bit kernels (nb_bk_prepare_multibit)."""
+    multi_bit = 2
+
+
+class MultiBitBootstrapKey(BootstrapKey):
+    """A bootstrap key that takes the key bits two at a time (DESIGN.md section 14): 3n/2 TGSW rows, row 3 g + p - 1
+    encrypting the indicator [s_2g = b0 and s_2g+1 = b1] of pattern p = b0 + 2 b1 = 1, 2, 3.  The blind rotation runs
+    n/2 steps of ACC += sum_p (X^{k_p} - 1) (Dec(ACC) [x] BK_{g,p}).  Gates, lookup tables and lut_tree take it as they
+    take a BootstrapKey; the separate-step bootstrap (single_kernel_bootstrap=False) and blind_rotate do not."""
+    multi_bit = 2
+
+    @classmethod
+    def from_rng(cls, thr, rng, lwe_key: LweKey, tgsw_key: TGswKey, perf_params=None):
+        """The rows are drawn where a BootstrapKey's are, 3n/2 TGSW encryptions in row order."""
+        in_out_params = lwe_key.params
+        bk_params = tgsw_key.params
+        accum_params = bk_params.tlwe_params
+        rows = 3 * in_out_params.size // 2
+        bk = TGswSampleArray.empty(thr, bk_params, (rows,))
+        tgsw_encrypt_int(thr, rng, bk, multi_bit_messages(lwe_key.key), accum_params.min_noise, tgsw_key, perf_params)
+        bk_transformed = MultiBitTGswSampleArray.empty(thr, bk_params, (rows,))
+        tgsw_transform_samples(thr, bk_transformed, bk, perf_params)
+        return cls(in_out_params, bk_transformed)
+
+    def dump(self, file_obj):
+        pickle.dump(MULTI_BIT_TAG, file_obj)
+        BootstrapKey.dump(self, file_obj)
 
 
 def _flat(sample: LweSampleArray):
@@ -93,7 +156,10 @@ def bootstrap_affine(thr, result: LweSampleArray, bk: BootstrapKey, ks: LweKeysw
 def _single_kernel(perf_params, bk=None):
     """Which bootstrap path to take.  Without explicit performance parameters: the fused kernel whenever the key's
     parameters allow it (what `PerformanceParameters(params).for_device(...)` would say)."""
-    from .tgsw import fused_kernel_supported
+    if getattr(bk, 'multi_bit', 1) == 2:
+        if perf_params is not None and getattr(perf_params, 'single_kernel_bootstrap', True) is False:
+            raise ValueError('a multi-bit bootstrap key runs on the fused kernel only (single_kernel_bootstrap=True)')
+        return True
     if perf_params is None:
         return bk is None or fused_kernel_supported(bk.bk_params)
     return getattr(perf_params, 'single_kernel_bootstrap', True) is not False

@@ -24,7 +24,7 @@ import torch
 from .lwe import LweParams, LweSampleArray, LweKey, LweKeyswitchKey, make_lwe_keyswitch_key
 from .tlwe import tlwe_encrypt_zero_with_masks
 from .tgsw import TGswKey, TGswSampleArray, TransformedTGswSampleArray, tgsw_transform_samples
-from .bootstrap import BootstrapKey
+from .bootstrap import BootstrapKey, MultiBitBootstrapKey, MultiBitTGswSampleArray, check_multi_bit, multi_bit_messages
 from .random_numbers import rand_gaussian_torus32
 
 NONCE_CIPHERTEXT, NONCE_BOOTSTRAP_KEY, NONCE_KEYSWITCH_KEY = 0, 1, 2
@@ -164,20 +164,23 @@ class CompressedCloudKey:
         return cls.from_rng_with_tgsw_key(thr, params, rng, secret_key)[0]
 
     @classmethod
-    def from_rng_with_tgsw_key(cls, thr, params, rng, secret_key):
-        """(compressed cloud key, TGswKey), as NuFHECloudKey.from_rng_with_tgsw_key."""
+    def from_rng_with_tgsw_key(cls, thr, params, rng, secret_key, multi_bit=1):
+        """(compressed cloud key, TGswKey), as NuFHECloudKey.from_rng_with_tgsw_key.  multi_bit=2: the 3n/2 rows of a
+        MultiBitBootstrapKey take the bootstrap key's place (bodies, masks and draws), which `decompress` restores."""
+        check_multi_bit(params, multi_bit)
         lwe_key = secret_key.lwe_key
         tgsw_key = TGswKey.from_rng(thr, params.tgsw_params, rng)
         seed = draw_seed(rng)
         bk_params = params.tgsw_params
         tl = bk_params.tlwe_params
         n = lwe_key.params.size
+        rows, messages = (3 * n // 2, multi_bit_messages(lwe_key.key)) if multi_bit == 2 else (n, lwe_key.key)
 
-        bk = TGswSampleArray.empty(thr, bk_params, (n,))
+        bk = TGswSampleArray.empty(thr, bk_params, (rows,))
         noises2 = rand_gaussian_torus32(thr, rng, 0, tl.min_noise, bk.samples.shape + (tl.polynomial_degree,))
-        tlwe_encrypt_zero_with_masks(thr, bk.samples, _bk_masks(thr, seed, bk_params, n), noises2, tl.min_noise,
+        tlwe_encrypt_zero_with_masks(thr, bk.samples, _bk_masks(thr, seed, bk_params, rows), noises2, tl.min_noise,
                                      tgsw_key.tlwe_key)
-        tgsw_add_message_seeded(thr, bk, lwe_key.key, tgsw_key)
+        tgsw_add_message_seeded(thr, bk, messages, tgsw_key)
         k = tl.mask_size
         bk_body = bk.samples.a.coeffs[..., k, :].contiguous()
 
@@ -198,14 +201,16 @@ class CompressedCloudKey:
         bk_params = params.tgsw_params
         k = bk_params.tlwe_params.mask_size
         n = params.in_out_params.size
-        bk = TGswSampleArray.empty(thr, bk_params, (n,))
+        rows = self.bk_body.shape[0]                 # n, or 3n/2 for a multi-bit key
+        bk = TGswSampleArray.empty(thr, bk_params, (rows,))
         coeffs = bk.samples.a.coeffs
-        coeffs[..., :k, :] = _bk_masks(thr, self.seed, bk_params, n)
+        coeffs[..., :k, :] = _bk_masks(thr, self.seed, bk_params, rows)
         coeffs[..., k, :] = self.bk_body.to(coeffs.device)
         bk.samples.current_variances.fill_(self.bk_variance)
-        bk_transformed = TransformedTGswSampleArray.empty(thr, bk_params, (n,))
+        multi = rows != n
+        bk_transformed = (MultiBitTGswSampleArray if multi else TransformedTGswSampleArray).empty(thr, bk_params, (rows,))
         tgsw_transform_samples(thr, bk_transformed, bk)
-        bootstrap_key = BootstrapKey(params.in_out_params, bk_transformed)
+        bootstrap_key = (MultiBitBootstrapKey if multi else BootstrapKey)(params.in_out_params, bk_transformed)
 
         in_size, t, base = self.ks_b.shape
         ks = LweSampleArray.empty(thr, params.in_out_params, (in_size, t, base))

@@ -1195,7 +1195,9 @@ static_assert(BK_ROW_U64 == BK_NTT_U64 + BK_FFT_U64, "key row layout");
 // table (tables.h: FftTables), complex: the pass-1 twiddles merged with the n0 part of the twist,
 // T[k1][n0] = w^n0 W512^(n0 k1), stored [k1][n0] so that the consecutive n0 of a warp read consecutive 16-byte
 // elements.  The rest of the twist, w^(64 m), and the pass-2 twiddles are compile-time constants (fft_w64).
-constexpr int FFT_TAB_T1 = 0, FFT_TAB_CPLX = 512;
+// The device copy continues at FFT_TAB_ROOTS with the multi-bit step's 2048th roots of unity R[e] = e^{2 pi i e / 2048}
+// (FftTables::roots; fft_phase_mac_mb).
+constexpr int FFT_TAB_T1 = 0, FFT_TAB_CPLX = 512, FFT_TAB_ROOTS = FFT_TAB_CPLX, FFT_ROOTS = 2048;
 NB_HD constexpr int fft_tab_t1(int k1, int n0) { return FFT_TAB_T1 + k1 * 64 + n0; }
 
 #if defined(__CUDA_ARCH__)
@@ -1544,6 +1546,64 @@ NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
         static_for<0, 4>([&](auto I) { st_cplx(spec_all + fft_pass3_pos(tid, s, decltype(I)::value), o[decltype(I)::value]); });
     }
 }
+// Multi-bit key (DESIGN.md section 14): one step handles the key bits s_2g, s_2g+1 of group g,
+//     ACC += sum_{p = 1..3} (X^{k_p} - 1) (Dec(ACC) [x] BK_{g,p}),   k_1 = abar_2g, k_2 = abar_2g+1, k_3 = k_1 + k_2,
+// so pass 3 runs the MAC against the 3 key rows of the group and multiplies each row's product by zeta_f^{k_p} - 1 at
+// its spectral point.  Bin f = k1 + 8 k2 + 128 k3 of the folded transform evaluates the polynomial at
+// zeta_f = e^{2 pi i (1 - 4 f) / 2048}, so zeta_f^k = R[k (1 - 4 k1 - 32 k2) mod 2048] (-i)^(k k3): one table value per
+// row and thread, and an exact quarter turn per output k3.
+// z (-i)^r, exact (swap and sign)
+NB_HD cplx c_quarter_turns(cplx z, int r)
+{
+    const bool sw = r & 1, neg_re = (r >> 1) & 1, neg_im = ((r >> 1) ^ r) & 1;
+    const double x = sw ? z.im : z.re, y = sw ? z.re : z.im;
+    return {neg_re ? -x : x, neg_im ? -y : y};
+}
+// key: the group's 3 key rows (BK_FFT_U64 each, patterns p = 1, 2, 3 in order); rot: the group's two rotation amounts
+// of both ciphertexts, [ct][2]
+NB_HD void fft_phase_mac_mb(int tid, cplx *spec_all, const cplx *key, const cplx *tab, const int *rot)
+{
+    const int j = tid >> 1, ct = tid & 1, g = fft_pass3_group(j);
+    const int a0 = rot[2 * ct], a1 = rot[2 * ct + 1];
+    const int kp[3] = {a0, a1, (a0 + a1) & (2 * NTT_N - 1)};
+    const int e0 = 1 - 4 * (g >> 4) - 32 * (g & 15);
+    cplx zb[3];
+    static_for<0, 3>([&](auto P) {
+        constexpr int p = decltype(P)::value;
+        zb[p] = ld_cplx_tab(tab + FFT_TAB_ROOTS + ((kp[p] * e0) & (2 * NTT_N - 1)));
+    });
+    cplx dg[4][4];
+    static_for<0, 4>([&](auto D) {
+        static_for<0, 4>([&](auto I) { dg[decltype(D)::value][decltype(I)::value] = ld_cplx(spec_all + fft_pass3_pos(tid, decltype(D)::value, decltype(I)::value)); });
+        dft4<false>(dg[decltype(D)::value]);
+    });
+#if defined(__CUDA_ARCH__)
+#pragma unroll 1
+#endif
+    for (int s = 0; s < 4; s++) {
+        cplx o[4];
+        static_for<0, 4>([&](auto K3) {
+            constexpr int k3 = decltype(K3)::value;
+            static_for<0, 3>([&](auto P) {
+                constexpr int p = decltype(P)::value;
+                const cplx *kr = key + p * (BK_FFT_U64 / 2);
+                cplx k[4];
+                static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(kr + fft_key_pos(4 * decltype(D)::value + s, j, k3)); });
+                cplx v = {d_mul(dg[0][k3].re, k[0].re), d_mul(dg[0][k3].re, k[0].im)};
+                v = {d_fma(-dg[0][k3].im, k[0].im, v.re), d_fma(dg[0][k3].im, k[0].re, v.im)};
+                static_for<1, 4>([&](auto D) { v = c_mac(v, dg[decltype(D)::value][k3], k[decltype(D)::value]); });
+                // zeta_f^{k_p} - 1: the rounded table value turned exactly, then one rounded subtraction
+                cplx f = c_quarter_turns(zb[p], (kp[p] * k3) & 3);
+                f.re = d_sub(f.re, 1.0);
+                if constexpr (p == 0) o[k3] = c_mul(v, f);
+                else o[k3] = c_mac(o[k3], v, f);
+            });
+        });
+        dft4<true>(o);
+        static_for<0, 4>([&](auto I) { st_cplx(spec_all + fft_pass3_pos(tid, s, decltype(I)::value), o[decltype(I)::value]); });
+    }
+}
+
 // inv1: task (pp = ct * 2 + mo, n0): both key halves of output polynomial mo, rounded and recombined mod 2^32.
 // ACCUMULATE: acc += result, else acc = result.
 template <bool ACCUMULATE> NB_HD void fft_phase_inv1(int task, i32 *acc_all, const cplx *spec_all, const cplx *tab)

@@ -20,6 +20,9 @@ struct nb_ctx {
     // engine keys prepared on this context whose coefficients are centred 32-bit integers: they carry the spectra of
     // the FP64 step, which the throughput shape runs on them (begin, end of the key's rows)
     std::vector<std::pair<const u64 *, const u64 *>> spectral_keys;
+    // multi-bit keys prepared on this context (nb_bk_prepare_multibit): 3 rows of spectra per group of two key bits,
+    // which every launch with them runs on the FP64 step (begin, end of the key's rows)
+    std::vector<std::pair<const u64 *, const u64 *>> multibit_keys;
     int fft;                             // developer knob: 0 keeps the NTT step for every key
     int sm_count;
     size_t wide_max;                     // largest batch launched in the wide (1 ciphertext / 256 threads) shape
@@ -88,9 +91,9 @@ struct NvtxRange {
 // A CTA of the fused bootstrap's work queue may wait for work that another resident CTA produces, so all the
 // sm_count x CTAS_PER_SM CTAs a launch is sized for must be co-resident: fail at context creation instead of hanging.
 // (the gate kernel and the programmable-bootstrap kernel of each shape)
-template <class Cfg> static int check_resident(nb_ctx *ctx)
+template <class Cfg, bool MB = false> static int check_resident(nb_ctx *ctx)
 {
-    for (auto kernel : {blind_rotate_kernel<Cfg>, blind_rotate_kernel<Cfg, true>}) {
+    for (auto kernel : {blind_rotate_kernel<Cfg, false, MB>, blind_rotate_kernel<Cfg, true, MB>}) {
         int n = 0;
         NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<Cfg>()),
                      "cudaFuncSetAttribute(blind_rotate)"));
@@ -151,8 +154,9 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check(ctx, cudaMemcpy(ctx->d_ones512, pt.ones512.data(), NTT_N * sizeof(u64), cudaMemcpyHostToDevice), "memcpy"));
     {
         FftTables ft;
-        NB_TRY(check(ctx, cudaMalloc(&ctx->d_fft_tab, FFT_TAB_CPLX * sizeof(cplx)), "cudaMalloc"));
+        NB_TRY(check(ctx, cudaMalloc(&ctx->d_fft_tab, (FFT_TAB_CPLX + FFT_ROOTS) * sizeof(cplx)), "cudaMalloc"));
         NB_TRY(check(ctx, cudaMemcpy(ctx->d_fft_tab, ft.tab.data(), FFT_TAB_CPLX * sizeof(cplx), cudaMemcpyHostToDevice), "memcpy"));
+        NB_TRY(check(ctx, cudaMemcpy(ctx->d_fft_tab + FFT_TAB_ROOTS, ft.roots.data(), FFT_ROOTS * sizeof(cplx), cudaMemcpyHostToDevice), "memcpy"));
     }
     // (check_resident sets the shared-memory limit of the single-CTA shapes)
     for (auto kernel : {blind_rotate_pair_kernel<true>, blind_rotate_pair_kernel<false>, blind_rotate_pair_kernel<true, true>,
@@ -165,6 +169,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check_resident<BrWide>(ctx));
     NB_TRY(check_resident<BrWide2>(ctx));
     NB_TRY(check_resident<BrFft>(ctx));
+    NB_TRY((check_resident<BrFft, true>(ctx)));
     {   // batches that fit one wave of wide CTAs (one ciphertext on 256 threads) take the low-latency shape
         const char *e = getenv("NUFHE_B200_WIDE_MAX");
         // up to one wave the wide shape has the shortest step; between one and ~1.7 waves it still wins, time-sliced
@@ -325,6 +330,21 @@ int nb_ff_elementwise(nb_ctx *ctx, int op, const uint64_t *a, const uint64_t *b,
 }
 
 size_t nb_bk_row_u64(void) { return BK_ROW_U64; }
+size_t nb_bk_multibit_row_u64(void) { return BK_FFT_U64; }
+
+}  // extern "C"
+
+// forget the registrations of keys that [begin, end) overwrites
+static void forget_keys(nb_ctx *ctx, const u64 *begin, const u64 *end)
+{
+    for (auto *keys : {&ctx->spectral_keys, &ctx->multibit_keys})
+        for (size_t i = 0; i < keys->size();) {
+            if ((*keys)[i].first < end && begin < (*keys)[i].second) keys->erase(keys->begin() + i);
+            else i++;
+        }
+}
+
+extern "C" {
 
 int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t rows)
 {
@@ -339,10 +359,7 @@ int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t 
     // the FP64 part of every row: key polynomials back to coefficients (plain form, inverse transform), integrality
     // check, 16-bit split, spectra (kernels.cuh: bk_spectra_kernel)
     const u64 *key_begin = (const u64 *)bk_int, *key_end = key_begin + rows * BK_ROW_U64;
-    for (size_t i = 0; i < ctx->spectral_keys.size();) {       // forget keys this one overwrites
-        if (ctx->spectral_keys[i].first < key_end && key_begin < ctx->spectral_keys[i].second) ctx->spectral_keys.erase(ctx->spectral_keys.begin() + i);
-        else i++;
-    }
+    forget_keys(ctx, key_begin, key_end);
     const size_t polys = rows * 8, words = polys * NTT_N;
     u64 *tmp = nullptr;
     NB_TRY(check(ctx, cudaMalloc(&tmp, 2 * words * sizeof(u64) + sizeof(int)), "cudaMalloc(bk_prepare)"));
@@ -352,7 +369,7 @@ int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t 
         blocks = (words + 255) / 256;
         bk_plain_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>((const u64 *)bk_ref, tmp, words);
         ntt_inverse_kernel<false><<<ntt_grid(ctx, polys), NTT_SWEEP_THREADS, ntt_smem_bytes(NTT_RAW_U64_BYTES), ctx->stream>>>(tmp, tmp + words, ctx->d_ph_inv, polys);
-        bk_spectra_kernel<<<(unsigned)polys, 64, 0, ctx->stream>>>(tmp + words, (u64 *)bk_int, ctx->d_fft_tab, d_flag);
+        bk_spectra_kernel<<<(unsigned)polys, 64, 0, ctx->stream>>>(tmp + words, (u64 *)bk_int, ctx->d_fft_tab, d_flag, BK_ROW_U64, BK_NTT_U64);
         rc = launch_check(ctx, "bk_spectra_kernel");
     }
     if (rc == NB_OK) rc = check(ctx, cudaMemcpyAsync(&not_integral, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream), "cudaMemcpyAsync");
@@ -360,6 +377,38 @@ int nb_bk_prepare(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_int, size_t 
     cudaFree(tmp);
     NB_TRY(rc);
     if (!not_integral) ctx->spectral_keys.emplace_back(key_begin, key_end);
+    return NB_OK;
+}
+
+int nb_bk_prepare_multibit(nb_ctx *ctx, const uint64_t *bk_ref, uint64_t *bk_mb, size_t groups)
+{
+    if (!ctx || !bk_ref || !bk_mb) return fail(ctx, NB_EINVAL, "nb_bk_prepare_multibit: null argument");
+    if (groups == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:bk_prepare_multibit");
+    const u64 *key_begin = (const u64 *)bk_mb, *key_end = key_begin + 3 * groups * BK_FFT_U64;
+    forget_keys(ctx, key_begin, key_end);
+    // as the FP64 part of nb_bk_prepare: coefficients (plain form, inverse transform), integrality check, 16-bit split,
+    // spectra; only the spectra are stored
+    const size_t polys = 3 * groups * 8, words = polys * NTT_N;
+    const size_t blocks = (words + 255) / 256, cap = (size_t)ctx->sm_count * 16;
+    u64 *tmp = nullptr;
+    NB_TRY(check(ctx, cudaMalloc(&tmp, 2 * words * sizeof(u64) + sizeof(int)), "cudaMalloc(bk_prepare_multibit)"));
+    int *d_flag = (int *)(tmp + 2 * words), not_integral = 0;
+    int rc = check(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), ctx->stream), "cudaMemsetAsync");
+    if (rc == NB_OK) {
+        bk_plain_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>((const u64 *)bk_ref, tmp, words);
+        ntt_inverse_kernel<false><<<ntt_grid(ctx, polys), NTT_SWEEP_THREADS, ntt_smem_bytes(NTT_RAW_U64_BYTES), ctx->stream>>>(tmp, tmp + words, ctx->d_ph_inv, polys);
+        bk_spectra_kernel<<<(unsigned)polys, 64, 0, ctx->stream>>>(tmp + words, (u64 *)bk_mb, ctx->d_fft_tab, d_flag, BK_FFT_U64, 0);
+        rc = launch_check(ctx, "bk_spectra_kernel(multi-bit)");
+    }
+    if (rc == NB_OK) rc = check(ctx, cudaMemcpyAsync(&not_integral, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream), "cudaMemcpyAsync");
+    if (rc == NB_OK) rc = check(ctx, cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize");
+    cudaFree(tmp);
+    NB_TRY(rc);
+    // a multi-bit key has no NTT form to fall back on
+    if (not_integral) return fail(ctx, NB_EINVAL, "nb_bk_prepare_multibit: key coefficients are not centred 32-bit integers");
+    ctx->multibit_keys.emplace_back(key_begin, key_end);
     return NB_OK;
 }
 
@@ -394,15 +443,17 @@ static int reserve_words(nb_ctx *ctx, void **buf, size_t *have, size_t want, siz
     return NB_OK;
 }
 
-template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
+// MB: a multi-bit key, whose chains are p.n / 2 groups long
+template <class Cfg, bool MB = false> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
 {
     const size_t slots = (size_t)ctx->sm_count * Cfg::CTAS_PER_SM;
     const size_t chains = (p.batch + Cfg::CT - 1) / Cfg::CT;
-    int chunks = p.plain ? 1 : pick_chunks(chains, slots, p.n, ctx->max_chunks);
-    if (!p.plain && ctx->force_chunks > 0 && chains > slots) chunks = ctx->force_chunks < p.n ? ctx->force_chunks : p.n;
+    const int nsteps = MB ? p.n / 2 : p.n;
+    int chunks = p.plain ? 1 : pick_chunks(chains, slots, nsteps, ctx->max_chunks);
+    if (!p.plain && ctx->force_chunks > 0 && chains > slots) chunks = ctx->force_chunks < nsteps ? ctx->force_chunks : nsteps;
     p.chains = (unsigned)chains;
-    p.steps_per_chunk = p.plain ? 1 : (p.n + chunks - 1) / chunks;
-    chunks = p.plain ? 1 : (p.n + p.steps_per_chunk - 1) / p.steps_per_chunk;
+    p.steps_per_chunk = p.plain ? 1 : (nsteps + chunks - 1) / chunks;
+    chunks = p.plain ? 1 : (nsteps + p.steps_per_chunk - 1) / p.steps_per_chunk;
     p.chunks = (unsigned)chunks;
     p.sched = nullptr; p.state = nullptr;
     p.sm_count = ctx->sm_count; p.stagger_cycles = ctx->stagger_cycles;
@@ -419,8 +470,8 @@ template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
         p.sched = ctx->d_sched; p.state = ctx->d_state;
         grid = slots;
     }
-    if (p.tv) blind_rotate_kernel<Cfg, true><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
-    else blind_rotate_kernel<Cfg><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
+    if (p.tv) blind_rotate_kernel<Cfg, true, MB><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
+    else blind_rotate_kernel<Cfg, false, MB><<<(int)grid, Cfg::THREADS, br_smem_bytes<Cfg>(), ctx->stream>>>(p, ctx->d_ph_fwd, ctx->d_ph_inv);
     return NB_OK;
 }
 
@@ -429,6 +480,16 @@ template <class Cfg> static int launch_br_cfg(nb_ctx *ctx, BlindRotateArgs &p)
 // step when the key has spectra.
 static int launch_br(nb_ctx *ctx, BlindRotateArgs &p)
 {
+    for (const auto &k : ctx->multibit_keys) {
+        if (p.bk < k.first || k.second <= p.bk) continue;
+        // a multi-bit key: the FP64 throughput shape at every batch size.  The explicit-accumulator calls
+        // (nb_blind_rotate, nb_external_product) have the per-bit semantics of the reference's key, which this key lacks.
+        if (p.plain || p.accum || p.bara)
+            return fail(ctx, NB_EUNSUPPORTED, "a multi-bit bootstrap key serves the fused bootstrap entry points only");
+        if (p.n % 2 || p.bk + (size_t)(p.n / 2) * 3 * BK_FFT_U64 > k.second)
+            return fail(ctx, NB_EINVAL, "the multi-bit key has fewer groups than n / 2, or n is odd");
+        return launch_br_cfg<BrFft, true>(ctx, p);
+    }
     if (!p.plain && p.n > 0 && p.batch <= ctx->pair_max) {
         p.sched = nullptr; p.state = nullptr; p.chains = (unsigned)p.batch; p.chunks = 1; p.steps_per_chunk = p.n;
         p.sm_count = ctx->sm_count; p.stagger_cycles = 0;

@@ -315,6 +315,36 @@ int emul_fft_step(i32 *acc_io, const u64 *bk_ref_row, const int *rot, int nct)
     return 0;
 }
 
+// One group of the multi-bit step (br_fft_step<true, BrFft, true>) for nct <= 2 ciphertexts, phase by phase: the 3
+// reference rows of the group (bk_ref_rows, each 8 x 1024 u64) and rot[c * 2 + b] = abar_{2g + b} of ciphertext c;
+// acc_io (nct, 2, 1024) is updated.  Returns -1 for a key without integral coefficients.
+int emul_fft_group_mb(i32 *acc_io, const u64 *bk_ref_rows, const int *rot, int nct)
+{
+    static FftTables F;
+    using Cfg = BrFft;
+    std::vector<cplx> key(3 * BK_FFT_SPECTRA * FFT_M), row;
+    for (int p = 0; p < 3; p++) {
+        if (fft_key_row(bk_ref_rows + (size_t)p * 8 * NTT_N, row)) return -1;
+        memcpy(key.data() + (size_t)p * BK_FFT_SPECTRA * FFT_M, row.data(), row.size() * sizeof(cplx));
+    }
+    // the device table: pass-1 table, then the roots at FFT_TAB_ROOTS
+    std::vector<cplx> tab(F.tab);
+    tab.insert(tab.end(), F.roots.begin(), F.roots.end());
+    std::vector<i32> acc(Cfg::CT * 2 * NTT_N, 0);
+    std::vector<cplx> w(Cfg::POLYS * FFT_SPEC_CPLX, cplx{1e300, -1e300});
+    for (int c = 0; c < nct; c++) memcpy(&acc[c * 2 * NTT_N], acc_io + c * 2 * NTT_N, sizeof(i32) * 2 * NTT_N);
+    int rots[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 2 * nct; i++) rots[i] = rot[i];
+    constexpr int TH = Cfg::THREADS;
+    for (int tid = 0; tid < TH; tid++) fft_phase_fwd1<false>(tid, acc.data(), w.data(), tab.data(), rots);
+    for (int tid = 0; tid < TH; tid++) fft_phase_fwd2(tid, w.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_mac_mb(tid, w.data(), key.data(), tab.data(), rots);
+    for (int tid = 0; tid < TH; tid++) fft_phase_inv2(tid, w.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_inv1<true>(tid, acc.data(), w.data(), tab.data());
+    for (int c = 0; c < nct; c++) memcpy(acc_io + c * 2 * NTT_N, &acc[c * 2 * NTT_N], sizeof(i32) * 2 * NTT_N);
+    return 0;
+}
+
 // The transform chain of the FP64 step on given inputs, for the exactness tests: digit polynomials dig[4][1024] (signed,
 // |d| <= 512) and key polynomials key[4][1024] (centred 32-bit); out[h][1024] = the UNROUNDED coefficients of
 // sum_d dig_d * key_d,h mod X^1024 + 1 for the key halves h = 0 (lo), 1 (hi), through the same passes and MAC as the
@@ -344,6 +374,46 @@ void emul_fft_product(const double *dig, const long long *key, double *out)
         double xl[16], xh[16];
         fft_inv1(n0, w.data() + fft_pass1_spec(n0, 0), tab, xl);
         fft_inv1(n0, w.data() + fft_pass1_spec(n0, 1), tab, xh);
+        for (int j = 0; j < 16; j++) {
+            out[0 * NTT_N + 64 * j + n0] = xl[j];
+            out[1 * NTT_N + 64 * j + n0] = xh[j];
+        }
+    }
+}
+
+// The multi-bit chain on given inputs, for the exactness tests: digit polynomials dig[4][1024] (signed, |d| <= 512),
+// key polynomials key[3][4][1024] (row p = 0, 1, 2 of a group, digit d; centred 32-bit) and the group's rotation
+// amounts rot[2] = (abar_2g, abar_2g+1); out[h][1024] = the UNROUNDED coefficients of
+// sum_p (X^{k_p} - 1) sum_d dig_d * key_{p,d},h mod X^1024 + 1 for the key halves h = 0 (lo), 1 (hi), through the same
+// passes and pass-3 MAC (fft_phase_mac_mb) as the kernel (one ciphertext, one output polynomial).
+void emul_fft_product_mb(const double *dig, const long long *key, const int *rot, double *out)
+{
+    static FftTables F;
+    std::vector<cplx> tab(F.tab);
+    tab.insert(tab.end(), F.roots.begin(), F.roots.end());
+    std::vector<cplx> ks(3 * BK_FFT_SPECTRA * FFT_M, cplx{0, 0});
+    for (int p = 0; p < 3; p++)
+        for (int d = 0; d < 4; d++)
+            fft_key_spectra(key + (p * 4 + d) * NTT_N, ks.data() + (size_t)p * BK_FFT_SPECTRA * FFT_M + (d * 2 + 0) * 2 * FFT_M, F);
+    std::vector<cplx> w(BrFft::POLYS * FFT_SPEC_CPLX, cplx{0, 0});
+    const int rots[4] = {rot[0], rot[1], 0, 0};
+    for (int tid = 0; tid < 128; tid++) {               // fwd1 of ciphertext 0: digit polynomials mi * 2 + 0 / 1
+        const int n0 = tid & 63, mi = tid >> 6;
+        double xa[16], xb[16];
+        for (int j = 0; j < 16; j++) {
+            xa[j] = dig[(mi * 2 + 0) * NTT_N + 64 * j + n0];
+            xb[j] = dig[(mi * 2 + 1) * NTT_N + 64 * j + n0];
+        }
+        fft_fwd1(n0, xa, w.data() + fft_pass1_spec(tid, 0), tab.data());
+        fft_fwd1(n0, xb, w.data() + fft_pass1_spec(tid, 1), tab.data());
+    }
+    for (int tid = 0; tid < 128; tid++) fft_phase_fwd2(tid, w.data());
+    for (int tid = 0; tid < 256; tid += 2) fft_phase_mac_mb(tid, w.data(), ks.data(), tab.data(), rots);
+    for (int tid = 0; tid < 128; tid++) fft_phase_inv2(tid, w.data());
+    for (int n0 = 0; n0 < 64; n0++) {
+        double xl[16], xh[16];
+        fft_inv1(n0, w.data() + fft_pass1_spec(n0, 0), tab.data(), xl);
+        fft_inv1(n0, w.data() + fft_pass1_spec(n0, 1), tab.data(), xh);
         for (int j = 0; j < 16; j++) {
             out[0 * NTT_N + 64 * j + n0] = xl[j];
             out[1 * NTT_N + 64 * j + n0] = xh[j];

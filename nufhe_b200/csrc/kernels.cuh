@@ -283,8 +283,11 @@ __global__ void bk_plain_kernel(const u64 *__restrict__ bk_ref, u64 *__restrict_
 // One CTA of 64 threads per key polynomial (blockIdx.x = row * 8 + m): its coefficients mod p (natural order) must be
 // centred 32-bit integers; they are split into 16-bit halves and both halves transformed with the passes of the
 // bootstrap.  A coefficient outside [-2^31, 2^31) sets *not_integral (the key then keeps the NTT step everywhere).
+// The spectra of row r go to bk_int + r * row_u64 + row_offset: after the NTT planes of an engine key row
+// (BK_ROW_U64, BK_NTT_U64), or alone (BK_FFT_U64, 0: a multi-bit key).
 __global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ coef, u64 *__restrict__ bk_int,
-                                                        const cplx *__restrict__ tab, int *__restrict__ not_integral)
+                                                        const cplx *__restrict__ tab, int *__restrict__ not_integral,
+                                                        size_t row_u64, size_t row_offset)
 {
     __shared__ __align__(16) cplx spec[2][FFT_SPEC_CPLX];
     const size_t poly = blockIdx.x, row = poly >> 3;
@@ -311,7 +314,7 @@ __global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ 
     __syncthreads();
     for (int t = n0; t < 2 * FFT_M / 4; t += 64) fft_fwd3(t & 127, spec[t >> 7]);
     __syncthreads();
-    cplx *out = reinterpret_cast<cplx *>(bk_int + row * BK_ROW_U64 + BK_NTT_U64);
+    cplx *out = reinterpret_cast<cplx *>(bk_int + row * row_u64 + row_offset);
     for (int P = n0; P < FFT_M; P += 64)
         for (int h = 0; h < 2; h++) out[fft_key_pos(m * 2 + h, P & 127, P >> 7)] = spec[h][fft_pass3_x(fft_pass3_group(P & 127), P >> 7)];
 }
@@ -547,20 +550,24 @@ NB_D int fft_step_tid()
 }
 
 // The FP64 step (br_phases.cuh: FP64 step): five barrier-separated phases on spectra of 512 complex doubles, one task
-// per thread in each; bk_row: the whole engine key row (its FP64 part is read)
-template <bool ROTATE, class Cfg>
+// per thread in each; bk_row: the whole engine key row (its FP64 part is read).
+// MB: one group of a multi-bit key (br_phases.cuh: fft_phase_mac_mb): bk_row = the group's 3 rows of spectra, rot = the
+// group's two rotation amounts per ciphertext; fwd1 decomposes ACC itself and inv1 adds to it.
+template <bool ROTATE, class Cfg, bool MB = false>
 NB_D void br_fft_step(const Br2Smem &s, const u64 *__restrict__ bk_row, const int *rot, int /* tid */, const cplx *__restrict__ tab)
 {
     static_assert(Cfg::CT == FFT_CT && Cfg::THREADS == 256, "the FP64 step's thread maps (fft_layout.cuh)");
+    static_assert(!MB || ROTATE, "a multi-bit group always accumulates");
     cplx *spec = reinterpret_cast<cplx *>(s.w);
     int tid = fft_step_tid();
-    fft_phase_fwd1<ROTATE>(tid, s.acc, spec, tab, rot);          // (ct, mi, n0), both digits
+    fft_phase_fwd1<ROTATE && !MB>(tid, s.acc, spec, tab, rot);   // (ct, mi, n0), both digits
     __syncthreads();
     tid = fft_step_tid();
     fft_phase_fwd2(tid, spec);                              // (ct, n2, s, k1): DFT16, W64 twiddles
     __syncthreads();
     tid = fft_step_tid();
-    fft_phase_mac(tid, spec, reinterpret_cast<const cplx *>(bk_row + BK_NTT_U64));   // (j, ct): DFT4, MAC, inverse DFT4
+    if constexpr (MB) fft_phase_mac_mb(tid, spec, reinterpret_cast<const cplx *>(bk_row), tab, rot);   // (j, ct): DFT4, 3-row MAC, inverse DFT4
+    else fft_phase_mac(tid, spec, reinterpret_cast<const cplx *>(bk_row + BK_NTT_U64));   // (j, ct): DFT4, MAC, inverse DFT4
     __syncthreads();
     tid = fft_step_tid();
     fft_phase_inv2(tid, spec);                              // (ct, n2, s, k1)
@@ -580,6 +587,13 @@ NB_D void st_release_u32(unsigned *p, unsigned v)
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
+// steps of a chain: p.n, or p.n / 2 groups of a multi-bit key (read where used, so that the other kernels keep their code)
+template <bool MB> NB_D int br_chain_steps(const BlindRotateArgs &p)
+{
+    if constexpr (MB) return p.n / 2;
+    else return p.n;
+}
+
 // The kernel is persistent: the grid is at most one wave of resident CTAs (Cfg::CTAS_PER_SM per SM) and every CTA
 // pulls work items from a queue until none are left.  A work item is one CHUNK of one CHAIN: a chain is the whole
 // blind rotation of Cfg::CT ciphertexts, a chunk `steps_per_chunk` consecutive CMux steps of it.  Cutting chains into
@@ -595,10 +609,13 @@ NB_D void st_release_u32(unsigned *p, unsigned v)
 // and a ready chain never waits behind an unready one -- with in-order tickets and per-chain progress counters, which
 // this replaces, a launch with slightly more chains than CTAs lost time to such head-of-line waits.
 // LUT: the programmable bootstrap (BlindRotateArgs::tv); its own instantiation, so that the gate kernels keep their code.
-template <class Cfg, bool LUT = false>
+// MB: a multi-bit key (BrFft only): a chain is p.n / 2 groups of two key bits instead of p.n steps, p.bk holds 3 rows of
+// BK_FFT_U64 per group, and s.rot holds both rotation amounts of the group per ciphertext ([parity][CT][2]).
+template <class Cfg, bool LUT = false, bool MB = false>
 __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g,
                                                                        const u64 *__restrict__ twd_inv_g)
 {
+    static_assert(!MB || Cfg::FFT, "multi-bit keys run the FP64 step");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Br2Smem s = br2_carve<Cfg>(smem_raw);
     __shared__ unsigned s_item, s_entry;
@@ -647,7 +664,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
         // ciphertext slots beyond the batch replay the last ciphertext and store nothing
         auto ct_of = [&](int slot) { size_t c = ct0 + slot; return c < p.batch ? c : p.batch - 1; };
         const int step0 = (int)chunk * p.steps_per_chunk;
-        const int step1 = p.plain ? 1 : min(p.n, step0 + p.steps_per_chunk);
+        const int step1 = p.plain ? 1 : min(br_chain_steps<MB>(p), step0 + p.steps_per_chunk);
 
         if (chunk == 0) {
             // accumulator initialisation: CT x 2 polynomials x 1024 coefficients
@@ -666,11 +683,22 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
             br2_stage_key(s.key, p.bk + (size_t)(p.plain ? 0 : step0) * BK_ROW_U64, tid, Cfg::THREADS);
             cp_async_wait<0>();
         }
-        if (p.plain) {
+        if (!MB && p.plain) {          // (never with a multi-bit key: capi.cu rejects it)
             __syncthreads();
             if constexpr (Cfg::FFT) br_fft_step<false, Cfg>(s, p.bk, s.rot, tid, p.fft_tab);
             else br2_step<false, Cfg>(s, p.bk, s.rot, tid);
             __syncthreads();
+        } else if constexpr (MB) {
+            // thread t < 2 CT loads bit t & 1 of the group for ciphertext slot t >> 1
+            if (tid < 2 * Cfg::CT) s.rot[(step0 & 1) * 2 * Cfg::CT + tid] = br_rotation<LUT>(p, ct_of(tid >> 1), 2 * step0 + (tid & 1));
+            __syncthreads();
+            for (int i = step0; i < step1; i++) {
+                int next = 0;
+                if (tid < 2 * Cfg::CT && i + 1 < step1) next = br_rotation<LUT>(p, ct_of(tid >> 1), 2 * (i + 1) + (tid & 1));
+                br_fft_step<true, Cfg, true>(s, p.bk + (size_t)i * 3 * BK_FFT_U64, s.rot + (i & 1) * 2 * Cfg::CT, tid, p.fft_tab);
+                if (tid < 2 * Cfg::CT) s.rot[((i + 1) & 1) * 2 * Cfg::CT + tid] = next;
+                __syncthreads();
+            }
         } else {
             if (tid < Cfg::CT) s.rot[(step0 & 1) * Cfg::CT + tid] = br_rotation<LUT>(p, ct_of(tid), step0);
             __syncthreads();
@@ -687,7 +715,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
             }
         }
 
-        if (!p.plain && step1 < p.n) {
+        if (!p.plain && step1 < br_chain_steps<MB>(p)) {
             // park the accumulators and publish the chain's progress
             int4 *dst = reinterpret_cast<int4 *>(p.state + (size_t)chain * ACC_WORDS);
             for (int e = tid; e < ACC_WORDS / 4; e += Cfg::THREADS) __stcg(dst + e, reinterpret_cast<const int4 *>(s.acc)[e]);

@@ -44,8 +44,8 @@ struct PhaseTables {
 // double and rounded once to double, so every component is within 2^-53 (relative) of the exact value -- what the
 // error bound of DESIGN.md section 4 assumes.
 struct FftTables {
-    std::vector<cplx> tab;
-    FftTables() : tab(FFT_TAB_CPLX)
+    std::vector<cplx> tab, roots;
+    FftTables() : tab(FFT_TAB_CPLX), roots(FFT_ROOTS)
     {
         const long double pi = acosl(-1.0L);
         auto e = [&](int num) {                      // e^{2 pi i num / 2048}
@@ -55,6 +55,8 @@ struct FftTables {
         // T[k1][n0] = w^n0 W512^(n0 k1) = e^{2 pi i n0 (1 - 4 k1) / 2048}, w = e^{i pi / 1024}
         for (int k1 = 0; k1 < 8; k1++)
             for (int n0 = 0; n0 < 64; n0++) tab[fft_tab_t1(k1, n0)] = e(n0 * (1 - 4 * k1));
+        // R[e] = e^{2 pi i e / 2048}: the rotations of the multi-bit step (br_phases.cuh: fft_phase_mac_mb)
+        for (int i = 0; i < FFT_ROOTS; i++) roots[i] = e(i);
     }
 };
 

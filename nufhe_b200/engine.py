@@ -131,6 +131,17 @@ class Engine:
         self._call('nb_bk_prepare', _ptr(bk_ref), _ptr(out), rows)
         return out
 
+    def bk_prepare_multibit(self, bk_ref):
+        """A multi-bit bootstrap key (3 reference rows per group of two key bits) as the fused kernels read it: the FP64
+        spectra of every row (nb_bk_prepare_multibit).  The result goes wherever a `bk_prepare` key goes."""
+        bk_ref = self._dense(bk_ref, torch.int64)
+        rows = bk_ref.numel() // (8 * N)
+        if rows % 3:
+            raise ValueError('a multi-bit key has 3 rows per group, got %d rows' % rows)
+        out = self.empty((rows, self.lib.nb_bk_multibit_row_u64()), torch.int64)
+        self._call('nb_bk_prepare_multibit', _ptr(bk_ref), _ptr(out), rows // 3)
+        return out
+
     def external_product(self, accum, bk_int, row):
         """accum (B,2,1024) int32 is updated in place: accum <- bk[row] (x) accum"""
         assert accum.is_contiguous() and accum.dtype == torch.int32

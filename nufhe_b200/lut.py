@@ -98,13 +98,30 @@ def make_test_vector(tables, bits, log2_outputs=0, out='int'):
     return (vals & 0xffffffff).astype(numpy.uint32).view(numpy.int32)
 
 
-def _sigma_estimate(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift):
+# Multi-bit keys (bootstrap.py: MultiBitBootstrapKey) carry three times the blind-rotation variance (DESIGN.md section
+# 14): the (P, L, shift) they allow, which follows from lut_sigma(..., multi_bit=2) (tests check it), and the standard
+# deviations measured by tools/multibit_noise.py with a multi-bit key, keyed as MEASURED_SIGMA, on an H100 80GB HBM3
+# (700 W, 1980 MHz), 65 536 inputs each.  All lie 2 - 3 % below the estimates; lut_sigma takes the larger of the two.
+ALLOWED_MULTI_BIT = {
+    (1, 0, None), (1, 1, None), (1, 2, None), (1, 0, 0), (1, 1, 0), (1, 2, 0),
+    (2, 0, None), (2, 1, None), (2, 0, 0),
+}
+MEASURED_SIGMA_MULTI_BIT = {
+    (0, None): 0.00586, (0, 0): 0.00804, (0, 1): 0.01237,
+    (1, None): 0.00698, (1, 0): 0.00882, (1, 1): 0.01290,
+    (2, None): 0.01035, (2, 0): 0.01167, (2, 1): 0.01505,
+}
+
+
+def _sigma_estimate(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift, multi_bit=1):
     """Analytic standard deviation of the rounded phase of a LUT input that is one LUT output (shift None) or
-    x * 2^shift + y of two: weight * (blind rotation + key switch) + mod-switch rounding."""
+    x * 2^shift + y of two: weight * (blind rotation + key switch) + mod-switch rounding.  A multi-bit key's rotation
+    has n / 2 steps of 3 external products, each times X^k - 1, which doubles its variance: 3 n products' worth."""
     tl = tgsw_params.tlwe_params
     n, N, k = in_out_params.size, tl.polynomial_degree, tl.mask_size
     half_digit = 2**tgsw_params.bs_log2_base / 2
-    blind_rotation = n * (k + 1) * tgsw_params.decomp_length * N * half_digit**2 / 3 * tl.min_noise**2
+    products = 3 * n if multi_bit == 2 else n
+    blind_rotation = products * (k + 1) * tgsw_params.decomp_length * N * half_digit**2 / 3 * tl.min_noise**2
     base = 2**ks_log2_base
     keyswitch = k * N * ks_decomp_length * (base - 1) / base * in_out_params.min_noise**2
     modswitch = (n / 2 + 1) * (2**log2_outputs / (2 * N))**2 / 12
@@ -112,17 +129,25 @@ def _sigma_estimate(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, 
     return (weight * (blind_rotation + keyswitch) + modswitch)**0.5
 
 
-def _sigma(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift):
-    est = _sigma_estimate(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift)
+def _sigma(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift, multi_bit=1):
+    est = _sigma_estimate(in_out_params, tgsw_params, ks_decomp_length, ks_log2_base, log2_outputs, shift, multi_bit)
     if tgsw_params.tlwe_params.mask_size == 1:
-        est = max(est, MEASURED_SIGMA.get((log2_outputs, shift), 0.0))
+        measured = MEASURED_SIGMA_MULTI_BIT if multi_bit == 2 else MEASURED_SIGMA
+        est = max(est, measured.get((log2_outputs, shift), 0.0))
     return est
 
 
-def lut_sigma(params, log2_outputs, shift=None):
-    """The standard deviation `check_noise` uses for a NuFHEParameters set (estimate, or the measured value if larger)."""
+def lut_sigma(params, log2_outputs, shift=None, multi_bit=1):
+    """The standard deviation `check_noise` uses for a NuFHEParameters set (estimate, or the measured value if larger);
+    multi_bit=2 for a multi-bit bootstrap key."""
     return _sigma(params.in_out_params, params.tgsw_params, params.ks_decomp_length, params.ks_log2_base,
-                  log2_outputs, shift)
+                  log2_outputs, shift, multi_bit)
+
+
+def bootstrap_variance(params, multi_bit=1):
+    """Estimated phase variance of a bootstrap output after the key switch: blind rotation + key switch."""
+    return _sigma_estimate(params.in_out_params, params.tgsw_params, params.ks_decomp_length, params.ks_log2_base,
+                           0, None, multi_bit)**2 - (params.in_out_params.size / 2 + 1) / (2 * 1024)**2 / 12
 
 
 def _check_config(bits, log2_outputs, shift):
@@ -141,11 +166,11 @@ def _check_margin(sigma, bits, log2_outputs, shift):
                             margin, MARGIN_SIGMAS))
 
 
-def check_noise(params, bits, log2_outputs, shift=None):
+def check_noise(params, bits, log2_outputs, shift=None, multi_bit=1):
     """Raise ValueError unless inputs that are LUT outputs (one, or x * 2^shift + y of two) stay 7 sigma inside their
-    boxes of half-width 2^-(bits + 2)."""
+    boxes of half-width 2^-(bits + 2); multi_bit=2 for a multi-bit bootstrap key."""
     _check_config(bits, log2_outputs, shift)
-    _check_margin(lut_sigma(params, log2_outputs, shift), bits, log2_outputs, shift)
+    _check_margin(lut_sigma(params, log2_outputs, shift, multi_bit), bits, log2_outputs, shift)
 
 
 class LookupTable:
@@ -241,7 +266,8 @@ def bootstrap_lut(thr, results, bk, ks, table: LookupTable, x: LweSampleArray, y
         raise ValueError("per-ciphertext tables of shape %s do not match results of shape %s" % (table.batch_shape, shape))
     _check_config(table.bits, L, None if y is None else shift)
     _check_margin(_sigma(bk.in_out_params, bk.bk_params, ks.decomp_length, ks.log2_base, L,
-                         None if y is None else shift), table.bits, L, None if y is None else shift)
+                         None if y is None else shift, getattr(bk, 'multi_bit', 1)), table.bits, L,
+                  None if y is None else shift)
     B = int(numpy.prod(shape, dtype=numpy.int64))
     p1 = _expand(x, shape)
     p2 = _expand(y, shape) if y is not None else None

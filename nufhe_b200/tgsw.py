@@ -161,13 +161,17 @@ def tgsw_transformed_external_mul(thr, result: TLweSampleArray, bootstrap_key, b
 
 
 def engine_format(thr, tgsw: TransformedTGswSampleArray):
-    """The bootstrap key re-laid for the MAC stage of the fused kernel (nb_bk_prepare), cached."""
+    """The bootstrap key re-laid for the MAC stage of the fused kernel (nb_bk_prepare, or nb_bk_prepare_multibit for
+    the rows of a multi-bit key), cached."""
     if not fused_kernel_supported(tgsw.params):
         raise ValueError("The fused bootstrap kernel supports mask_size=1, decomp_length=2, bs_log2_base=10, "
                          "polynomial_degree=1024 only; other parameters run on the multi-kernel path "
                          "(single_kernel_bootstrap=False)")
     cached = getattr(tgsw, '_engine_format', None)
     if cached is None or cached.device != tgsw.samples.a.coeffs.device:
-        cached = thr.bk_prepare(tgsw.samples.a.coeffs)
+        if getattr(tgsw, 'multi_bit', 1) == 2:
+            cached = thr.bk_prepare_multibit(tgsw.samples.a.coeffs)     # bootstrap.py: MultiBitBootstrapKey
+        else:
+            cached = thr.bk_prepare(tgsw.samples.a.coeffs)
         tgsw._engine_format = cached
     return cached

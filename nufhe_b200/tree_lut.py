@@ -33,6 +33,12 @@ MEASURED_SIGMA = {
     (2, 2): 0.00619, (2, 3): 0.00743, (2, 4): 0.00846,
     (1, 2): 0.00622, (1, 3): 0.00742, (1, 4): 0.00849,
 }
+# The same with a multi-bit bootstrap key (tools/multibit_noise.py, same card and count; DESIGN.md section 14), up to
+# one level past what the rule allows.  All lie 2 - 3 % below the estimates.
+MEASURED_SIGMA_MULTI_BIT = {
+    (2, 2): 0.00804, (2, 3): 0.00971,
+    (1, 2): 0.00803, (1, 3): 0.00974, (1, 4): 0.01116,
+}
 
 
 class NuFHETreeKey(_GadgetKey):
@@ -66,13 +72,14 @@ def _modswitch_variance(params, log2_outputs=0):
     return (n / 2 + 1) * (2**log2_outputs / (2 * N))**2 / 12
 
 
-def level_variance(params):
+def level_variance(params, multi_bit=1):
     """Blind rotation + key switch of one level: the estimate of lut._sigma_estimate, or for k = 1 the measured
-    one-output LUT variance less its mod-switch term when that is larger."""
+    one-output LUT variance less its mod-switch term when that is larger (multi_bit=2: a multi-bit bootstrap key)."""
     est = lut._sigma_estimate(params.in_out_params, params.tgsw_params, params.ks_decomp_length, params.ks_log2_base,
-                              0, None)**2 - _modswitch_variance(params)
-    if params.tgsw_params.tlwe_params.mask_size == 1:
-        est = max(est, lut.MEASURED_SIGMA[(0, None)]**2 - _modswitch_variance(params))
+                              0, None, multi_bit)**2 - _modswitch_variance(params)
+    measured = (lut.MEASURED_SIGMA_MULTI_BIT if multi_bit == 2 else lut.MEASURED_SIGMA).get((0, None))
+    if params.tgsw_params.tlwe_params.mask_size == 1 and measured:
+        est = max(est, measured**2 - _modswitch_variance(params))
     return est
 
 
@@ -88,44 +95,46 @@ def test_vector_variance(params, bits):
     return key + rounding
 
 
-def output_variance(params, bits, digits):
+def output_variance(params, bits, digits, multi_bit=1):
     """Phase variance of a level-`digits` output: D levels of blind rotation and key switch, D - 1 encrypted test
     vectors."""
-    return digits * level_variance(params) + (digits - 1) * test_vector_variance(params, bits)
+    return digits * level_variance(params, multi_bit) + (digits - 1) * test_vector_variance(params, bits)
 
 
-def tree_sigma(params, bits, digits):
+def tree_sigma(params, bits, digits, multi_bit=1):
     """Standard deviation of the rounded phase of a level-`digits` tree output used as a one-input LUT input: the
     output variance plus the mod-switch; the measured value if larger."""
-    sigma = (output_variance(params, bits, digits) + _modswitch_variance(params))**0.5
+    sigma = (output_variance(params, bits, digits, multi_bit) + _modswitch_variance(params))**0.5
     if params.tgsw_params.tlwe_params.mask_size == 1:
-        sigma = max(sigma, MEASURED_SIGMA.get((bits, digits), 0.0))
+        measured = MEASURED_SIGMA_MULTI_BIT if multi_bit == 2 else MEASURED_SIGMA
+        sigma = max(sigma, measured.get((bits, digits), 0.0))
     return sigma
 
 
-def max_digits(params, bits):
-    """The largest D whose outputs stay lut.MARGIN_SIGMAS standard deviations inside their boxes (4 for P = 2)."""
+def max_digits(params, bits, multi_bit=1):
+    """The largest D whose outputs stay lut.MARGIN_SIGMAS standard deviations inside their boxes (4 for P = 2; 2 with
+    a multi-bit bootstrap key)."""
     best = 0
     for d in range(1, MAX_DIGITS + 1):
-        if 2.0**-(bits + 2) / tree_sigma(params, bits, d) >= lut.MARGIN_SIGMAS:
+        if 2.0**-(bits + 2) / tree_sigma(params, bits, d, multi_bit) >= lut.MARGIN_SIGMAS:
             best = d
     return best
 
 
-def _check_config(params, bits, digits):
+def _check_config(params, bits, digits, multi_bit=1):
     if bits not in (1, 2):
         raise ValueError('tree LUTs take digits of 1 or 2 bits, got %r' % (bits,))
-    top = max_digits(params, bits)
+    top = max_digits(params, bits, multi_bit)
     if int(digits) != digits or not 2 <= digits <= top:
         raise ValueError('a tree LUT on %d-bit digits takes 2 to %d digits with these parameters, got %r'
                          % (bits, top, digits))
 
 
-def _level1_log2_outputs(params, bits, columns):
+def _level1_log2_outputs(params, bits, columns, multi_bit=1):
     """Columns per level-1 bootstrap: the largest 2^L (L <= 2, 2^L <= columns) that the LUT noise rule allows."""
     best = 0
     for L in range(lut.MAX_LOG2_OUTPUTS + 1):
-        if (1 << L) <= columns and 2.0**-(bits + 2) / lut.lut_sigma(params, L) >= lut.MARGIN_SIGMAS:
+        if (1 << L) <= columns and 2.0**-(bits + 2) / lut.lut_sigma(params, L, None, multi_bit) >= lut.MARGIN_SIGMAS:
             best = L
     return best
 
@@ -137,8 +146,10 @@ class TreeLookupTable:
     [f, d_{D-1}, ..., d_0].  Holds the device-resident level-1 test vectors: the F 2^(bits (D-1)) columns f(v, .) in
     groups of 2^L (zero columns pad the last group), `tv` (Q, N) for Q = ceil(columns / 2^L)."""
 
-    def __init__(self, thr, params, tables, bits, digits, out='int'):
-        _check_config(params, bits, digits)
+    def __init__(self, thr, params, tables, bits, digits, out='int', multi_bit=1):
+        """multi_bit=2: a table for a VM whose cloud key has a multi-bit bootstrap key (its noise rules)."""
+        _check_config(params, bits, digits, multi_bit)
+        self.multi_bit = multi_bit
         if out not in ('int', 'bool'):
             raise ValueError("out must be 'int' or 'bool'")
         M = 1 << bits
@@ -153,7 +164,7 @@ class TreeLookupTable:
         self.bits, self.digits, self.out = int(bits), int(digits), out
         self.functions = tables.shape[0]
         self.columns = self.functions * M**(digits - 1)
-        self.log2_outputs = _level1_log2_outputs(params, bits, self.columns)
+        self.log2_outputs = _level1_log2_outputs(params, bits, self.columns, multi_bit)
         K = 1 << self.log2_outputs
         self.groups = -(-self.columns // K)
         cols = numpy.zeros((self.groups * K, M), numpy.int64)
@@ -236,6 +247,9 @@ def lut_tree(thr, results, bk, ks, tree_key, table: TreeLookupTable, digits, per
         raise TypeError('lut_tree needs a TreeLookupTable (vm.make_tree_lut), got %s' % type(table).__name__)
     if tree_key.params != table.params:
         raise ValueError('the tree key was made for other parameters than this table')
+    if getattr(bk, 'multi_bit', 1) != table.multi_bit:
+        raise ValueError('the table was made for another kind of bootstrap key (multi_bit=%d, the key has %d): make it '
+                         'with this VM' % (table.multi_bit, getattr(bk, 'multi_bit', 1)))
     digits = list(digits)
     if len(digits) != table.digits:
         raise ValueError('the table takes %d digits, got %d' % (table.digits, len(digits)))
