@@ -1513,9 +1513,26 @@ NB_HD void fft_phase_inv2(int tid, cplx *spec_all)
 // pass 3, fused: group fft_pass3_group(tid / 2) of ciphertext tid & 1 (fft_pass3_pos): the forward DFT4 of the 4 digit spectra, then for each output
 // spectrum s = mo * 2 + h the MAC out = sum_d D_d K[d][mo][h] at the 4 points and the inverse DFT4; the outputs
 // overwrite the digit spectra at the same positions (the thread holds all of them).
+// The key values of two outputs k3 are in flight at any time, one loop iteration ahead of their use: those of outputs
+// 0 and 1 of spectrum s are loaded while outputs 2 and 3 of spectrum s - 1 are computed, transformed and stored (the
+// first ones before the digit spectra are read), so the L2 latency of the key stream overlaps work instead of
+// stalling every output spectrum.  The arithmetic is the same in the same order.
 NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
 {
-    const int j = tid >> 1;
+#ifdef NB_FFT_KEY_L1_BOUND
+    // TIMING EXPERIMENT ONLY (wrong results): every key load hits the same 2 KB of the row -- what the step would take
+    // if the key stream cost nothing (DESIGN.md section 4, FP64 step breakdown)
+    const int kj = (tid >> 1) & 15;
+#else
+    const int kj = tid >> 1;
+#endif
+    // the 4 key values (digits d) of output k3 of spectrum s
+    auto load_key = [&](cplx *k, int s, int k3) {
+        static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(key + fft_key_pos(4 * decltype(D)::value + s, kj, k3)); });
+    };
+    cplx ka[4], kb[4];          // even / odd outputs k3
+    load_key(ka, 0, 0);
+    load_key(kb, 0, 1);
     cplx dg[4][4];
     static_for<0, 4>([&](auto D) {
         static_for<0, 4>([&](auto I) { dg[decltype(D)::value][decltype(I)::value] = ld_cplx(spec_all + fft_pass3_pos(tid, decltype(D)::value, decltype(I)::value)); });
@@ -1528,19 +1545,14 @@ NB_HD void fft_phase_mac(int tid, cplx *spec_all, const cplx *key)
         cplx o[4];
         static_for<0, 4>([&](auto K3) {
             constexpr int k3 = decltype(K3)::value;
-#ifdef NB_FFT_KEY_L1_BOUND
-            // TIMING EXPERIMENT ONLY (wrong results): every key load hits the same 2 KB of the row -- what the step
-            // would take if the key stream cost nothing (DESIGN.md section 4, FP64 step breakdown)
-            const int kj = j & 15;
-#else
-            const int kj = j;
-#endif
-            cplx k[4];
-            static_for<0, 4>([&](auto D) { k[decltype(D)::value] = ld_cplx_stream(key + fft_key_pos(4 * decltype(D)::value + s, kj, k3)); });
+            cplx *k = (k3 & 1) ? kb : ka;
             cplx v = {d_mul(dg[0][k3].re, k[0].re), d_mul(dg[0][k3].re, k[0].im)};
             v = {d_fma(-dg[0][k3].im, k[0].im, v.re), d_fma(dg[0][k3].im, k[0].re, v.im)};
             static_for<1, 4>([&](auto D) { v = c_mac(v, dg[decltype(D)::value][k3], k[decltype(D)::value]); });
             o[k3] = v;
+            // refill: outputs 2, 3 of this spectrum, then outputs 0, 1 of the next one
+            if constexpr (k3 < 2) load_key(k, s, k3 + 2);
+            else if (s < 3) load_key(k, s + 1, k3 - 2);
         });
         dft4<true>(o);
         static_for<0, 4>([&](auto I) { st_cplx(spec_all + fft_pass3_pos(tid, s, decltype(I)::value), o[decltype(I)::value]); });

@@ -112,9 +112,10 @@ def step_loop(kernel_ins, loop_addrs, labels):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--lib', default=os.path.join(ROOT, 'nufhe_b200', 'csrc', 'libnufhe_b200.so'))
-    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb1ELb1EEELb0E',
+    ap.add_argument('--kernel', default='blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb1ELb1EEELb0ELb0E',
                     help='substring of the mangled kernel name (default: the gate kernel of the 2-ciphertext shape with '
-                         'the FP64 step; the NTT one is blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0EEELb0E, the '
+                         'the FP64 step and a standard key -- its multi-bit instantiation ends in Lb0ELb1E, and a '
+                         'shorter default would count both; the NTT one is blind_rotate_kernelINS_5BrCfgILi2ELi256ELi2ELb0ELb0EEELb0E, the '
                          'wide shape blind_rotate_kernelINS_5BrCfgILi1ELi256ELi2ELb0ELb0EEELb0E, the pair shape '
                          'blind_rotate_pair_kernelILb1ELb0E)')
     ap.add_argument('--by-func', action='store_true', help='also split each phase by innermost ff.cuh / br_phases function')
