@@ -258,6 +258,28 @@ int nb_tree_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, 
 int nb_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
                                   const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch);
 
+/* ---- encrypted-index table lookups (DESIGN.md section 15; no reference counterpart).  A query holds m TGSW selectors
+ * (the client-encrypted bits of an index, N = 1024, k = 1, l = 2, Bg = 2^10), each (2, 2, 2, N) int32 in the layout of
+ * a bootstrap-key row.  All three run the FP64 CMux step; GLWE samples are (2, N) int32.
+ * nb_index_prepare: `rows` selector rows -> spectra (rows, BK_FFT_U64) uint64 (nb_bk_multibit_row_u64() words per row,
+ *     the layout nb_bk_prepare_multibit stores).
+ * nb_index_cmux_level: out[q][i] = in[q][2i] + sel[q] (x) (in[q][2i+1] - in[q][2i]) for i < nodes, q < queries; in[q]
+ *     starts in_query_stride int32 words after in[q-1] (0: one plaintext level shared by every query), sel[q]
+ *     sel_query_stride uint64 words after sel[q-1]; out (queries, nodes, 2, N).
+ * nb_index_rotate_extract: for j < min(bits, 10), ACC <- ACC + sel_j[q] (x) ((X^(-2^j) - 1) ACC), sel_j[q] = sel +
+ *     q sel_query_stride + j BK_FFT_U64, then sample extraction.  bits >= 10: `columns` accumulators per query
+ *     (consecutive, acc_query_stride words between queries), each extracted at coefficient 0.  bits < 10: one
+ *     accumulator per query, extracted at coefficients w 2^bits, w < columns.  Column w of query q goes to row
+ *     w * queries + q of out_a (columns * queries, N) and out_b (columns * queries).
+ * NB_EINVAL for a NULL pointer, bits outside 1..20, columns = 0, columns 2^bits > N for bits < 10, or a batch beyond
+ * the grid; rows / nodes / queries = 0 is a no-op. */
+int nb_index_prepare(nb_ctx *ctx, const int32_t *ggsw, size_t rows, uint64_t *spectra);
+int nb_index_cmux_level(nb_ctx *ctx, const int32_t *in, size_t in_query_stride, const uint64_t *sel,
+                        size_t sel_query_stride, int32_t *out, size_t nodes, size_t queries);
+int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_stride, const uint64_t *sel,
+                            size_t sel_query_stride, int bits, size_t columns, int32_t *out_a, int32_t *out_b,
+                            size_t queries);
+
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,14 @@ from .tree_lut import (
     TreeLookupTable,
     lut_tree,
     )
+from .index_lookup import (
+    NuFHEIndexSecretKey,
+    EncryptedIndexArray,
+    CompressedEncryptedIndexArray,
+    IndexTable,
+    encrypt_index,
+    lookup,
+    )
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

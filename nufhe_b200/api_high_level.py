@@ -1,4 +1,6 @@
 """High-level API (reference: nufhe/api_high_level.py): find_devices, DeviceID, Context, VirtualMachine."""
+import io
+
 import torch
 
 from .api_low_level import (
@@ -9,6 +11,8 @@ from .public_key import NuFHEPublicKey
 from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
                       decrypt_packed, decrypt_packed_int)
 from .tree_lut import NuFHETreeKey, TreeLookupTable, lut_tree
+from .index_lookup import (NuFHEIndexSecretKey, IndexTable, encrypt_index, load_encrypted_index, lookup,
+                           _check_params as check_index_params)
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -101,19 +105,33 @@ class Context:
     def make_secret_key(self, **params):
         return NuFHESecretKey.from_rng(self.thread, NuFHEParameters(**params), self.rng)
 
-    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False, multi_bit=1):
+    def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False, multi_bit=1,
+                       index_key=False):
         """compressed=True returns a CompressedCloudKey (about 12 times smaller to store or send); its `decompress()`
         gives the NuFHECloudKey that make_virtual_machine takes.  tree_key=True returns (cloud key, NuFHETreeKey), the
         key of VirtualMachine.lut_tree; its draws follow all of the cloud key's, so the cloud key is the same either
         way.  multi_bit=2 gives the cloud key a MultiBitBootstrapKey (key bits two at a time: half the CMux steps per
         bootstrap, about 3x the key rows and more noise; DESIGN.md section 14); ValueError for parameters it cannot
-        take (tlwe_mask_size = 2, an odd LWE dimension) and for multi_bit outside {1, 2}."""
+        take (tlwe_mask_size = 2, an odd LWE dimension) and for multi_bit outside {1, 2}.
+        index_key=True also returns the NuFHEIndexSecretKey that encrypts indices for VirtualMachine.lookup; it draws
+        nothing.  With several extras the order is (cloud key, tree key, index key).  ValueError for tlwe_mask_size != 1."""
+        if index_key:
+            check_index_params(secret_key.params)
         cls = CompressedCloudKey if compressed else NuFHECloudKey
         cloud_key, tgsw_key = cls.from_rng_with_tgsw_key(self.thread, secret_key.params, self.rng, secret_key,
                                                          multi_bit=multi_bit)
-        if not tree_key:
-            return cloud_key
-        return cloud_key, NuFHETreeKey.from_secret_key(self.thread, self.rng, secret_key, tgsw_key)
+        out = [cloud_key]
+        if tree_key:
+            out.append(NuFHETreeKey.from_secret_key(self.thread, self.rng, secret_key, tgsw_key))
+        if index_key:
+            out.append(NuFHEIndexSecretKey.from_tgsw_key(secret_key.params, tgsw_key))
+        return out[0] if len(out) == 1 else tuple(out)
+
+    def encrypt_index(self, index_key: NuFHEIndexSecretKey, values, bits, compressed=False):
+        """Encrypted indices 0 <= v < 2^bits (bits = 1..20) for VirtualMachine.lookup: one TGSW selector per bit,
+        32 KB per bit (an EncryptedIndexArray), or 16 KB per bit with compressed=True (a CompressedEncryptedIndexArray,
+        `decompress()` to compute).  ValueError for bits or values out of range."""
+        return encrypt_index(self.thread, self.rng, index_key, values, bits, compressed=compressed)
 
     def make_public_key(self, secret_key: NuFHESecretKey):
         """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
@@ -193,6 +211,17 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return NuFHETreeKey.loads(file_or_bytestring, self.thread)
         return NuFHETreeKey.load(file_or_bytestring, self.thread)
+
+    def load_index_secret_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHEIndexSecretKey.loads(file_or_bytestring, self.thread)
+        return NuFHEIndexSecretKey.load(file_or_bytestring, self.thread)
+
+    def load_encrypted_index(self, file_or_bytestring):
+        """An EncryptedIndexArray or CompressedEncryptedIndexArray, whichever was saved."""
+        if isinstance(file_or_bytestring, bytes):
+            file_or_bytestring = io.BytesIO(file_or_bytestring)
+        return load_encrypted_index(file_or_bytestring, self.thread)
 
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
@@ -284,6 +313,19 @@ class VirtualMachine:
         lut_tree(self.thread, dest, self.cloud_key.bootstrap_key, self.cloud_key.keyswitch_key, tree_key, table,
                  digits, perf_params=self.perf_params)
         return dest[0] if table.single else dest
+
+    def make_index_table(self, table, out='int', bits=None):
+        """A table for encrypted-index lookups (nufhe_b200/index_lookup.py: IndexTable): shape (2^m,) or (W, 2^m),
+        1 <= m <= 20, W <= 2^(10 - m) below m = 10.  out='int' encodes entries as `bits`-bit integers (for vm.lut and
+        decrypt_int), out='bool' as gate bits."""
+        return IndexTable(self.thread, self.params, table, out=out, bits=bits)
+
+    def lookup(self, index, table, dest=None):
+        """table[idx] for every index of the EncryptedIndexArray `index`: one ciphertext array of the index's shape, or a
+        list of W for a table of W columns.  CMux gates only, no bootstrap (DESIGN.md section 15).  TypeError for
+        anything but an EncryptedIndexArray (decompress a compressed one first), ValueError for other parameters or a
+        bit count other than the table's."""
+        return lookup(self.thread, self.cloud_key.keyswitch_key, index, table, dest=dest)
 
     def int_add(self, x, y, dest=None):
         """x + y of two integer ciphertexts without a bootstrap (the caller keeps the sum below 2^bits)."""

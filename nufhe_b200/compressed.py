@@ -7,6 +7,9 @@ the engine regenerates the masks from it with ChaCha20 (Engine.seeded_uniform, n
     ciphertext array     its own, per encryption    0       shape + (n,)
     bootstrap key        the cloud key's seed       1       (n, k+1, l, k, N): the TLWE masks, polys [..., :k, :]
     key-switch key       the cloud key's seed       2       (in, t, base-1, n_out); rows h = 0 stay zero
+    packing key          its own                    4       (n, t, k, N)
+    tree key             its own                    5       (n, t, k, N)
+    encrypted index      its own, per encryption    6       (rows, k+1, l, k, N), rows = shape x bits (index_lookup.py)
 
 Seeds are drawn from the context RNG as `rng.uniform_torus32((8,))`.  `decompress()` gives the ordinary objects
 (LweSampleArray, NuFHECloudKey) that the rest of the library takes.

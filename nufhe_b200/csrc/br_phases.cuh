@@ -1472,7 +1472,12 @@ NB_HD void fft_inv1(int n0, const cplx *sp, const cplx *tab, double *x)
 // ---- the FP64 step of a CTA of 2 ciphertexts on 256 threads: spectra fft_spec(ct, s), s = mi * 2 + j before the MAC
 // and s = mo * 2 + h after it.
 // fwd1: task (pm = ct * 2 + mi, n0): the rotated coefficients serve both digit polynomials (as phase_fwd1_both_digits)
-template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, cplx *spec_all, const cplx *tab, const int *rot_a)
+// ROUND: added to every coefficient before the digits are cut.  0 (the bootstrap, as nufhe's decomposition): the
+// digits truncate, Dec(x) g = x - (x mod 2^12).  DIGIT_ROUND (index_lookup.cuh): they round to the nearest multiple of
+// 2^12, so the approximation error is centred instead of averaging -2^11.
+constexpr u32 DIGIT_ROUND = 1u << 11;      // half the precision 2^(32 - l log2 Bg) of the decomposition
+template <bool ROTATE, u32 ROUND = 0>
+NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, cplx *spec_all, const cplx *tab, const int *rot_a)
 {
     const int n0 = task & 63, pm = task >> 6;
     const i32 *acc = acc_all + pm * NTT_N;
@@ -1484,7 +1489,7 @@ template <bool ROTATE> NB_HD void fft_phase_fwd1(int task, const i32 *acc_all, c
         constexpr int j1 = decltype(J)::value;
         const int idx = 64 * j1 + n0;
         const i32 c = ROTATE ? rotate_minus_one(acc, idx, ar, flip) : acc[idx];
-        t[j1] = (u32)c + (0x80000000u + (1u << 21));
+        t[j1] = (u32)c + (0x80000000u + (1u << 21) + ROUND);
     });
     cplx t1[8];
     fft_load_t1(n0, tab, t1);

@@ -7,6 +7,7 @@
 #include <nvtx3/nvToolsExt.h>
 #include "../../include/nufhe_b200.h"
 #include "kernels.cuh"
+#include "index_lookup.cuh"
 #include "tables.h"
 
 using namespace nb;
@@ -35,6 +36,8 @@ struct nb_ctx {
     int32_t *d_state;                    // parked accumulators of time-sliced launches
     size_t state_words;
     float *d_cv_blocks;                  // block sums of the key-switch variances (split launches)
+    u64 *d_index_tmp;                    // nb_index_prepare: field elements of one chunk of selector rows
+    size_t index_tmp_words;
     size_t cv_words;
     int force_chunks;                    // developer knob: chunk count of every multi-wave launch (0 = automatic)
     int stagger_cycles;                  // start-up offset of the second CTA per SM in single-wave launches
@@ -119,6 +122,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     ctx->d_fft_tab = nullptr;
     ctx->d_sched = nullptr; ctx->d_state = nullptr; ctx->sched_words = ctx->state_words = 0;
     ctx->d_cv_blocks = nullptr; ctx->cv_words = 0;
+    ctx->d_index_tmp = nullptr; ctx->index_tmp_words = 0;
     *out = ctx;   // returned even on failure so that nb_last_error() can be read; caller destroys it
     NB_ON_DEVICE(ctx);
     cudaDeviceProp prop;
@@ -170,6 +174,9 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check_resident<BrWide2>(ctx));
     NB_TRY(check_resident<BrFft>(ctx));
     NB_TRY((check_resident<BrFft, true>(ctx)));
+    for (auto kernel : {index_lookup_kernel<false>, index_lookup_kernel<true>})
+        NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<BrFft>()),
+                     "cudaFuncSetAttribute(index_lookup)"));
     {   // batches that fit one wave of wide CTAs (one ciphertext on 256 threads) take the low-latency shape
         const char *e = getenv("NUFHE_B200_WIDE_MAX");
         // up to one wave the wide shape has the shortest step; between one and ~1.7 waves it still wins, time-sliced
@@ -227,6 +234,7 @@ void nb_ctx_destroy(nb_ctx *ctx)
     if (ctx->d_sched) cudaFree(ctx->d_sched);
     if (ctx->d_state) cudaFree(ctx->d_state);
     if (ctx->d_cv_blocks) cudaFree(ctx->d_cv_blocks);
+    if (ctx->d_index_tmp) cudaFree(ctx->d_index_tmp);
     delete ctx;
 }
 
@@ -1000,6 +1008,79 @@ int nb_tree_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, 
     NvtxRange nvtx_range("nufhe_b200:tree_assemble");
     tree_assemble_kernel<<<(unsigned)ctas, TREE_ASM_THREADS, 0, ctx->stream>>>(v, b, bits, (u32)mask_size, tv);
     return launch_check(ctx, "tree_assemble_kernel");
+}
+
+// ---- encrypted-index lookups (index_lookup.cuh) ----
+
+int nb_index_prepare(nb_ctx *ctx, const int32_t *ggsw, size_t rows, uint64_t *spectra)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!ggsw || !spectra) return fail(ctx, NB_EINVAL, "nb_index_prepare: null argument");
+    if (rows == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:index_prepare");
+    // field elements of CHUNK rows at a time (64 KB per row) in a scratch buffer the context keeps, so that a call
+    // allocates (and synchronises the device) only the first time, then bk_spectra_kernel's split and transforms
+    constexpr size_t CHUNK = 1024;
+    const size_t chunk = rows < CHUNK ? rows : CHUNK, cap = (size_t)ctx->sm_count * 16;
+    NB_TRY(reserve_words(ctx, (void **)&ctx->d_index_tmp, &ctx->index_tmp_words, chunk * 8 * NTT_N + 1, sizeof(u64)));
+    u64 *tmp = ctx->d_index_tmp;
+    // bk_spectra_kernel's integrality flag: int32 coefficients never set it, so it is neither initialised nor read
+    int *d_flag = (int *)(tmp + chunk * 8 * NTT_N);
+    for (size_t r0 = 0; r0 < rows; r0 += chunk) {
+        const size_t n = (rows - r0 < chunk ? rows - r0 : chunk), words = n * 8 * NTT_N, blocks = (words + 255) / 256;
+        index_i32_to_field_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(ggsw + r0 * 8 * NTT_N, tmp, words);
+        bk_spectra_kernel<<<(unsigned)(n * 8), 64, 0, ctx->stream>>>(tmp, (u64 *)spectra + r0 * BK_FFT_U64, ctx->d_fft_tab,
+                                                                      d_flag, BK_FFT_U64, 0);
+        NB_TRY(launch_check(ctx, "index_prepare"));
+    }
+    return NB_OK;
+}
+
+static int index_launch(nb_ctx *ctx, IndexArgs &p, bool rotate, const char *what)
+{
+    p.items = p.queries * p.nodes;
+    const size_t ctas = (p.items + BrFft::CT - 1) / BrFft::CT;
+    if (p.nodes > ((size_t)1 << 40) / p.queries || ctas > 0x7fffffffu)
+        return fail(ctx, NB_EINVAL, std::string(what) + ": too many items");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range(rotate ? "nufhe_b200:index_rotate_extract" : "nufhe_b200:index_cmux_level");
+    p.fft_tab = ctx->d_fft_tab;
+    if (rotate) index_lookup_kernel<true><<<(unsigned)ctas, BrFft::THREADS, br_smem_bytes<BrFft>(), ctx->stream>>>(p);
+    else index_lookup_kernel<false><<<(unsigned)ctas, BrFft::THREADS, br_smem_bytes<BrFft>(), ctx->stream>>>(p);
+    return launch_check(ctx, what);
+}
+
+int nb_index_cmux_level(nb_ctx *ctx, const int32_t *in, size_t in_query_stride, const uint64_t *sel,
+                        size_t sel_query_stride, int32_t *out, size_t nodes, size_t queries)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!in || !sel || !out) return fail(ctx, NB_EINVAL, "nb_index_cmux_level: null argument");
+    if (nodes == 0 || queries == 0) return NB_OK;
+    IndexArgs p{};
+    p.in = in; p.in_stride = in_query_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out = out; p.nodes = nodes; p.queries = queries;
+    return index_launch(ctx, p, false, "nb_index_cmux_level");
+}
+
+int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_stride, const uint64_t *sel,
+                            size_t sel_query_stride, int bits, size_t columns, int32_t *out_a, int32_t *out_b,
+                            size_t queries)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!acc || !sel || !out_a || !out_b) return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: null argument");
+    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: bits must be 1 to 20");
+    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
+        return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: columns * 2^bits must be at most N below 10 bits");
+    if (queries == 0) return NB_OK;
+    IndexArgs p{};
+    p.in = acc; p.in_stride = acc_query_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out_a = out_a; p.out_b = out_b; p.queries = queries;
+    p.nodes = bits >= 10 ? columns : 1;
+    p.samples = bits >= 10 ? 1 : (int)columns;
+    p.steps = bits < 10 ? bits : 10;
+    p.log2_stride = bits;
+    return index_launch(ctx, p, true, "nb_index_rotate_extract");
 }
 
 }  // extern "C"

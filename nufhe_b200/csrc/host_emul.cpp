@@ -315,6 +315,36 @@ int emul_fft_step(i32 *acc_io, const u64 *bk_ref_row, const int *rot, int nct)
     return 0;
 }
 
+// The FP64 step of the encrypted-index kernels (index_lookup.cuh: index_fft_step) on 2 ciphertext slots, each with its
+// own key row: bk_ref_rows (2, 8, 1024) u64 in the reference's form, slot c reads row c.  rot != NULL: the CMux step
+// ACC += row [x] ((X^rot[c] - 1) ACC); else the plain product ACC = row [x] ACC, both with the rounded decomposition of
+// the index kernels (DIGIT_ROUND).  acc_io (2, 2, 1024) is updated.
+// Returns -1 for a row without integral coefficients.
+int emul_fft_step_slots(i32 *acc_io, const u64 *bk_ref_rows, const int *rot)
+{
+    static FftTables F;
+    using Cfg = BrFft;
+    std::vector<cplx> key[2];
+    for (int c = 0; c < 2; c++)
+        if (fft_key_row(bk_ref_rows + (size_t)c * 8 * NTT_N, key[c])) return -1;
+    std::vector<cplx> w(Cfg::POLYS * FFT_SPEC_CPLX, cplx{1e300, -1e300});
+    int rots[2] = {0, 0};
+    if (rot) for (int c = 0; c < 2; c++) rots[c] = rot[c];
+    const cplx *tab = F.tab.data();
+    constexpr int TH = Cfg::THREADS;
+    for (int tid = 0; tid < TH; tid++) {
+        if (rot) fft_phase_fwd1<true, DIGIT_ROUND>(tid, acc_io, w.data(), tab, rots);
+        else fft_phase_fwd1<false, DIGIT_ROUND>(tid, acc_io, w.data(), tab, rots);
+    }
+    for (int tid = 0; tid < TH; tid++) fft_phase_fwd2(tid, w.data());
+    for (int tid = 0; tid < TH; tid++) fft_phase_mac(tid, w.data(), key[tid & 1].data());     // the slot's own row
+    for (int tid = 0; tid < TH; tid++) fft_phase_inv2(tid, w.data());
+    for (int tid = 0; tid < TH; tid++) {
+        if (rot) fft_phase_inv1<true>(tid, acc_io, w.data(), tab); else fft_phase_inv1<false>(tid, acc_io, w.data(), tab);
+    }
+    return 0;
+}
+
 // One group of the multi-bit step (br_fft_step<true, BrFft, true>) for nct <= 2 ciphertexts, phase by phase: the 3
 // reference rows of the group (bk_ref_rows, each 8 x 1024 u64) and rot[c * 2 + b] = abar_{2g + b} of ciphertext c;
 // acc_io (nct, 2, 1024) is updated.  Returns -1 for a key without integral coefficients.

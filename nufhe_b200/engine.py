@@ -456,6 +456,61 @@ class Engine:
                    _ptr(out_b), B)
         return out_a, out_b
 
+    # --- encrypted-index lookups (nufhe_b200/index_lookup.py) -----------------------------------
+    def index_prepare(self, ggsw):
+        """Selector rows (..., 2, 2, 2, N) int32 -> their FP64 spectra (rows, nb_bk_multibit_row_u64()) (nb_index_prepare)."""
+        ggsw = self._dense(ggsw, torch.int32)
+        rows = ggsw.numel() // (8 * N)
+        out = self.empty((rows, self.lib.nb_bk_multibit_row_u64()), torch.int64)
+        if rows:
+            self._call('nb_index_prepare', _ptr(ggsw), rows, _ptr(out))
+        return out
+
+    @staticmethod
+    def _index_nodes(x, queries, what):
+        """(nodes, stride): x (queries, nodes, 2, N) per query, or (nodes, 2, N) shared by all queries (stride 0)."""
+        if x.shape[-2:] != (2, N) or x.dim() not in (3, 4) or (x.dim() == 4 and x.shape[0] != queries):
+            raise ValueError('%s: %s GLWE samples for %d queries' % (what, tuple(x.shape), queries))
+        return x.shape[-3], (0 if x.dim() == 3 else x.shape[1] * 2 * N)
+
+    @staticmethod
+    def _index_sel(sel, bit, queries, what):
+        if sel.dim() != 3 or sel.shape[0] != queries or not 0 <= bit < sel.shape[1]:
+            raise ValueError('%s: selector spectra %s for %d queries, bit %d' % (what, tuple(sel.shape), queries, bit))
+        return ctypes.c_void_p(sel.data_ptr() + bit * sel.shape[2] * sel.element_size()), sel.shape[1] * sel.shape[2]
+
+    def index_cmux_level(self, x, sel, bit, queries):
+        """One CMux-tree level (nb_index_cmux_level): out[q][i] = x[q][2i] + C [x] (x[q][2i+1] - x[q][2i]) with C the
+        selector `bit` of query q in sel (queries, m, R) (index_prepare); x (queries, 2 nodes, 2, N) or (2 nodes, 2, N)
+        shared by every query.  Returns (queries, nodes, 2, N)."""
+        x = self._dense(x, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        pairs, stride = self._index_nodes(x, queries, 'index_cmux_level')
+        if pairs % 2:
+            raise ValueError('index_cmux_level: an odd node count %d' % pairs)
+        sp, sstride = self._index_sel(sel, bit, queries, 'index_cmux_level')
+        out = self.empty((queries, pairs // 2, 2, N), torch.int32)
+        if queries and pairs:
+            self._call('nb_index_cmux_level', _ptr(x), stride, sp, sstride, _ptr(out), pairs // 2, queries)
+        return out
+
+    def index_rotate_extract(self, acc, sel, bits, columns, queries):
+        """Rotation by the low index bits and extraction (nb_index_rotate_extract): acc (queries, A, 2, N) or (A, 2, N)
+        shared, A = columns for bits >= 10, else 1; sel (queries, bits, R).  Returns a (columns, queries, N) and
+        b (columns, queries)."""
+        acc = self._dense(acc, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        accs, stride = self._index_nodes(acc, queries, 'index_rotate_extract')
+        if accs != (columns if bits >= 10 else 1) or sel.dim() != 3 or sel.shape[1] != bits:
+            raise ValueError('index_rotate_extract: %d accumulators and %s selector spectra for %d columns of %d bits'
+                             % (accs, tuple(sel.shape), columns, bits))
+        sp, sstride = self._index_sel(sel, 0, queries, 'index_rotate_extract')
+        out_a, out_b = self.empty((columns, queries, N), torch.int32), self.empty((columns, queries), torch.int32)
+        if queries:
+            self._call('nb_index_rotate_extract', _ptr(acc), stride, sp, sstride, int(bits), columns, _ptr(out_a),
+                       _ptr(out_b), queries)
+        return out_a, out_b
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()
