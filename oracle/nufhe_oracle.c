@@ -436,6 +436,36 @@ void orc_blind_rotate(i32 *acc, const u64 *bk, const i32 *bara, size_t n, size_t
             mux_rotate_one(acc + b * 2 * NPOLY, bk + i * 8 * NPOLY, bara[b * n + i]);
 }
 
+/* The multi-bit blind rotation of nufhe_b200 (DESIGN.md section 14; the reference has no multi-bit key), built from the
+ * restated steps above.  Key bits are taken two at a time; group g reads rows 3g, 3g+1, 3g+2 of bk (TGSW encryptions
+ * of the indicators of the bit patterns p = 1, 2, 3, p = s_2g + 2 s_2g+1) and does
+ *     ACC += sum_p (X^{k_p} - 1) (Dec(ACC) (x) BK_{g,p}),   k_1 = bara_2g, k_2 = bara_2g+1, k_3 = k_1 + k_2 mod 2N.
+ * Every external product is the exact integer product reduced mod 2^32 (its coefficients stay far below p / 2), and
+ * multiplication by X^k - 1 commutes with that reduction, so the result is exact.  acc (B,2,N); bara (B, n), n even. */
+static void mux_rotate_mb_one(i32 *acc /*2,N*/, const u64 *bk_group /*3 rows*/, int k0, int k1)
+{
+    const int ks[3] = {k0, k1, (k0 + k1) % (2 * NPOLY)};
+    i32 prod[2 * NPOLY], rot[2 * NPOLY];
+    u32 sum[2 * NPOLY] = {0};
+    for (int p = 0; p < 3; p++) {
+        memcpy(prod, acc, sizeof(prod));
+        external_mul_one(prod, bk_group + (size_t)p * 8 * NPOLY);
+        shift_poly_one(rot, prod, ks[p], 1);
+        shift_poly_one(rot + NPOLY, prod + NPOLY, ks[p], 1);
+        for (int x = 0; x < 2 * NPOLY; x++) sum[x] += (u32)rot[x];
+    }
+    for (int x = 0; x < 2 * NPOLY; x++) acc[x] = (i32)((u32)acc[x] + sum[x]);
+}
+
+void orc_blind_rotate_mb(i32 *acc, const u64 *bk, const i32 *bara, size_t n, size_t batch)
+{
+    init_tables();
+#pragma omp parallel for schedule(dynamic, 1)
+    for (size_t b = 0; b < batch; b++)
+        for (size_t g = 0; g < n / 2; g++)
+            mux_rotate_mb_one(acc + b * 2 * NPOLY, bk + g * 3 * 8 * NPOLY, bara[b * n + 2 * g], bara[b * n + 2 * g + 1]);
+}
+
 /* LweKeyswitchReference, lwe_cpu.py:62-93.  ks_a (in, t, base, out), ks_b/ks_cv (in, t, base). */
 void orc_lwe_keyswitch(i32 *res_a, i32 *res_b, float *res_cv,
                        const i32 *ks_a, const i32 *ks_b, const float *ks_cv,

@@ -30,6 +30,7 @@ MU = numpy.int32(2**29)            # phase_to_t32(1, 8), numeric_functions.py:30
 
 
 def build(force=False):
+    """(Re)compile libnufhe_oracle.so when it is missing or older than nufhe_oracle.c."""
     src = os.path.join(_HERE, 'nufhe_oracle.c')
     if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < os.path.getmtime(src):
         subprocess.check_call(['make', '-C', _HERE, '-s', 'libnufhe_oracle.so'])
@@ -273,6 +274,20 @@ def blind_rotate(acc, bk, bara):
     B = out.size // (2 * N)
     n = bara.size // B
     lib().orc_blind_rotate(_p(out), _p(bk), _p(bara), _sz(n), _sz(B))
+    return out
+
+
+def blind_rotate_mb(acc, bk, bara):
+    """The multi-bit blind rotation (orc_blind_rotate_mb): acc (B, 2, N), bara (B, n) in [0, 2N) with n even, bk the
+    multi-bit key's 3n/2 (or more) rows in the reference's transformed form (B, 2, 2, 2, N) uint64."""
+    out = _c(acc, numpy.int32).copy()
+    bk = _c(bk, numpy.uint64)
+    bara = _c(bara, numpy.int32)
+    B = out.size // (2 * N)
+    n = bara.size // B
+    assert n % 2 == 0 and bk.size >= 3 * (n // 2) * 8 * N, (n, bk.shape)
+    assert ((bara >= 0) & (bara < 2 * N)).all()
+    lib().orc_blind_rotate_mb(_p(out), _p(bk), _p(bara), _sz(n), _sz(B))
     return out
 
 

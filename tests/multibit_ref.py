@@ -11,9 +11,12 @@ Every product is an exact integer polynomial reduced mod 2^32.  It is computed w
 halves of the key (coefficients below 6 x 2^36, so the rounding error of a length-1024 FFT is orders of magnitude
 below 1/2), and every coefficient is checked to lie within 1/4 of an integer before it is rounded: a sanity check
 that catches a reference drifting towards its precision limit, not a proof of exactness (an error above 3/4 would
-pass it).  This is a float reference, not an exact-integer oracle: the C oracle has no multi-bit mode.  What pins it
-instead: the same machinery run as the standard rotation (`blind_rotate_std`) gives the C oracle's bootstrap bit for
-bit, and with noiseless keys both rotations give the exact rotation (tests/test_host_multibit.py)."""
+pass it).  It is fast enough for large batches on the GPU (torch), but it is not exact.  The exact-integer oracle is the
+C oracle's multi-bit rotation (`blind_rotate_oracle`, O.blind_rotate_mb, on the key's transformed rows): every
+composition below takes the rotation as its `rotate` argument, so the same composition runs on either.  The two agree
+bit for bit on noisy keys, random and edge rotations (tests/test_host_multibit.py); the same float machinery run as the
+standard rotation (`blind_rotate_std`) gives the C oracle's bootstrap bit for bit, and with noiseless keys every
+rotation gives the exact rotation."""
 import numpy
 import torch
 
@@ -129,6 +132,12 @@ def blind_rotate_mb(acc, bara, bk_raw, device='cpu'):
     return _from_acc(acc)
 
 
+def blind_rotate_oracle(acc, bara, bk_ref, device=None):
+    """the exact-integer multi-bit rotation of the C oracle (O.blind_rotate_mb); bk_ref is the key in the reference's
+    transformed form (the second value of multibit_key), not its raw rows"""
+    return O.blind_rotate_mb(acc, bk_ref, bara)
+
+
 def blind_rotate_std(acc, bara, bk_raw, device='cpu'):
     """the standard rotation through the same machinery: ACC += Dec((X^a_i - 1) ACC) [x] BK_i"""
     F = _Fft(device)
@@ -159,13 +168,13 @@ def bootstrap_extract(x1, x2, c, s1, s2, mu, bk_raw, device='cpu', rotate=blind_
     return O.tlwe_extract_lwe_samples(acc)
 
 
-def bootstrap_extract2(job_a, job_b, mu, bk_raw, device='cpu'):
-    ra = bootstrap_extract(*job_a, mu, bk_raw, device)
-    rb = bootstrap_extract(*job_b, mu, bk_raw, device)
+def bootstrap_extract2(job_a, job_b, mu, bk_raw, device='cpu', rotate=blind_rotate_mb):
+    ra = bootstrap_extract(*job_a, mu, bk_raw, device, rotate)
+    rb = bootstrap_extract(*job_b, mu, bk_raw, device, rotate)
     return numpy.concatenate([ra[0], rb[0]]), numpy.concatenate([ra[1], rb[1]])
 
 
-def bootstrap_lut_extract(x1, x2, c, s1, s2, tv, L, bk_raw, device='cpu'):
+def bootstrap_lut_extract(x1, x2, c, s1, s2, tv, L, bk_raw, device='cpu', rotate=blind_rotate_mb):
     """the programmable bootstrap (nb_bootstrap_lut_extract) with a multi-bit key"""
     from fused_ref import prologue, _extract_outputs
     a, b = prologue(x1, x2, c, s1, s2)
@@ -174,17 +183,17 @@ def bootstrap_lut_extract(x1, x2, c, s1, s2, tv, L, bk_raw, device='cpu'):
     bara = (O.t32_to_phase(a, (2 * N) >> L).astype(numpy.int64) << L).astype(numpy.int32)
     tvs = numpy.ascontiguousarray(numpy.broadcast_to(numpy.asarray(tv).reshape(-1, N), (B, N)))
     acc = O.tlwe_noiseless_trivial(O.shift_torus_polynomial(tvs[:, None, :], barb, invert_powers=True)[:, 0])
-    acc = blind_rotate_mb(acc, bara, bk_raw, device)
+    acc = rotate(acc, bara, bk_raw, device)
     return _extract_outputs(acc, L)
 
 
-def bootstrap_glwe_lut_extract(x, tv, bk_raw, device='cpu'):
+def bootstrap_glwe_lut_extract(x, tv, bk_raw, device='cpu', rotate=blind_rotate_mb):
     """nb_bootstrap_glwe_lut_extract with a multi-bit key"""
     from fused_ref import i32
     a, b = i32(x[0]), i32(x[1])
     barb, bara = O.t32_to_phase(b, 2 * N), O.t32_to_phase(a, 2 * N)
     acc = O.shift_torus_polynomial(numpy.asarray(tv, numpy.int32), barb, invert_powers=True)
-    acc = blind_rotate_mb(acc, bara, bk_raw, device)
+    acc = rotate(acc, bara, bk_raw, device)
     return O.tlwe_extract_lwe_samples(acc)
 
 

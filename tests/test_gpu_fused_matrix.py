@@ -25,15 +25,12 @@ import torch
 
 import gen_inputs as G
 import fused_ref as F
+from fused_ref import EDGE_ROT, Mode, gate_mode, glwe_mode, guarded, lut_mode, ptr, unguard, x2_mode
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
 N = 1024
-GUARD = 3                                   # sentinel rows before and after every output
-SENTINEL = 0x5A5A5A5A
 FFT_U64 = 16 * 512 * 2                      # the FP64 part at the end of every engine key row
-EDGE_ROT = [0, 1, 1023, 1024, 1025, 2047]
-TV_EDGES = [-2**31, 2**31 - 1, 0]
 
 # (WIDE_MAX, WIDE2_MAX, PAIR_MAX, PAIR_ASYNC, FFT)
 SHAPES = {'fp64': ('0', '0', '0', '1', '1'), 'ntt': ('0', '0', '0', '1', '0'),
@@ -104,189 +101,7 @@ def runs_fp64(shape, kind):
     return shape == 'fp64' or (shape.startswith('pair') and kind == 'plain')
 
 
-# ---- inputs with constructed edge rows ------------------------------------------------------------------------------
-
-def _i32(v):
-    v = int(v) % 2**32
-    return v - 2**32 if v >= 2**31 else v
-
-
-def _solve(target, s, rest):
-    """x with s x = target - rest mod 2^32 (s = 2^k u, u odd; target - rest must be a multiple of 2^k)"""
-    d = (int(target) - int(rest)) % 2**32
-    k = ((s & -s).bit_length() - 1)
-    assert d % (1 << k) == 0, (target, s, rest)
-    return _i32((d >> k) * pow(s >> k, -1, 2**32))
-
-
-def gate_targets():
-    """prologue bodies / mask coefficients whose mod-switch to [0, 2N) is an edge value: the centre and the lower
-    rounding tie of each"""
-    return [v << 21 for v in EDGE_ROT] + [(v << 21) - 2**20 for v in EDGE_ROT]
-
-
-def lut_targets(L):
-    """the rounding ties of modswitch_lut: m 2^(21+L) + 2^(20+L) + {-1, 0, 1}, m = 0, 1, around N and at the wrap"""
-    ms = [0, 1, 2**(10 - L) - 1, 2**(10 - L), 2**(11 - L) - 1]
-    return [(m << (21 + L)) + (1 << (20 + L)) + d for m in ms for d in (-1, 0, 1)]
-
-
-def lwe_inputs(rng, B, n, c, s1, s2, two, targets, even_only=False):
-    """x1 (and x2 if `two`) random, the first rows solved so that the prologue's body and mask coefficients cycle
-    through `targets`: for x2 where s2 is odd, else for x1 with x2 = 0"""
-    x1 = (G.torus32(rng, (B, n)), G.torus32(rng, (B,)))
-    x2 = (G.torus32(rng, (B, n)), G.torus32(rng, (B,))) if two else None
-    T = [t for t in targets if not even_only or t % 2 == 0]
-    for r in range(min(B, len(T))):
-        for i in range(n + 1):
-            t = T[(r + i) % len(T)]
-            cc = int(c) if i == n else 0
-            if two and s2 % 2:
-                v1 = int(x1[1][r] if i == n else x1[0][r, i])
-                v = _solve(t, s2, cc + s1 * v1)
-                if i == n:
-                    x2[1][r] = v
-                else:
-                    x2[0][r, i] = v
-            else:
-                if two:
-                    if i == n:
-                        x2[1][r] = 0
-                    else:
-                        x2[0][r, i] = 0
-                v = _solve(t, s1, cc)
-                if i == n:
-                    x1[1][r] = v
-                else:
-                    x1[0][r, i] = v
-    return x1, x2
-
-
-def make_test_vectors(rng, rows, width=None):
-    tv = G.torus32(rng, (rows, N) if width is None else (rows, width, N))
-    flat = tv.reshape(-1, N)
-    for r in range(min(flat.shape[0], 6)):
-        flat[r, 0], flat[r, N - 1] = TV_EDGES[r % 3], TV_EDGES[(r + 1) % 3]
-    return tv
-
-
-# ---- modes: inputs, the oracle on rows `rows`, and the C ABI call ---------------------------------------------------
-
-def _ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def _guarded(eng, rows, width):
-    return torch.full((rows + 2 * GUARD, width), SENTINEL, dtype=torch.int32, device=eng.device)
-
-
-def _host(buf, what):
-    h = buf.cpu().numpy()
-    assert (h[:GUARD] == SENTINEL).all() and (h[-GUARD:] == SENTINEL).all(), 'a store outside the rows of ' + what
-    return h[GUARD:-GUARD]
-
-
-def _dev(eng, x):
-    return (None, None) if x is None else (eng.to_device(x[0]), eng.to_device(x[1]))
-
-
-class Mode:
-    """kind: gate, x2 (extract2, B = job batch), lut, glwe, explicit, plain.  want[k] holds output k for the
-    ciphertexts (job rows for x2) `rows`, leading axis first; run() returns the same outputs for the batch's prefix."""
-
-    def __init__(self, name, kind, n, want, rows, upload, call):
-        self.name, self.kind, self.n, self.want, self.rows = name, kind, n, want, rows
-        self.upload, self.call = upload, call
-        self.key_free = False
-
-    def check(self, got, B, what):
-        k = int(numpy.searchsorted(self.rows, B))
-        sel = self.rows[:k]
-        for i, (g, w) in enumerate(zip(got, self.want)):
-            assert (g[sel] == w[:k]).all(), (what, self.name, B, 'output', i)
-
-    def equal(self, got, B):
-        k = int(numpy.searchsorted(self.rows, B))
-        return all((g[self.rows[:k]] == w[:k]).all() for g, w in zip(got, self.want))
-
-
-def gate_mode(name, n, bk, c, s1, s2, mu, two, seed, B, rows=None, x=None):
-    rng = G.rs(seed)
-    x1, x2 = x if x is not None else lwe_inputs(rng, B, n, c, s1, s2, two, gate_targets(), even_only=s1 % 2 == 0)
-    rows = numpy.arange(B) if rows is None else rows
-    sub = lambda v: None if v is None else (v[0][rows], v[1][rows])   # noqa: E731
-    want = F.bootstrap_extract(sub(x1), sub(x2), c, s1, s2, mu, bk)
-
-    def call(eng, dev, bk_int, b):
-        (a1, b1), (a2, b2) = dev
-        oa, ob = _guarded(eng, b, N), _guarded(eng, b, 1)
-        eng._call('nb_bootstrap_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), c, s1, s2, mu, bk_int.data_ptr(), n,
-                  oa[GUARD].data_ptr(), ob[GUARD].data_ptr(), b)
-        return _host(oa, 'out_a'), _host(ob, 'out_b')[:, 0]
-    m = Mode(name, 'gate', n, want, rows, lambda eng: (_dev(eng, x1), _dev(eng, x2)), call)
-    # mu = -2^31 is its own negation: the accumulator is the constant -2^31 at every step, whatever the key
-    m.key_free = mu == -2**31
-    return m
-
-
-def x2_mode(name, n, bk, job_a, job_b, mu, seed, B, rows=None):
-    """job = (c, s1, s2, two); every operand and constant of job B differs from job A's"""
-    rng = G.rs(seed)
-    xs = [lwe_inputs(rng, B, n, c, s1, s2, two, gate_targets(), even_only=s1 % 2 == 0) for c, s1, s2, two in (job_a, job_b)]
-    rows = numpy.arange(B) if rows is None else rows
-    sub = lambda v: None if v is None else (v[0][rows], v[1][rows])   # noqa: E731
-    ja = (sub(xs[0][0]), sub(xs[0][1])) + tuple(job_a[:3])
-    jb = (sub(xs[1][0]), sub(xs[1][1])) + tuple(job_b[:3])
-    wa, wb = F.bootstrap_extract(*ja, mu, bk), F.bootstrap_extract(*jb, mu, bk)
-
-    def call(eng, dev, bk_int, b):
-        (a1, b1), (a2, b2), (c1, d1), (c2, d2) = dev
-        oa, ob = _guarded(eng, 2 * b, N), _guarded(eng, 2 * b, 1)
-        eng._call('nb_bootstrap_extract2', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), *job_a[:3],
-                  _ptr(c1), _ptr(d1), _ptr(c2), _ptr(d2), *job_b[:3], mu, bk_int.data_ptr(), n,
-                  oa[GUARD].data_ptr(), ob[GUARD].data_ptr(), b)
-        ga, gb = _host(oa, 'out_a'), _host(ob, 'out_b')[:, 0]
-        return ga[:b], gb[:b], ga[b:], gb[b:]
-    return Mode(name, 'x2', n, (wa[0], wa[1], wb[0], wb[1]), rows,
-                lambda eng: tuple(_dev(eng, v) for v in (xs[0][0], xs[0][1], xs[1][0], xs[1][1])), call)
-
-
-def lut_mode(name, n, bk, L, per_ct, two, seed, B, rows=None):
-    rng = G.rs(seed)
-    c, s1, s2 = (12345678, 2, -3) if two else (-987654, -1, 5)       # s2 is ignored without x2
-    x1, x2 = lwe_inputs(rng, B, n, c, s1, s2, two, lut_targets(L))
-    tv = make_test_vectors(rng, B if per_ct else 1)
-    tv = tv if per_ct else tv[0]
-    rows = numpy.arange(B) if rows is None else rows
-    K = 1 << L
-    sub = lambda v: None if v is None else (v[0][rows], v[1][rows])   # noqa: E731
-    wa, wb = F.bootstrap_lut_extract(sub(x1), sub(x2), c, s1, s2, tv[rows] if per_ct else tv, L, bk)
-
-    def call(eng, dev, bk_int, b):
-        (a1, b1), (a2, b2), dtv = dev
-        oa, ob = _guarded(eng, b * K, N), _guarded(eng, b * K, 1)
-        eng._call('nb_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), c, s1, s2, dtv.data_ptr(),
-                  N if per_ct else 0, L, bk_int.data_ptr(), n, oa[GUARD].data_ptr(), ob[GUARD].data_ptr(), b)
-        return _host(oa, 'out_a').reshape(b, K, N), _host(ob, 'out_b').reshape(b, K)
-    return Mode(name, 'lut', n, (wa.reshape(-1, K, N), wb.reshape(-1, K)), rows,
-                lambda eng: (_dev(eng, x1), _dev(eng, x2), eng.to_device(tv)), call)
-
-
-def glwe_mode(name, n, bk, seed, B, rows=None):
-    rng = G.rs(seed)
-    x, _ = lwe_inputs(rng, B, n, 0, 1, 0, False, gate_targets() + lut_targets(0))
-    tv = make_test_vectors(rng, B, 2)
-    rows = numpy.arange(B) if rows is None else rows
-    want = F.bootstrap_glwe_lut_extract((x[0][rows], x[1][rows]), tv[rows], bk)
-
-    def call(eng, dev, bk_int, b):
-        (a, bb), dtv = dev
-        oa, ob = _guarded(eng, b, N), _guarded(eng, b, 1)
-        eng._call('nb_bootstrap_glwe_lut_extract', _ptr(a), _ptr(bb), dtv.data_ptr(), bk_int.data_ptr(), n,
-                  oa[GUARD].data_ptr(), ob[GUARD].data_ptr(), b)
-        return _host(oa, 'out_a'), _host(ob, 'out_b')[:, 0]
-    return Mode(name, 'glwe', n, want, rows, lambda eng: (_dev(eng, x), eng.to_device(tv)), call)
-
+# ---- modes only the standard key has ----------------------------------------------------------------------------
 
 def explicit_mode(name, n, bk, seed, B):
     rng = G.rs(seed)
@@ -298,10 +113,10 @@ def explicit_mode(name, n, bk, seed, B):
 
     def call(eng, dev, bk_int, b):
         dacc, dbara = dev
-        oa, ob, oacc = _guarded(eng, b, N), _guarded(eng, b, 1), _guarded(eng, b, 2 * N)
-        eng._call('nb_blind_rotate', dacc.data_ptr(), dbara.data_ptr(), bk_int.data_ptr(), n, oa[GUARD].data_ptr(),
-                  ob[GUARD].data_ptr(), oacc[GUARD].data_ptr(), b)
-        return _host(oa, 'out_a'), _host(ob, 'out_b')[:, 0], _host(oacc, 'accum_out').reshape(b, 2, N)
+        oa, ob, oacc = guarded(eng, b, N), guarded(eng, b, 1), guarded(eng, b, 2 * N)
+        eng._call('nb_blind_rotate', dacc.data_ptr(), dbara.data_ptr(), bk_int.data_ptr(), n, oa[F.GUARD].data_ptr(),
+                  ob[F.GUARD].data_ptr(), oacc[F.GUARD].data_ptr(), b)
+        return unguard(oa, 'out_a'), unguard(ob, 'out_b')[:, 0], unguard(oacc, 'accum_out').reshape(b, 2, N)
     mode = Mode(name, 'explicit', n, (wa, wb, wacc), numpy.arange(B),
                 lambda eng: (eng.to_device(acc), eng.to_device(bara)), call)
     mode.acc = acc
@@ -315,10 +130,10 @@ def plain_mode(name, n, bk, seed, B):
     want = F.external_product(acc, bk, row)
 
     def call(eng, dev, bk_int, b):
-        buf = _guarded(eng, b, 2 * N)
-        buf[GUARD:GUARD + b] = dev[:b].reshape(b, 2 * N)
-        eng._call('nb_external_product', buf[GUARD].data_ptr(), bk_int.data_ptr(), row, b)
-        return (_host(buf, 'accum').reshape(b, 2, N),)
+        buf = guarded(eng, b, 2 * N)
+        buf[F.GUARD:F.GUARD + b] = dev[:b].reshape(b, 2 * N)
+        eng._call('nb_external_product', buf[F.GUARD].data_ptr(), bk_int.data_ptr(), row, b)
+        return (unguard(buf, 'accum').reshape(b, 2, N),)
     return Mode(name, 'plain', n, (want,), numpy.arange(B), lambda eng: eng.to_device(acc), call)
 
 

@@ -1,6 +1,6 @@
-"""Multi-bit bootstrap keys on the CPU (DESIGN.md section 14): the reference rotation (tests/multibit_ref.py) against
-the oracle and the noiseless-key identity, the kernel's pass-3 model run by the host emulator against the reference
-bit for bit, the exactness bound at worst-case inputs, key generation on the oracle-backed engine double, and the
+"""Multi-bit bootstrap keys on the CPU (DESIGN.md section 14): the C oracle's exact multi-bit rotation and the float
+reference rotation (tests/multibit_ref.py) against each other, against the oracle's standard bootstrap and against the
+noiseless-key identity, the kernel's pass-3 model run by the host emulator against both bit for bit, the exactness bound at worst-case inputs, key generation on the oracle-backed engine double, and the
 noise rules and argument checks of the Python layer."""
 import ctypes
 import hashlib
@@ -46,11 +46,55 @@ def test_reference_standard_rotation_matches_the_oracle():
     assert numpy.array_equal(got[0], want[0]) and numpy.array_equal(got[1], want[1])
 
 
-@pytest.mark.parametrize('rotate', [M.blind_rotate_std, M.blind_rotate_mb])
+EDGE_ROT = [0, 1, N - 1, N, N + 1, 2 * N - 1]
+
+
+def test_oracle_rotation_matches_reference_at_random_rotations():
+    """the exact oracle's multi-bit rotation equals the float reference bit for bit: noisy key, random accumulators and
+    rotations, n = 26"""
+    keys = O.OracleKeys(37, n=26, make_bk=False)
+    raw, ref = M.multibit_key(keys, 38)
+    rng = numpy.random.RandomState(6)
+    B = 8
+    acc = rng.randint(-2**31, 2**31, size=(B, 2, N), dtype=numpy.int64).astype(numpy.int32)
+    bara = rng.randint(0, 2 * N, size=(B, keys.n)).astype(numpy.int32)
+    got = M.blind_rotate_oracle(acc, bara, ref)
+    assert numpy.array_equal(got, M.blind_rotate_mb(acc, bara, raw))
+    assert not numpy.array_equal(got, acc)
+
+
+def test_oracle_rotation_matches_reference_at_every_edge_pair():
+    """every ordered pair of the rotation edges 0, 1, N - 1, N, N + 1, 2N - 1 as some group's (abar_2g, abar_2g+1),
+    including the pairs whose sum wraps past 2N: the oracle equals the float reference bit for bit"""
+    keys = O.OracleKeys(39, n=36, make_bk=False)
+    raw, ref = M.multibit_key(keys, 40)
+    pairs = numpy.array([(x, y) for x in EDGE_ROT for y in EDGE_ROT], numpy.int32)      # 36 pairs
+    rng = numpy.random.RandomState(7)
+    B = 2
+    acc = rng.randint(-2**31, 2**31, size=(B, 2, N), dtype=numpy.int64).astype(numpy.int32)
+    bara = pairs.reshape(B, keys.n)
+    assert (pairs.sum(1) >= 2 * N).any()
+    assert numpy.array_equal(M.blind_rotate_oracle(acc, bara, ref), M.blind_rotate_mb(acc, bara, raw))
+
+
+def test_oracle_rotation_refuses_bad_arguments():
+    keys = O.OracleKeys(41, n=4, make_bk=False)
+    ref = M.multibit_key(keys, 42)[1]
+    acc = numpy.zeros((1, 2, N), numpy.int32)
+    with pytest.raises(AssertionError):
+        O.blind_rotate_mb(acc, ref, numpy.zeros((1, 3), numpy.int32))            # odd n
+    with pytest.raises(AssertionError):
+        O.blind_rotate_mb(acc, ref, numpy.zeros((1, 6), numpy.int32))            # fewer than n / 2 groups
+    with pytest.raises(AssertionError):
+        O.blind_rotate_mb(acc, ref, numpy.full((1, 4), 2 * N, numpy.int32))      # rotation outside [0, 2N)
+
+
+@pytest.mark.parametrize('rotate', [M.blind_rotate_std, M.blind_rotate_mb, M.blind_rotate_oracle])
 def test_noiseless_keys_rotate_exactly(rotate):
-    """noiseless keys, test vectors of multiples of 2^12: both rotations give exactly X^(sum abar_i s_i) tv"""
+    """noiseless keys, test vectors of multiples of 2^12: every rotation gives exactly X^(sum abar_i s_i) tv"""
     keys = O.OracleKeys(33, n=64, make_bk=False)
-    raw = (M.multibit_key if rotate is M.blind_rotate_mb else M.standard_key)(keys, 0, noiseless=True)[0]
+    raw, ref = (M.standard_key if rotate is M.blind_rotate_std else M.multibit_key)(keys, 0, noiseless=True)
+    raw = ref if rotate is M.blind_rotate_oracle else raw
     rng = numpy.random.RandomState(2)
     B = 6
     bara = rng.randint(0, 2 * N, size=(B, keys.n))
@@ -77,8 +121,8 @@ def _group(emul, acc, rows_ref, rot):
 @pytest.mark.parametrize('case', ['random', 'worst'])
 def test_emulated_group_matches_reference(emul, case):
     """one group of the kernel's multi-bit step (fwd1, fwd2, the 3-row pass 3, inv2, inv1; host emulator) against the
-    reference, both ciphertext slots, for a noisy key and for keys at the extremes of the 32-bit range with digits at
-    -512 / 511"""
+    float reference and the exact oracle, both ciphertext slots, for a noisy key and for keys at the extremes of the
+    32-bit range with digits at -512 / 511"""
     rng = numpy.random.RandomState(3 if case == 'random' else 4)
     keys = O.OracleKeys(35, n=2, make_bk=False)
     if case == 'random':
@@ -105,6 +149,7 @@ def test_emulated_group_matches_reference(emul, case):
         got = _group(emul, acc, ref, rot)
         want = M.blind_rotate_mb(acc, rot, raw)
         assert numpy.array_equal(got, want)
+        assert numpy.array_equal(got, M.blind_rotate_oracle(acc, rot, ref))
 
 
 def _negacyclic(a, b):
