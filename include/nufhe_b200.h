@@ -3,7 +3,8 @@
  * path of nucypher/nufhe, for programmable bootstrapping (lookup tables on small encrypted integers,
  * nb_bootstrap_lut_extract), for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
  * device from a seed (nb_seeded_uniform_i32), for public-key encryption (nb_pk_prepare, nb_pk_encrypt), and for
- * packing results into GLWE samples (nb_pack_digits, nb_ntt_mac, nb_pack_finish).
+ * packing results into GLWE samples (nb_pack_digits, nb_ntt_mac, nb_pack_finish), and for compact public-key
+ * encryption (nb_compact_finish, nb_compact_extract).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -279,6 +280,24 @@ int nb_index_cmux_level(nb_ctx *ctx, const int32_t *in, size_t in_query_stride, 
 int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_stride, const uint64_t *sel,
                             size_t sel_query_stride, int bits, size_t columns, int32_t *out_a, int32_t *out_b,
                             size_t queries);
+
+/* ---- compact public-key encryption (DESIGN.md section 16; no reference counterpart).  B messages go into
+ * G = ceil(B / 1024) GLWE samples under the bootstrap key's GLWE key S (k + 1 polynomials of N = 1024 coefficients),
+ * message c in group c / 1024, slot c % 1024, every coefficient rounded to 16 bits.  Encryption: nb_ntt_forward_i32 of
+ * the binary polynomials r (G, N), nb_ntt_mac with the spectra of the compact public key (1, k + 1, N),
+ * nb_ntt_inverse_i32, nb_compact_finish.  Expansion: nb_compact_extract, then nb_keyswitch with the cloud key.
+ * nb_compact_finish: c (G, k + 1, N) int32 (the products), e1 (G, k, N), e2 (G, N) and the messages mus (B,) int32 ->
+ *     out (G, k + 1, N) uint16: round_16(c_u + e1_u) for polynomials u < k, round_16(c_k + e2 + mus[g N + p]) at an
+ *     occupied coefficient p of the body and 0 at an empty one, round_16(x) = (x + 2^15) >> 16 on the 32-bit x.
+ *     NB_EINVAL for a NULL pointer and k < 1.
+ * nb_compact_extract: data (ceil(rows / 1024), k + 1, N) uint16 -> out_a (rows, k N), out_b (rows,) int32: with
+ *     x' = x << 16, row c = g N + p holds a[u N + j] = A'_u[p - j] for j <= p and -A'_u[N + p - j] for j > p, and
+ *     b = body'[p].  NB_EINVAL for a NULL pointer, k < 1, data not 8-byte or out_a not 16-byte aligned, and more than
+ *     65535 groups.
+ * batch / rows = 0 is a no-op for both. */
+int nb_compact_finish(nb_ctx *ctx, const int32_t *c, const int32_t *e1, const int32_t *e2, const int32_t *mus,
+                      int mask_size, uint16_t *out, size_t batch);
+int nb_compact_extract(nb_ctx *ctx, const uint16_t *data, int mask_size, int32_t *out_a, int32_t *out_b, size_t rows);
 
 #ifdef __cplusplus
 }

@@ -58,6 +58,12 @@ from .packing import (
     make_packing_keys,
     pack,
     )
+from .compact import (
+    NuFHECompactPublicKey,
+    CompactLweSampleArray,
+    compact_encrypt,
+    expand,
+    )
 from .tree_lut import (
     NuFHETreeKey,
     TreeLookupTable,

@@ -8,6 +8,7 @@ from .api_low_level import (
 from .lwe import LweSampleArray, lwe_copy, lwe_add_to
 from .compressed import CompressedLweSampleArray, CompressedCloudKey
 from .public_key import NuFHEPublicKey
+from .compact import NuFHECompactPublicKey, CompactLweSampleArray, expand
 from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
                       decrypt_packed, decrypt_packed_int)
 from .tree_lut import NuFHETreeKey, TreeLookupTable, lut_tree
@@ -106,7 +107,7 @@ class Context:
         return NuFHESecretKey.from_rng(self.thread, NuFHEParameters(**params), self.rng)
 
     def make_cloud_key(self, secret_key: NuFHESecretKey, compressed=False, tree_key=False, multi_bit=1,
-                       index_key=False):
+                       index_key=False, compact_public_key=False):
         """compressed=True returns a CompressedCloudKey (about 12 times smaller to store or send); its `decompress()`
         gives the NuFHECloudKey that make_virtual_machine takes.  tree_key=True returns (cloud key, NuFHETreeKey), the
         key of VirtualMachine.lut_tree; its draws follow all of the cloud key's, so the cloud key is the same either
@@ -114,7 +115,11 @@ class Context:
         bootstrap, about 3x the key rows and more noise; DESIGN.md section 14); ValueError for parameters it cannot
         take (tlwe_mask_size = 2, an odd LWE dimension) and for multi_bit outside {1, 2}.
         index_key=True also returns the NuFHEIndexSecretKey that encrypts indices for VirtualMachine.lookup; it draws
-        nothing.  With several extras the order is (cloud key, tree key, index key).  ValueError for tlwe_mask_size != 1."""
+        nothing.  With several extras the order is (cloud key, tree key, index key, compact public key).  ValueError for
+        tlwe_mask_size != 1.
+        compact_public_key=True also returns a NuFHECompactPublicKey (about 5 KB; DESIGN.md section 16): whoever holds it
+        encrypts up to 1024 messages per 4 KB ciphertext, which `VirtualMachine.expand` turns into LWE samples under this
+        cloud key.  Its draws follow all the other keys', so those are the same either way."""
         if index_key:
             check_index_params(secret_key.params)
         cls = CompressedCloudKey if compressed else NuFHECloudKey
@@ -125,6 +130,8 @@ class Context:
             out.append(NuFHETreeKey.from_secret_key(self.thread, self.rng, secret_key, tgsw_key))
         if index_key:
             out.append(NuFHEIndexSecretKey.from_tgsw_key(secret_key.params, tgsw_key))
+        if compact_public_key:
+            out.append(NuFHECompactPublicKey.from_tgsw_key(self.thread, self.rng, secret_key.params, tgsw_key))
         return out[0] if len(out) == 1 else tuple(out)
 
     def encrypt_index(self, index_key: NuFHEIndexSecretKey, values, bits, compressed=False):
@@ -148,8 +155,9 @@ class Context:
         return secret_key, cloud_key
 
     def encrypt(self, key, message, compressed=False):
-        """`key` is a NuFHESecretKey or a NuFHEPublicKey.  compressed=True (secret key only) returns a
-        CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute)."""
+        """`key` is a NuFHESecretKey, a NuFHEPublicKey or a NuFHECompactPublicKey.  compressed=True (secret key only)
+        returns a CompressedLweSampleArray (a seed and the bodies; `decompress()` to compute).  A compact public key
+        returns a CompactLweSampleArray (`VirtualMachine.expand` to compute)."""
         return encrypt(self.thread, self.rng, key, message, compressed=compressed)
 
     def decrypt(self, secret_key, ciphertext):
@@ -191,6 +199,16 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return NuFHEPublicKey.loads(file_or_bytestring, self.thread)
         return NuFHEPublicKey.load(file_or_bytestring, self.thread)
+
+    def load_compact_public_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHECompactPublicKey.loads(file_or_bytestring, self.thread)
+        return NuFHECompactPublicKey.load(file_or_bytestring, self.thread)
+
+    def load_compact_ciphertext(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return CompactLweSampleArray.loads(file_or_bytestring, self.thread)
+        return CompactLweSampleArray.load(file_or_bytestring, self.thread)
 
     def load_packed_ciphertext(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
@@ -341,6 +359,16 @@ class VirtualMachine:
         if packing_key.params != self.params:
             raise ValueError('the packing key was made for other parameters than this virtual machine')
         return pack(self.thread, packing_key, ciphertexts)
+
+    def expand(self, compact: CompactLweSampleArray):
+        """The LweSampleArray, of the same shape, of compact public-key ciphertexts (nufhe_b200/compact.py): sample
+        extraction, then this VM's key switch, a few groups per pass.  TypeError for anything but a
+        CompactLweSampleArray, ValueError for one made for other parameters."""
+        if not isinstance(compact, CompactLweSampleArray):
+            raise TypeError('expand needs a CompactLweSampleArray, got %s' % type(compact).__name__)
+        if compact.params != self.params:
+            raise ValueError('the compact ciphertexts were made for other parameters than this virtual machine')
+        return expand(self.thread, self.params, self.cloud_key.keyswitch_key, compact)
 
     def capture(self, circuit, reserve_batch=None):
         """Record `circuit()` -- any sequence of this VM's gates on device-resident ciphertexts -- into a CUDA graph;

@@ -168,6 +168,11 @@ def t32_to_bool(mu):
 
 def _encrypt_mus(thr, rng, key, shape, mus, compressed):
     from .public_key import NuFHEPublicKey, public_encrypt
+    from .compact import NuFHECompactPublicKey, compact_encrypt
+    if isinstance(key, NuFHECompactPublicKey):
+        if compressed:
+            raise ValueError("a compact public-key encryption is already compact: compressed=True does not apply")
+        return compact_encrypt(thr, rng, key, mus.reshape(shape))
     if isinstance(key, NuFHEPublicKey):
         if compressed:
             raise ValueError("a public-key encryption cannot be compressed: its mask depends on the secret random "
@@ -186,7 +191,8 @@ def _encrypt_mus(thr, rng, key, shape, mus, compressed):
 def encrypt(thr, rng, key, message, compressed=False):
     """api_low_level.py:266-281.  compressed=True returns a CompressedLweSampleArray: the mask is regenerated from a
     seed (nufhe_b200/compressed.py), so only the bodies and the seed are stored or sent.  `key` is a NuFHESecretKey or
-    a NuFHEPublicKey (nufhe_b200/public_key.py; not with compressed=True)."""
+    a NuFHEPublicKey (nufhe_b200/public_key.py; not with compressed=True); a NuFHECompactPublicKey
+    (nufhe_b200/compact.py; not with compressed=True) gives a CompactLweSampleArray."""
     message = numpy.asarray(message)
     mus = thr.to_device(numpy.ascontiguousarray(bool_to_t32(message)))
     return _encrypt_mus(thr, rng, key, message.shape, mus, compressed)
@@ -200,7 +206,8 @@ def decrypt(thr, key: NuFHESecretKey, ciphertext: LweSampleArray):
 
 def encrypt_int(thr, rng, key, values, bits, compressed=False):
     """Encrypt integers in [0, 2^bits), bits = 1..3, for lookup tables (nufhe_b200/lut.py: m * 2^(31 - bits)).
-    compressed=True returns a CompressedLweSampleArray, as for encrypt(); `key` may be a NuFHEPublicKey."""
+    compressed=True returns a CompressedLweSampleArray, as for encrypt(); `key` may be a NuFHEPublicKey or a
+    NuFHECompactPublicKey."""
     from .lut import encode_int
     values = numpy.asarray(values)
     mus = thr.to_device(numpy.ascontiguousarray(encode_int(values, bits)))

@@ -10,6 +10,8 @@ the engine regenerates the masks from it with ChaCha20 (Engine.seeded_uniform, n
     packing key          its own                    4       (n, t, k, N)
     tree key             its own                    5       (n, t, k, N)
     encrypted index      its own, per encryption    6       (rows, k+1, l, k, N), rows = shape x bits (index_lookup.py)
+    compact public key   its own                    7       (k, N) (compact.py)
+    compact encryption   its own, per encryption    8       (G, N / 32) words of the binary polynomials r (compact.py)
 
 Seeds are drawn from the context RNG as `rng.uniform_torus32((8,))`.  `decompress()` gives the ordinary objects
 (LweSampleArray, NuFHECloudKey) that the rest of the library takes.

@@ -8,6 +8,7 @@
 #include "../../include/nufhe_b200.h"
 #include "kernels.cuh"
 #include "index_lookup.cuh"
+#include "compact.cuh"
 #include "tables.h"
 
 using namespace nb;
@@ -1081,6 +1082,40 @@ int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_st
     p.steps = bits < 10 ? bits : 10;
     p.log2_stride = bits;
     return index_launch(ctx, p, true, "nb_index_rotate_extract");
+}
+
+// ---- compact public-key encryption (compact.cuh) ----
+
+int nb_compact_finish(nb_ctx *ctx, const int32_t *c, const int32_t *e1, const int32_t *e2, const int32_t *mus,
+                      int mask_size, uint16_t *out, size_t batch)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!c || !e1 || !e2 || !mus || !out) return fail(ctx, NB_EINVAL, "nb_compact_finish: null argument");
+    if (mask_size < 1 || mask_size > (1 << 16)) return fail(ctx, NB_EINVAL, "nb_compact_finish: bad mask size");
+    if (batch == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:compact_finish");
+    const size_t total = (batch + PACK_N - 1) / PACK_N * (size_t)(mask_size + 1) * PACK_N;
+    compact_finish_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(c, e1, e2, mus, (u32)mask_size, (u64)batch, out,
+                                                                        (u64)total);
+    return launch_check(ctx, "compact_finish_kernel");
+}
+
+int nb_compact_extract(nb_ctx *ctx, const uint16_t *data, int mask_size, int32_t *out_a, int32_t *out_b, size_t rows)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!data || !out_a || !out_b) return fail(ctx, NB_EINVAL, "nb_compact_extract: null argument");
+    if (mask_size < 1 || mask_size > 65535) return fail(ctx, NB_EINVAL, "nb_compact_extract: bad mask size");
+    if (((uintptr_t)data & 7) || ((uintptr_t)out_a & 15))
+        return fail(ctx, NB_EINVAL, "nb_compact_extract: data must be 8-byte and out_a 16-byte aligned");
+    if (rows == 0) return NB_OK;
+    const size_t groups = (rows + PACK_N - 1) / PACK_N;
+    if (groups > 65535) return fail(ctx, NB_EINVAL, "nb_compact_extract: more than 65535 groups in one call");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:compact_extract");
+    const dim3 grid(PACK_N / CX_ROWS, (unsigned)groups, (unsigned)mask_size);
+    compact_extract_kernel<<<grid, CX_THREADS, 0, ctx->stream>>>(data, (u32)mask_size, (u64)rows, out_a, out_b);
+    return launch_check(ctx, "compact_extract_kernel");
 }
 
 }  // extern "C"

@@ -11,6 +11,7 @@
 #include "pk_layout.cuh"
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
+#include "compact_layout.cuh"
 
 using namespace nb;
 
@@ -603,6 +604,23 @@ void emul_pack_digits(const i32 *a, size_t count, i32 *out)
 void emul_pack_round16(const u32 *x, size_t count, uint16_t *out) { for (size_t i = 0; i < count; i++) out[i] = pack_round16(x[i]); }
 void emul_pack_unround16(const uint16_t *x, size_t count, u32 *out) { for (size_t i = 0; i < count; i++) out[i] = pack_unround16(x[i]); }
 void emul_pack_slot(u64 c, u64 *group, u32 *slot) { *group = pack_group(c); *slot = pack_slot(c); }
+
+// Compact public-key encryption (compact_layout.cuh): `count` output coefficients (body / occupied flags as bytes), and
+// the extraction of slot p from one group's data (k + 1, N) uint16 -> a (k N,), *b.
+void emul_compact_coeff(const u32 *product, const u32 *noise, const uint8_t *body, const uint8_t *occupied,
+                        const u32 *mu, size_t count, uint16_t *out)
+{
+    for (size_t i = 0; i < count; i++) out[i] = compact_coeff(product[i], noise[i], body[i] != 0, occupied[i] != 0, mu[i]);
+}
+void emul_compact_extract(const uint16_t *data, int k, u32 p, i32 *a, i32 *b)
+{
+    std::vector<u32> poly(PACK_N);
+    for (int u = 0; u < k; u++) {
+        for (int i = 0; i < PACK_N; i++) poly[i] = pack_unround16(data[u * PACK_N + i]);
+        for (u32 j = 0; j < (u32)PACK_N; j++) a[u * PACK_N + j] = compact_extract(poly.data(), p, j);
+    }
+    *b = (i32)pack_unround16(data[k * PACK_N + p]);
+}
 
 // Tree-based programmable bootstrapping (tree_layout.cuh).  emul_tree_keyswitch: tree_prepare_kernel's planes, then
 // tree_keyswitch_kernel's tile loop with a scalar model of mma.sync.m16n8k32.row.col.s32.s8.u8.s32 that places each

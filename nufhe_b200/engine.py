@@ -404,6 +404,38 @@ class Engine:
             self._call('nb_pack_finish', _ptr(c), _ptr(b), k1 - 1, _ptr(out), batch)
         return out
 
+    def compact_finish(self, c, e1, e2, mus):
+        """The products c (G, k+1, N) int32, the noises e1 (G, k, N) and e2 (G, N) and the messages mus (B,) int32 ->
+        compact data (G, k+1, N) uint16: round_16(c + e1) for the masks, round_16(c + e2 + mu) at the occupied slots of
+        the body, 0 at its empty slots (nb_compact_finish)."""
+        c = self._dense(c, torch.int32)
+        e1 = self._dense(e1, torch.int32)
+        e2 = self._dense(e2, torch.int32)
+        mus = self._dense(mus, torch.int32).reshape(-1)
+        batch = mus.numel()
+        if c.dim() != 3 or c.shape[2] != N or c.shape[0] != (batch + N - 1) // N:
+            raise ValueError('compact_finish: %s products for %d messages' % (tuple(c.shape), batch))
+        groups, k1 = c.shape[0], c.shape[1]
+        if tuple(e1.shape) != (groups, k1 - 1, N) or tuple(e2.shape) != (groups, N):
+            raise ValueError('compact_finish: noises %s and %s for products %s'
+                             % (tuple(e1.shape), tuple(e2.shape), tuple(c.shape)))
+        out = self.empty(tuple(c.shape), torch.uint16)
+        if batch:
+            self._call('nb_compact_finish', _ptr(c), _ptr(e1), _ptr(e2), _ptr(mus), k1 - 1, _ptr(out), batch)
+        return out
+
+    def compact_extract(self, data, rows):
+        """Compact data (G, k+1, N) uint16 -> the LWE samples of its first `rows` slots under the extracted key of S:
+        a (rows, k N) and b (rows,) int32, every coefficient shifted back by 16 bits (nb_compact_extract)."""
+        data = self._dense(data, torch.uint16)
+        if data.dim() != 3 or data.shape[2] != N or data.shape[0] != (rows + N - 1) // N:
+            raise ValueError('compact_extract: data %s for %d rows' % (tuple(data.shape), rows))
+        k1 = data.shape[1]
+        out_a, out_b = self.empty((rows, (k1 - 1) * N), torch.int32), self.empty((rows,), torch.int32)
+        if rows:
+            self._call('nb_compact_extract', _ptr(data), k1 - 1, _ptr(out_a), _ptr(out_b), rows)
+        return out_a, out_b
+
     def tree_prepare(self, masks, body):
         """The tree key's masks (n, t, k, N) and bodies (n, t, N) int32 laid into the 4 byte planes that tree_keyswitch
         reads (nb_tree_prepare): a uint8 tensor of nb_tree_planes_bytes(n, k) bytes."""
