@@ -134,6 +134,20 @@ int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, cons
                  size_t in_size, size_t n, int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv,
                  size_t batch);
 
+/* ---- the key switch as a tensor-core GEMM (DESIGN.md section 4).  nb_ks_prepare lays a key-switch key with in = 1024,
+ * n = 500, t = 8 and base 4 into the byte planes that keyswitch_mma_kernel streams (`out`: nb_ks_prepared_bytes()
+ * bytes, 16-byte aligned, about 50 MB), and registers them on the context under (ks_a, ks_b).  From then on
+ * nb_keyswitch with that ks_a and ks_b runs batches from a measured threshold up (environment variable
+ * NUFHE_B200_KS_MMA_MIN, read at context creation) as one exact u8 x u8 -> s32 wgmma GEMM; results and variances are
+ * bit-identical to the other path.  Rows d = 0 are left out of the GEMM: a key whose d = 0 rows are not all zero is
+ * prepared but not registered, and keeps the other path.  *registered (may be NULL) is 1 when the key was
+ * registered.  Prepare again after changing the key, and call nb_ks_forget(ctx, ks_a) before freeing `out` or the
+ * key.  NB_EUNSUPPORTED for other parameters, NB_EINVAL for a NULL pointer or a misaligned `out`. */
+size_t nb_ks_prepared_bytes(void);
+int nb_ks_prepare(nb_ctx *ctx, const int32_t *ks_a, const int32_t *ks_b, uint8_t *out, size_t in_size, size_t n, int t,
+                  int log2_base, int *registered);
+int nb_ks_forget(nb_ctx *ctx, const int32_t *ks_a);
+
 /* ---- LweLinear / LweNoiselessTrivial (lwe.py:346-422): res = (0, c) + s1 * x1 + s2 * x2 ------- */
 int nb_lwe_affine(nb_ctx *ctx, int32_t *res_a, int32_t *res_b, const int32_t *x1_a, const int32_t *x1_b,
                   const int32_t *x2_a, const int32_t *x2_b, int32_t c, int32_t s1, int32_t s2, size_t batch,

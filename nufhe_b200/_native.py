@@ -44,6 +44,9 @@ SIGNATURES = {
     'nb_bootstrap_extract2': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32,
                               _vp, _sz, _vp, _vp, _sz],
     'nb_keyswitch': [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp, _vp, _vp, _sz],
+    'nb_ks_prepared_bytes': [],
+    'nb_ks_prepare': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp],
+    'nb_ks_forget': [_vp, _vp],
     'nb_lwe_affine': [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _sz, _sz],
     'nb_shift_torus_polynomial': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _int, _sz],
     'nb_tlwe_noiseless_trivial': [_vp, _vp, _vp, _vp, _int, _int, _sz],
@@ -72,7 +75,7 @@ SIGNATURES = {
     'nb_compact_finish': [_vp, _vp, _vp, _vp, _vp, _int, _vp, _sz],
     'nb_compact_extract': [_vp, _vp, _int, _vp, _vp, _sz],
 }
-_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_bk_multibit_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
+_RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_ks_prepared_bytes': ctypes.c_size_t, 'nb_bk_multibit_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
              'nb_tree_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p,
              'nb_build_info': ctypes.c_char_p}
 

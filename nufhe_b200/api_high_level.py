@@ -272,6 +272,8 @@ class VirtualMachine:
         from .tgsw import engine_format, fused_kernel_supported
         if perf_params.single_kernel_bootstrap and fused_kernel_supported(cloud_key.bootstrap_key.bk_params):
             engine_format(thread, cloud_key.bootstrap_key.tgsw)
+        # and the key-switch key for the tensor-core key switch, for the same reason
+        cloud_key.keyswitch_key.prepare_gemm(thread)
 
     def empty_ciphertext(self, shape):
         return empty_ciphertext(self.thread, self.params, shape)

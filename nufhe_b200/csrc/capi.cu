@@ -13,6 +13,10 @@
 
 using namespace nb;
 
+// smallest batch whose key switch runs on keyswitch_mma_kernel when the key is prepared (NUFHE_B200_KS_MMA_MIN
+// overrides it)
+constexpr size_t KS_MMA_MIN_DEFAULT = 256;
+
 struct nb_ctx {
     int device;
     cudaStream_t stream;
@@ -37,6 +41,10 @@ struct nb_ctx {
     int32_t *d_state;                    // parked accumulators of time-sliced launches
     size_t state_words;
     float *d_cv_blocks;                  // block sums of the key-switch variances (split launches)
+    // key-switch keys prepared on this context for keyswitch_mma_kernel (nb_ks_prepare): (ks_a, ks_b) -> planes
+    struct KsKey { const int32_t *ks_a, *ks_b; const uint8_t *planes; };
+    std::vector<KsKey> ks_keys;
+    size_t ks_mma_min;                   // smallest batch whose key switch runs as the tensor-core GEMM
     u64 *d_index_tmp;                    // nb_index_prepare: field elements of one chunk of selector rows
     size_t index_tmp_words;
     size_t cv_words;
@@ -170,6 +178,13 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
                      "cudaFuncSetAttribute(blind_rotate pair)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)KS_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch)"));
+    NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)KM_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch_mma)"));
+    {
+        // below this batch the split launch of keyswitch_kernel is faster than the GEMM
+        const char *e = getenv("NUFHE_B200_KS_MMA_MIN");
+        ctx->ks_mma_min = e ? (size_t)atoll(e) : KS_MMA_MIN_DEFAULT;
+    }
     NB_TRY(check_resident<BrDefault>(ctx));
     NB_TRY(check_resident<BrWide>(ctx));
     NB_TRY(check_resident<BrWide2>(ctx));
@@ -656,7 +671,35 @@ int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, cons
     p.src1_a = src1_a; p.src1_b = src1_b; p.src2_a = src2_a; p.src2_b = src2_b; p.c = c;
     p.ks_a = ks_a; p.ks_b = ks_b; p.ks_cv = ks_cv; p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
     p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch;
-    if (t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N) {
+    const bool fast = t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N;
+    const uint8_t *planes = nullptr;
+    if (fast && batch >= ctx->ks_mma_min &&
+        (((uintptr_t)src1_a | (uintptr_t)(src2_a ? src2_a : src1_a)) & 15) == 0 && ((uintptr_t)res_a & 7) == 0)
+        for (const auto &k : ctx->ks_keys)
+            if (k.ks_a == ks_a && k.ks_b == ks_b) planes = k.planes;
+    if (planes) {
+        // the GEMM: tiles of 256 ciphertexts x 32 output columns; K is split over blockIdx.z (partial sums meet in
+        // integer atomics) while a launch would leave half of the SMs idle
+        KeyswitchMmaArgs m{};
+        m.src1_a = src1_a; m.src1_b = src1_b; m.src2_a = src2_a; m.src2_b = src2_b; m.c = c;
+        m.planes = planes; m.res_a = res_a; m.res_b = res_b; m.batch = batch;
+        const size_t tiles = (batch + KM_M - 1) / KM_M * KM_NTILES;
+        int splits = 1;
+        while (splits < 16 && tiles * (size_t)splits * 2 <= (size_t)ctx->sm_count) splits *= 2;
+        m.splits = splits;
+        if (splits > 1) {
+            NB_TRY(check(ctx, cudaMemsetAsync(res_a, 0, batch * n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+            NB_TRY(check(ctx, cudaMemsetAsync(res_b, 0, batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+        }
+        keyswitch_mma_kernel<<<dim3((unsigned)((batch + KM_M - 1) / KM_M), KM_NTILES, splits), KM_THREADS, KM_SMEM_BYTES,
+                               ctx->stream>>>(m);
+        if (res_cv) {
+            NB_TRY(launch_check(ctx, "keyswitch_mma_kernel"));
+            ks_cv_kernel<<<(unsigned)((batch + 31) / 32), 256, 0, ctx->stream>>>(src1_a, src2_a, ks_cv, res_cv, batch);
+        }
+        return launch_check(ctx, "keyswitch_mma_kernel");
+    }
+    if (fast) {
         // The consumer loop always walks KS_TILE ciphertext slots, so a CTA costs the same whatever its tile:
         // fill the tiles, then split the 1024 input coefficients over blockIdx.y until the SMs are covered
         // (partial sums meet in integer atomics).  One ciphertext: 128 CTAs x 8 coefficients.
@@ -684,6 +727,51 @@ int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, cons
         keyswitch_generic_kernel<<<(int)batch, 512, 0, ctx->stream>>>(p);
     }
     return launch_check(ctx, "keyswitch_kernel");
+}
+
+size_t nb_ks_prepared_bytes(void) { return KM_PLANES_BYTES; }
+
+int nb_ks_prepare(nb_ctx *ctx, const int32_t *ks_a, const int32_t *ks_b, uint8_t *out, size_t in_size, size_t n, int t,
+                  int log2_base, int *registered)
+{
+    if (!ctx || !ks_a || !ks_b || !out) return fail(ctx, NB_EINVAL, "nb_ks_prepare: null argument");
+    if (registered) *registered = 0;
+    if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N))
+        return fail(ctx, NB_EUNSUPPORTED, "nb_ks_prepare: the GEMM layout is for in = 1024, n = 500, t = 8, base 4 only");
+    if ((uintptr_t)out & 15) return fail(ctx, NB_EINVAL, "nb_ks_prepare: out must be 16-byte aligned");
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:ks_prepare");
+    nb_ks_forget(ctx, ks_a);
+    for (size_t i = 0; i < ctx->ks_keys.size();) {      // registrations whose planes `out` overwrites
+        const uint8_t *p = ctx->ks_keys[i].planes;
+        if (p < out + KM_PLANES_BYTES && out < p + KM_PLANES_BYTES) ctx->ks_keys.erase(ctx->ks_keys.begin() + i);
+        else i++;
+    }
+    int *d_flag = nullptr, pad_nonzero = 0;
+    NB_TRY(check(ctx, cudaMalloc(&d_flag, sizeof(int)), "cudaMalloc(ks_prepare)"));
+    int rc = check(ctx, cudaMemsetAsync(d_flag, 0, sizeof(int), ctx->stream), "cudaMemsetAsync");
+    if (rc == NB_OK) {
+        ks_prepare_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(ks_a, ks_b, out, d_flag);
+        rc = launch_check(ctx, "ks_prepare_kernel");
+    }
+    if (rc == NB_OK) rc = check(ctx, cudaMemcpyAsync(&pad_nonzero, d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream), "cudaMemcpyAsync");
+    if (rc == NB_OK) rc = check(ctx, cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize");
+    cudaFree(d_flag);
+    NB_TRY(rc);
+    // a key with non-zero d = 0 rows keeps keyswitch_kernel, which adds them
+    if (!pad_nonzero) ctx->ks_keys.push_back({ks_a, ks_b, out});
+    if (registered) *registered = !pad_nonzero;
+    return NB_OK;
+}
+
+int nb_ks_forget(nb_ctx *ctx, const int32_t *ks_a)
+{
+    if (!ctx) return NB_EINVAL;
+    for (size_t i = 0; i < ctx->ks_keys.size();) {
+        if (ctx->ks_keys[i].ks_a == ks_a) ctx->ks_keys.erase(ctx->ks_keys.begin() + i);
+        else i++;
+    }
+    return NB_OK;
 }
 
 static int ew_grid(nb_ctx *ctx, size_t n)

@@ -1284,6 +1284,267 @@ __global__ void ks_cv_finalize_kernel(float *__restrict__ res_cv, const float *_
     res_cv[c] = cv;
 }
 
+// ---- the key switch as a tensor-core GEMM (DESIGN.md section 4): res = -OneHot . Key mod 2^32.
+// OneHot has one row per ciphertext and one column per (j, k, d >= 1): 1 where digit (j, k) equals d (row d = 0 of a
+// generated key is zero padding, so it is dropped: nb_ks_prepare registers only keys whose d = 0 rows are zero).
+// Key has those 24 576 rows and 512 columns (ks_a, then ks_b in column 500, then zeros), split into its 4 byte planes,
+// which become 4 x 512 u8 columns.  Every plane sum is at most 8192 * 255 < 2^21, so the u8 x u8 -> s32 products are
+// exact and sum_p S_p << 8p is the key switch's sum mod 2^32.
+// Tiles: a CTA takes KM_M = 256 ciphertexts (4 consumer warpgroups of 64) and one N tile of 128 GEMM columns: output
+// columns 32 nt .. 32 nt + 31, in all 4 planes (plane p in GEMM columns 32p .. 32p + 31), so one thread holds the 4
+// plane sums of each of its outputs.  K runs in KM_GROUPS stages of 96: stage G holds j = G + 256 tig (tig < 4), d
+// (one per k32 chunk) and k, in the order that makes thread (g, tig) of a warp build its A fragments from the digits of
+// one coefficient j per row: byte e of register half h of chunk c is [digit(j, 4h + 3 - e) == c + 1] (ks_mma_k_index).
+constexpr int KM_M = 256;                       // ciphertexts per CTA
+constexpr int KM_NT = 128;                      // GEMM columns per CTA: 32 outputs x 4 byte planes
+constexpr int KM_NTILES = 512 / 32;             // N tiles over the 512 padded output columns
+constexpr int KM_GROUPS = KS_IN / 4;            // K stages: 4 coefficients j (96 rows of K) each
+constexpr int KM_STAGE_BYTES = 96 * KM_NT;      // one stage of one N tile: 3 chunks of [16 x 8 rows][2 x 16 B]
+constexpr int KM_STAGES = 8;                    // TMA ring depth
+constexpr int KM_CONSUMERS = 4 * 128;
+constexpr int KM_THREADS = KM_CONSUMERS + 128;  // + producer warpgroup (one lane issues the copies)
+// registers per thread after setmaxnreg: the producer warpgroup gives back what the consumers' 64 accumulators need
+// (640 threads launch with 96 each)
+constexpr int KM_PRODUCER_REGS = 24, KM_CONSUMER_REGS = 112;
+constexpr size_t KM_SMEM_BYTES = (size_t)KM_STAGES * KM_STAGE_BYTES + 2 * KM_STAGES * 8;
+constexpr size_t KM_PLANES_BYTES = (size_t)KM_NTILES * KM_GROUPS * KM_STAGE_BYTES;   // 50 331 648
+
+// The row of the key (j, k, d) and the byte position in the prepared layout of K index `kpos` (0 .. 95) of stage G:
+// chunk c = kpos / 32, half h = (kpos / 16) & 1, tig = (kpos / 4) & 3, e = kpos & 3.
+NB_HD void ks_mma_k_index(int G, int kpos, int *j, int *k, int *d)
+{
+    const int c = kpos >> 5, h = (kpos >> 4) & 1, tig = (kpos >> 2) & 3, e = kpos & 3;
+    *j = G + KM_GROUPS * tig;
+    *k = 4 * h + 3 - e;
+    *d = c + 1;
+}
+// byte offset in the prepared key of (N tile nt, stage G, GEMM column col < 128, K index kpos < 96): chunks of 32 K
+// rows in the no-swizzle K-major layout of wgmma, core matrices of 8 columns x 16 bytes, the two K halves of a group
+// of 8 columns side by side (leading byte offset 128), groups of 8 columns 256 bytes apart (stride byte offset)
+NB_HD size_t ks_mma_offset(int nt, int G, int col, int kpos)
+{
+    return ((size_t)nt * KM_GROUPS + G) * KM_STAGE_BYTES + (size_t)(kpos >> 5) * (32 * KM_NT) + (col >> 3) * 256 +
+           ((kpos >> 4) & 1) * 128 + (col & 7) * 16 + (kpos & 15);
+}
+
+struct KeyswitchMmaArgs {
+    const i32 *src1_a, *src1_b, *src2_a, *src2_b;   // (B, 1024), (B,); rows 16-byte aligned
+    i32 c;
+    const uint8_t *planes;                          // nb_ks_prepare
+    i32 *res_a, *res_b;                             // (B, 500), (B,)
+    size_t batch;
+    int splits;                                     // > 1: blockIdx.z takes KM_GROUPS / splits stages, integer
+                                                    // atomics into zeroed outputs
+};
+
+// nb_ks_prepare: one thread per 4 consecutive bytes of the layout (same j, d, column; k = 4h + 3 .. 4h), and a check
+// that the d = 0 rows are zero (their one-hot columns are not in the GEMM)
+__global__ void ks_prepare_kernel(const i32 *__restrict__ ks_a, const i32 *__restrict__ ks_b, uint8_t *__restrict__ planes,
+                                  int *__restrict__ pad_nonzero)
+{
+    const size_t words = KM_PLANES_BYTES / 4, pad_words = (size_t)KS_IN * 8 * (KS_N + 1);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < words + pad_words; i += (size_t)gridDim.x * blockDim.x) {
+        if (i >= words) {
+            const size_t r = (i - words) / (KS_N + 1), x = (i - words) % (KS_N + 1);   // row (j, k, d = 0)
+            if ((x < KS_N ? ks_a[r * 4 * KS_N + x] : ks_b[r * 4]) != 0) atomicOr(pad_nonzero, 1);
+            continue;
+        }
+        size_t rest = i;
+        const int kq = (int)(rest & 3); rest >>= 2;      // 4-byte group inside the 16-byte core-matrix row
+        const int n_in = (int)(rest & 7); rest >>= 3;
+        const int h = (int)(rest & 1); rest >>= 1;
+        const int n8 = (int)(rest & 15); rest >>= 4;
+        const int c = (int)(rest % 3); rest /= 3;
+        const int G = (int)(rest % KM_GROUPS), nt = (int)(rest / KM_GROUPS);
+        const int col = n8 * 8 + n_in, plane = col >> 5, oc = 32 * nt + (col & 31);
+        u32 v = 0;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            int j, k, d;
+            ks_mma_k_index(G, 32 * c + 16 * h + 4 * kq + e, &j, &k, &d);
+            const size_t row = ((size_t)j * 8 + k) * 4 + d;
+            const u32 w = oc < KS_N ? (u32)ks_a[row * KS_N + oc] : oc == KS_N ? (u32)ks_b[row] : 0u;
+            v |= ((w >> (8 * plane)) & 0xFFu) << (8 * e);
+        }
+        *reinterpret_cast<u32 *>(planes + ks_mma_offset(nt, G, col, 32 * c + 16 * h + 4 * kq)) = v;
+    }
+}
+
+// 4 one-hot bytes from 4 flags at bits 0, 2, 4, 6 (the shifted copies do not overlap below bit 25)
+NB_D u32 km_spread(u32 y) { return (y * 0x41041u) & 0x01010101u; }
+
+NB_D void km_wgmma(u32 *d, const u32 *a, u64 desc)
+{
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
+        "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,"
+        "%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64, %65, %66, %67}, %68, p;\n}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+          "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]),
+          "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+          "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]),
+          "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]),
+          "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]),
+          "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]),
+          "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc), "r"(1));
+}
+
+// the 16-bit digit word of one input coefficient: digit k in bits 14 - 2k, 15 - 2k
+NB_D u32 km_digits(u32 a) { return (a + (1u << (32 - (1 + 2 * 8)))) >> 16; }
+
+__global__ void __launch_bounds__(KM_THREADS, 1) keyswitch_mma_kernel(KeyswitchMmaArgs p)
+{
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    unsigned char *ring = smem_raw;
+    u64 *full = reinterpret_cast<u64 *>(ring + KM_STAGES * KM_STAGE_BYTES);
+    u64 *empty = full + KM_STAGES;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int nt = blockIdx.y;
+    const int nstages = KM_GROUPS / p.splits, G0 = blockIdx.z * nstages;
+    if (tid == 0) {
+        for (int s = 0; s < KM_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], KM_CONSUMERS / 32); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp >= KM_CONSUMERS / 32) {
+        // ---- producer: one lane streams this N tile's stages G0 .. G0 + nstages - 1, 12 KB each
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(KM_PRODUCER_REGS));
+        if (warp == KM_CONSUMERS / 32 && lane == 0) {
+            const uint8_t *src = p.planes + ((size_t)nt * KM_GROUPS + G0) * KM_STAGE_BYTES;
+            for (int s = 0; s < nstages; s++) {
+                const int slot = s % KM_STAGES;
+                if (s >= KM_STAGES) mbar_wait(&empty[slot], ((s / KM_STAGES) - 1) & 1);
+                mbar_expect_tx(&full[slot], KM_STAGE_BYTES);
+                bulk_g2s(ring + slot * KM_STAGE_BYTES, src + (size_t)s * KM_STAGE_BYTES, KM_STAGE_BYTES, &full[slot]);
+            }
+        }
+        return;
+    }
+
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(KM_CONSUMER_REGS));
+    // ---- consumers: warpgroup wg owns ciphertexts 64 wg .. 64 wg + 63 of the tile; thread (g, tig) builds the rows
+    // g and g + 8 of its warp's 16, for coefficient j = G + 256 tig of stage G
+    const int g = lane >> 2, tig = lane & 3;
+    const size_t r0 = (size_t)blockIdx.x * KM_M + (warp >> 2) * 64 + (warp & 3) * 16 + g, r1 = r0 + 8;
+    const bool v0 = r0 < p.batch, v1 = r1 < p.batch;
+    const i32 *s1 = p.src1_a + r0 * KS_IN + KM_GROUPS * tig;          // row g + 8: 8 * KS_IN further
+    const i32 *s2 = p.src2_a ? p.src2_a + r0 * KS_IN + KM_GROUPS * tig : nullptr;
+    auto load4 = [&](int G, int4 *x0, int4 *x1) {   // src1 (+ src2) of stages G .. G + 3, zeros for rows past the batch
+        *x0 = v0 ? __ldg(reinterpret_cast<const int4 *>(s1 + G)) : make_int4(0, 0, 0, 0);
+        *x1 = v1 ? __ldg(reinterpret_cast<const int4 *>(s1 + 8 * KS_IN + G)) : make_int4(0, 0, 0, 0);
+        if (s2) {
+            const int4 y0 = v0 ? __ldg(reinterpret_cast<const int4 *>(s2 + G)) : make_int4(0, 0, 0, 0);
+            const int4 y1 = v1 ? __ldg(reinterpret_cast<const int4 *>(s2 + 8 * KS_IN + G)) : make_int4(0, 0, 0, 0);
+            x0->x += y0.x; x0->y += y0.y; x0->z += y0.z; x0->w += y0.w;
+            x1->x += y1.x; x1->y += y1.y; x1->z += y1.z; x1->w += y1.w;
+        }
+    };
+    // rows past the batch: digit word 0 (all digits 0, no one-hot column set)
+    auto pack = [&](i32 a0, i32 a1) { return (v0 ? km_digits((u32)a0) : 0u) | ((v1 ? km_digits((u32)a1) : 0u) << 16); };
+
+    u32 acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = 0;
+    const u32 ring_base = smem_u32(ring);
+    // matrix descriptor of chunk 0 of slot 0: start >> 4, leading byte offset 128 >> 4, stride byte offset 256 >> 4,
+    // no swizzle
+    const u64 desc0 = (u64)((ring_base & 0x3FFFF) >> 4) | ((u64)(128 >> 4) << 16) | ((u64)(256 >> 4) << 32);
+
+    int4 n0, n1;
+    load4(G0, &n0, &n1);
+    for (int q = 0; q < nstages; q += 4) {
+        const u32 w[4] = {pack(n0.x, n1.x), pack(n0.y, n1.y), pack(n0.z, n1.z), pack(n0.w, n1.w)};
+        if (q + 4 < nstages) load4(G0 + q + 4, &n0, &n1);
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int s = q + u, slot = s % KM_STAGES;
+            u32 a[3][4];
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                const u32 x = w[u] ^ (0x55555555u * (u32)(c + 1));
+                const u32 z = ~(x | (x >> 1)) & 0x55555555u;      // bit 14 - 2k (+ 16 for row g + 8): digit k == c + 1
+                a[c][0] = km_spread((z >> 8) & 0x55u);            // row g, k = 3 .. 0
+                a[c][1] = km_spread((z >> 24) & 0x55u);           // row g + 8, k = 3 .. 0
+                a[c][2] = km_spread(z & 0x55u);                   // row g, k = 7 .. 4
+                a[c][3] = km_spread((z >> 16) & 0x55u);           // row g + 8, k = 7 .. 4
+            }
+            mbar_wait(&full[slot], (s / KM_STAGES) & 1);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+            for (int c = 0; c < 3; c++)
+                km_wgmma(acc, a[c], desc0 + (u64)((slot * KM_STAGE_BYTES + c * 32 * KM_NT) >> 4));
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[slot]);
+        }
+    }
+
+    // ---- epilogue: acc[4i + 2r + e] is row g + 8r, GEMM column 8i + 2 tig + e; plane p in i = 4p .. 4p + 3
+    const bool split = p.splits > 1;
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+        const size_t row = r ? r1 : r0;
+        if (!(r ? v1 : v0)) continue;
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            u32 v[2];
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const int x = 4 * i + 2 * r + e;
+                v[e] = 0u - (acc[x] + (acc[x + 16] << 8) + (acc[x + 32] << 16) + (acc[x + 48] << 24));
+            }
+            const int col = 32 * nt + 8 * i + 2 * tig;
+            if (col < KS_N) {               // KS_N is even: both columns are mask coefficients
+                i32 *dst = p.res_a + row * KS_N + col;
+                if (!split) *reinterpret_cast<int2 *>(dst) = make_int2((i32)v[0], (i32)v[1]);
+                else {
+                    atomicAdd(reinterpret_cast<unsigned int *>(dst), v[0]);
+                    atomicAdd(reinterpret_cast<unsigned int *>(dst + 1), v[1]);
+                }
+            } else if (col == KS_N) {       // column 500: ks_b
+                const u32 b = blockIdx.z ? 0u : (u32)p.src1_b[row] + (p.src2_b ? (u32)p.src2_b[row] : 0u) + (u32)p.c;
+                if (!split) p.res_b[row] = (i32)(b + v[0]);
+                else atomicAdd(reinterpret_cast<unsigned int *>(p.res_b + row), b + v[0]);
+            }
+        }
+    }
+}
+
+// The variances beside keyswitch_mma_kernel, in the fixed shape of keyswitch_kernel (KS_CV_BLOCK_J): thread (q, part)
+// adds the 64 terms of blocks 16 part .. 16 part + 15 of ciphertext q in (j, k) order, thread (q, 0) adds the 128
+// block sums in block order.
+__global__ void __launch_bounds__(256) ks_cv_kernel(const i32 *__restrict__ src1_a, const i32 *__restrict__ src2_a,
+                                                    const float *__restrict__ ks_cv, float *__restrict__ res_cv, size_t batch)
+{
+    __shared__ float blocks[KS_CV_BLOCKS][33];
+    const int q = threadIdx.x & 31, part = threadIdx.x >> 5;
+    const size_t ct = (size_t)blockIdx.x * 32 + q;
+    if (ct < batch) {
+        for (int bk = part * (KS_CV_BLOCKS / 8); bk < (part + 1) * (KS_CV_BLOCKS / 8); bk++) {
+            float blk = 0.f;
+            for (int jj = 0; jj < KS_CV_BLOCK_J; jj++) {
+                const int j = bk * KS_CV_BLOCK_J + jj;
+                u32 v = (u32)src1_a[ct * KS_IN + j];
+                if (src2_a) v += (u32)src2_a[ct * KS_IN + j];
+                const u32 bits = km_digits(v);
+#pragma unroll
+                for (int k = 0; k < 8; k++) blk += __ldg(ks_cv + (j * 8 + k) * 4 + ((bits >> (14 - 2 * k)) & 3u));
+            }
+            blocks[bk][q] = blk;
+        }
+    }
+    __syncthreads();
+    if (part == 0 && ct < batch) {
+        float cv = 0.f;
+        for (int bk = 0; bk < KS_CV_BLOCKS; bk++) cv += blocks[bk][q];
+        res_cv[ct] = cv;
+    }
+}
+
 // Generic decomposition parameters (API parity with LweKeyswitch(…, decomp_length, log2_base)): the
 // straightforward per-ciphertext gather.
 __global__ void __launch_bounds__(512) keyswitch_generic_kernel(KeyswitchArgs p)

@@ -4,6 +4,7 @@ data, int64 holding the uint64 bit patterns of field elements) and enqueue work 
 PyTorch is used for device memory and streams only.
 """
 import ctypes
+import weakref
 
 import numpy
 import torch
@@ -234,6 +235,27 @@ class Engine:
                    _ptr(ks_cv), in_size, n, t, int(base).bit_length() - 1, _ptr(res_a), _ptr(res_b),
                    _ptr(res_cv), B)
         return res_a, res_b, res_cv
+
+    def ks_prepare(self, ks_a, ks_b):
+        """Lay a key-switch key (in = 1024, n = 500, t = 8, base 4) into the byte planes of the tensor-core key switch
+        and register them for (ks_a, ks_b) on this engine (nb_ks_prepare).  Returns the planes, which must stay alive
+        while the registration is wanted (it is dropped when they are freed), or None when the key's d = 0 rows are
+        not zero: such a key keeps the gather kernel.  Prepare outside any captured region: it allocates and
+        synchronizes."""
+        assert ks_a.is_contiguous() and ks_b.is_contiguous()
+        in_size, t, base, n = ks_a.shape
+        planes = self.empty((self.lib.nb_ks_prepared_bytes(),), torch.uint8)
+        registered = ctypes.c_int(0)
+        self._call('nb_ks_prepare', _ptr(ks_a), _ptr(ks_b), _ptr(planes), in_size, n, t, int(base).bit_length() - 1,
+                   ctypes.addressof(registered))
+        if not registered.value:
+            return None
+        weakref.finalize(planes, self._ks_forget, ks_a.data_ptr())
+        return planes
+
+    def _ks_forget(self, ks_a_ptr):
+        if self.handle:
+            self.lib.nb_ks_forget(self.handle, ctypes.c_void_p(ks_a_ptr))
 
     # --- the separate steps of the multi-kernel bootstrap (bootstrap.py:96-196) -------------------
     SHIFT_INVERT, SHIFT_MINUS_ONE, SHIFT_PLAIN = 0, 1, 2

@@ -212,6 +212,20 @@ class LweKeyswitchKey:
         lwe = self.lwe
         return (lwe.a.contiguous(), lwe.b.contiguous(), lwe.current_variances.contiguous())
 
+    def prepare_gemm(self, thr):
+        """Register the key for the tensor-core key switch on thr's device (Engine.ks_prepare), once per key array.
+        Every key switch with this key's arrays on that engine then uses it, at batches from the library's threshold.
+        Engines without it (the CPU test double) and other decomposition parameters keep the gather kernel."""
+        prepare = getattr(thr, 'ks_prepare', None)
+        if prepare is None or (self.input_size, self.decomp_length, self.log2_base, self.output_size) != (1024, 8, 2, 500):
+            return
+        if not (self.lwe.a.is_contiguous() and self.lwe.b.is_contiguous()):
+            return                              # the registration is for the arrays every key switch passes
+        ks_a, ks_b, _ = self.device_arrays()
+        cached = getattr(self, '_gemm_planes', None)
+        if cached is None or cached[0] is not thr or cached[1] != ks_a.data_ptr():
+            self._gemm_planes = (thr, ks_a.data_ptr(), prepare(ks_a, ks_b))
+
 
 def make_lwe_keyswitch_key(thr, lwe, in_key, out_key, noises_a, noises_b, log2_base, noise):
     """MakeLweKeyswitchKey (lwe_gpu.py:63-124, lwe_gpu.mako:18-56; ref lwe_cpu.py:26-59): row h=0 is
