@@ -33,6 +33,7 @@ class Engine:
         rc = self.lib.nb_ctx_create(self.device.index, stream_ptr, ctypes.byref(handle))
         self.handle = handle
         self._stream_ptr = stream_ptr.value or 0
+        self._ks_registrations = {}           # ks_a address -> token of its live ks_prepare registration
         if rc != _native.NB_OK:
             try:
                 _native.check(handle, rc, 'nb_ctx_create')
@@ -239,9 +240,10 @@ class Engine:
     def ks_prepare(self, ks_a, ks_b):
         """Lay a key-switch key (in = 1024, n = 500, t = 8, base 4) into the byte planes of the tensor-core key switch
         and register them for (ks_a, ks_b) on this engine (nb_ks_prepare).  Returns the planes, which must stay alive
-        while the registration is wanted (it is dropped when they are freed), or None when the key's d = 0 rows are
-        not zero: such a key keeps the gather kernel.  Prepare outside any captured region: it allocates and
-        synchronizes."""
+        while the registration is wanted, or None when the key's d = 0 rows are not zero: such a key keeps the gather
+        kernel.  The registration is dropped when the planes, ks_a or ks_b are freed, so that a later key at the same
+        addresses never meets these planes.  Preparing the key again moves its registration to the new planes.
+        Prepare outside any captured region: it allocates and synchronizes."""
         assert ks_a.is_contiguous() and ks_b.is_contiguous()
         in_size, t, base, n = ks_a.shape
         planes = self.empty((self.lib.nb_ks_prepared_bytes(),), torch.uint8)
@@ -250,10 +252,18 @@ class Engine:
                    ctypes.addressof(registered))
         if not registered.value:
             return None
-        weakref.finalize(planes, self._ks_forget, ks_a.data_ptr())
+        # nb_ks_prepare replaced any earlier registration of ks_a: the finalizers of the earlier planes must leave
+        # this one alone, so each registration carries its own token
+        token = object()
+        self._ks_registrations[ks_a.data_ptr()] = token
+        for owner in (planes, ks_a, ks_b):
+            weakref.finalize(owner, self._ks_forget, ks_a.data_ptr(), token)
         return planes
 
-    def _ks_forget(self, ks_a_ptr):
+    def _ks_forget(self, ks_a_ptr, token):
+        if self._ks_registrations.get(ks_a_ptr) is not token:
+            return                                  # already dropped, or replaced by a later prepare of the key
+        del self._ks_registrations[ks_a_ptr]
         if self.handle:
             self.lib.nb_ks_forget(self.handle, ctypes.c_void_p(ks_a_ptr))
 
