@@ -948,11 +948,10 @@ size_t nb_pk_planes_bytes(size_t m, size_t n)
     return 4 * m * (size_t)pk_cols_padded((u32)n);
 }
 
-// m rows of [A | b] for an n-word LWE key: m a multiple of 32 (whole k-steps) and every plane sum, at most m * 255,
-// below 2^31 so that the s32 accumulators are exact
+// m rows of [A | b] for an n-word LWE key: m a multiple of 32 (whole k-steps), and exact sums for 0/1 bytes of R
 static int pk_check_shape(nb_ctx *ctx, size_t m, size_t n, const char *what)
 {
-    if (m == 0 || m % 32 != 0 || (uint64_t)m * 255 >= (1ull << 31))
+    if (m == 0 || m % 32 != 0 || !plane_gemm_exact(m, 1))
         return fail(ctx, NB_EINVAL, std::string(what) + ": m must be a positive multiple of 32 with m * 255 < 2^31");
     if (n == 0 || n > (1u << 30)) return fail(ctx, NB_EINVAL, std::string(what) + ": bad LWE dimension");
     return NB_OK;
@@ -967,8 +966,9 @@ int nb_pk_prepare(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t m, siz
     NvtxRange nvtx_range("nufhe_b200:pk_prepare");
     const size_t quads = (size_t)pk_cols_padded((u32)n) * (m / 4);
     size_t blocks = (quads + 255) / 256, cap = (size_t)ctx->sm_count * 16;
-    pk_prepare_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(a, b, (u32)m, (u32)n, planes);
-    return launch_check(ctx, "pk_prepare_kernel");
+    plane_prepare_kernel<PkSource, const i32 *__restrict__, const i32 *__restrict__, u32, u32>
+        <<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(planes, a, b, (u32)m, (u32)n);
+    return launch_check(ctx, "plane_prepare_kernel<PkSource>");
 }
 
 int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, size_t m, size_t n, const int32_t *mus,
@@ -981,13 +981,14 @@ int nb_pk_encrypt(nb_ctx *ctx, const uint32_t *r_bits, const uint8_t *planes, si
     if (batch == 0) return NB_OK;
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:pk_encrypt");
-    const size_t rows_per_cta = (size_t)PK_WARPS * PK_MTILES * 16;
+    const size_t rows_per_cta = (size_t)GEMM_WARPS * GEMM_MTILES * 16;
     const size_t ctas = (batch + rows_per_cta - 1) / rows_per_cta;
     if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_pk_encrypt: batch too large");
-    const dim3 grid((unsigned)ctas, pk_cols_padded((u32)n) / 8);
-    pk_encrypt_kernel<<<grid, PK_WARPS * 32, 0, ctx->stream>>>(r_bits, planes, (u32)m, (u32)n, mus, row_variance,
-                                                               out_a, out_b, out_cv, (u64)batch);
-    return launch_check(ctx, "pk_encrypt_kernel");
+    const dim3 grid((unsigned)ctas, pk_cols_padded((u32)n) / (8 * PkGemm::NTILES));
+    plane_gemm_kernel<PkGemm, const u32 *__restrict__, u32, u32, const i32 *__restrict__, float, i32 *__restrict__,
+                      i32 *__restrict__, float *__restrict__><<<grid, GEMM_WARPS * 32, 0, ctx->stream>>>(
+        planes, (u64)batch, r_bits, (u32)m, (u32)n, mus, row_variance, out_a, out_b, out_cv);
+    return launch_check(ctx, "plane_gemm_kernel<PkGemm>");
 }
 
 int nb_pack_digits(nb_ctx *ctx, const int32_t *a, size_t n, int32_t *digits, size_t batch)
@@ -1042,10 +1043,10 @@ size_t nb_tree_planes_bytes(size_t n, int mask_size)
     return 4 * (size_t)tree_k_padded((u32)n) * (size_t)(mask_size + 1) * PACK_N;
 }
 
-// n t digit rows: every plane sum, at most kpad * 128 * 255, must stay below 2^31 for the s32 accumulators to be exact
+// n t digit rows padded to kpad, and exact sums for signed digits of magnitude up to 128
 static int tree_check_shape(nb_ctx *ctx, size_t n, int mask_size, const char *what)
 {
-    if (n == 0 || n > (1u << 20) || (uint64_t)tree_k_padded((u32)n) * 128 * 255 >= (1ull << 31))
+    if (n == 0 || n > (1u << 20) || !plane_gemm_exact(tree_k_padded((u32)n), 128))
         return fail(ctx, NB_EINVAL, std::string(what) + ": n t (padded to 32) * 128 * 255 must be below 2^31");
     if (mask_size < 1 || mask_size > 16) return fail(ctx, NB_EINVAL, std::string(what) + ": bad mask size");
     return NB_OK;
@@ -1060,9 +1061,9 @@ int nb_tree_prepare(nb_ctx *ctx, const int32_t *masks, const int32_t *body, size
     NvtxRange nvtx_range("nufhe_b200:tree_prepare");
     const size_t quads = (size_t)(mask_size + 1) * PACK_N * (tree_k_padded((u32)n) / 4);
     const size_t blocks = (quads + 255) / 256, cap = (size_t)ctx->sm_count * 16;
-    tree_prepare_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(masks, body, (u32)n,
-                                                                                      (u32)mask_size, planes);
-    return launch_check(ctx, "tree_prepare_kernel");
+    plane_prepare_kernel<TreeSource, const i32 *__restrict__, const i32 *__restrict__, u32, u32>
+        <<<(int)(blocks < cap ? blocks : cap), 256, 0, ctx->stream>>>(planes, masks, body, (u32)n, (u32)mask_size);
+    return launch_check(ctx, "plane_prepare_kernel<TreeSource>");
 }
 
 int nb_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *planes, size_t n, int mask_size, int32_t *out,
@@ -1072,15 +1073,16 @@ int nb_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *planes, size
     if (!a || !planes || !out) return fail(ctx, NB_EINVAL, "nb_tree_keyswitch: null argument");
     NB_TRY(tree_check_shape(ctx, n, mask_size, "nb_tree_keyswitch"));
     if (rows == 0) return NB_OK;
-    const size_t rows_per_cta = (size_t)TREE_WARPS * TREE_MTILES * 16;
+    const size_t rows_per_cta = (size_t)GEMM_WARPS * GEMM_MTILES * 16;
     const size_t ctas = (rows + rows_per_cta - 1) / rows_per_cta;
     if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, "nb_tree_keyswitch: too many rows");
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:tree_keyswitch");
     const u32 cols = (u32)(mask_size + 1) * PACK_N;
-    const dim3 grid((unsigned)ctas, cols / (8 * TREE_NTILES));
-    tree_keyswitch_kernel<<<grid, TREE_WARPS * 32, 0, ctx->stream>>>(a, planes, (u32)n, cols, out, (u64)rows);
-    return launch_check(ctx, "tree_keyswitch_kernel");
+    const dim3 grid((unsigned)ctas, cols / (8 * TreeGemm::NTILES));
+    plane_gemm_kernel<TreeGemm, const i32 *__restrict__, u32, u32, i32 *__restrict__>
+        <<<grid, GEMM_WARPS * 32, 0, ctx->stream>>>(planes, (u64)rows, a, (u32)n, cols, out);
+    return launch_check(ctx, "plane_gemm_kernel<TreeGemm>");
 }
 
 int nb_tree_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, int mask_size, int32_t *tv,

@@ -8,6 +8,7 @@
 #include "tables.h"
 #include "lut_index.cuh"
 #include "chacha.cuh"
+#include "plane_gemm.cuh"
 #include "pk_layout.cuh"
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
@@ -506,17 +507,19 @@ void emul_lut_tail(const i32 *acc, int j, i32 *out_a, i32 *out_b)
 // The ChaCha20 block function of the seeded masks (chacha.cuh): out[16] = block `counter` of the stream (seed[8], nonce)
 void emul_chacha_block(const u32 *seed, u64 counter, u64 nonce, u32 *out) { chacha20_block(seed, counter, nonce, out); }
 
-// Public-key encryption (pk_layout.cuh): pk_prepare_kernel's planes, then pk_encrypt_kernel's tile loop with a scalar
-// model of mma.sync.m16n8k32.row.col.s32.u8.u8.s32.  The model places each register byte by the fragment layout of the
-// PTX ISA (not by pk_layout.cuh), so a lane that feeds the wrong bits or plane bytes gives a wrong result here.
-static void mma_m16n8k32_u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4])
+// The byte-plane GEMM (plane_gemm.cuh): plane_prepare_kernel's planes, then plane_gemm_kernel's tile loop for the
+// same operand policy, with a scalar model of mma.sync.m16n8k32.row.col.s32.{u8,s8}.u8.s32.  The model places each
+// register byte by the fragment layout of the PTX ISA (not by plane_gemm.cuh), so a lane that feeds the wrong bits,
+// digits or plane bytes gives a wrong result here.
+static void mma_m16n8k32(bool signed_a, const u32 a[32][4], const u32 b[32][2], i32 c[32][4])
 {
-    u32 A[16][32], B[32][8];
+    i32 A[16][32], B[32][8];
     for (int l = 0; l < 32; l++) {
         const int g = l >> 2, t = l & 3;
         for (int j = 0; j < 16; j++) {          // a_j: register j / 4, byte j % 4
             const int row = g + ((j < 4 || (j >= 8 && j < 12)) ? 0 : 8), k = 4 * t + (j & 3) + (j >= 8 ? 16 : 0);
-            A[row][k] = (a[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
+            const u32 byte = (a[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
+            A[row][k] = signed_a ? (i32)(int8_t)byte : (i32)byte;
         }
         for (int j = 0; j < 8; j++) {           // b_j: register j / 4, byte j % 4
             const int k = 4 * t + (j & 3) + (j >= 4 ? 16 : 0);
@@ -530,7 +533,7 @@ static void mma_m16n8k32_u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4]
         if (!any) continue;                     // (a zero row adds nothing)
         for (int c2 = 0; c2 < 8; c2++) {
             i32 s = 0;
-            for (int k = 0; k < 32; k++) s += (i32)(A[r][k] * B[k][c2]);
+            for (int k = 0; k < 32; k++) s += A[r][k] * B[k][c2];
             D[r][c2] = s;
         }
     }
@@ -540,58 +543,72 @@ static void mma_m16n8k32_u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4]
     }
 }
 
-void emul_pk_encrypt(const u32 *r_bits, const i32 *a, const i32 *b, size_t m, size_t n, const i32 *mus,
-                     float row_variance, i32 *out_a, i32 *out_b, float *out_cv, size_t batch)
+extern "C++" template <class P, class Src>
+void emul_plane_gemm(const P &op, const Src &src, u64 rows)
 {
-    const u32 npad = pk_cols_padded((u32)n), words = (u32)(m >> 5);
-    std::vector<uint8_t> planes((size_t)4 * npad * m);
-    for (u32 col = 0; col < npad; col++)
-        for (u32 k = 0; k < m; k++) {
-            const u32 w = pk_source_word(a, b, (u32)n, k, col);
-            for (int p = 0; p < 4; p++) planes[pk_plane_offset(p, col, k, (u32)m, npad)] = (uint8_t)(w >> (8 * p));
+    const u32 K = src.K(), cols = src.cols();
+    std::vector<uint8_t> planes((size_t)4 * K * cols);
+    for (u32 col = 0; col < cols; col++)
+        for (u32 k = 0; k < K; k++) {
+            const u32 w = src(k, col);
+            for (int p = 0; p < 4; p++) planes[plane_offset(p, col, k, K, cols)] = (uint8_t)(w >> (8 * p));
         }
     auto load32 = [&](u64 off) { u32 v; memcpy(&v, planes.data() + off, 4); return v; };
-    const u64 plane_stride = pk_plane_offset(1, 0, 0, (u32)m, npad);
-    for (u64 row0 = 0; row0 < batch; row0 += 16 * PK_MTILES)      // one warp
-        for (u32 col0 = 0; col0 < npad; col0 += 8) {
-            static i32 acc[4][PK_MTILES][32][4];
-            memset(acc, 0, sizeof(acc));
-            for (u32 ks = 0; ks < words; ks++) {
-                u32 bf[4][32][2], af[PK_MTILES][32][4];
+    const u64 plane_stride = plane_offset(1, 0, 0, K, cols);
+    constexpr int NT = P::NTILES;
+    std::vector<i32> acc((size_t)4 * GEMM_MTILES * NT * 32 * 4);
+    auto A = [&](int p, int mt, int nt) {
+        return reinterpret_cast<i32 (*)[4]>(&acc[(((size_t)p * GEMM_MTILES + mt) * NT + nt) * 128]);
+    };
+    for (u64 row0 = 0; row0 < rows; row0 += 16 * GEMM_MTILES)        // one warp
+        for (u32 col0 = 0; col0 < cols; col0 += 8 * NT) {               // its CTA's column tiles
+            std::fill(acc.begin(), acc.end(), 0);
+            for (u32 ks = 0; ks < K >> 5; ks++) {
+                u32 bf[NT][4][32][2], af[GEMM_MTILES][32][4];
                 for (int l = 0; l < 32; l++) {
                     const int g = l >> 2, t = l & 3;
-                    const u64 bcol = pk_plane_offset(0, col0 + g, 0, (u32)m, npad);
-                    for (int p = 0; p < 4; p++)
-                        for (int h = 0; h < 2; h++) bf[p][l][h] = load32(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h));
-                    for (int mt = 0; mt < PK_MTILES; mt++) {
-                        u32 w[2];
+                    for (int nt = 0; nt < NT; nt++) {
+                        const u64 bcol = plane_offset(0, col0 + 8 * nt + g, 0, K, cols);
+                        for (int p = 0; p < 4; p++)
+                            for (int h = 0; h < 2; h++)
+                                bf[nt][p][l][h] = load32(bcol + p * plane_stride + 32 * ks + frag_k(t, h));
+                    }
+                    for (int mt = 0; mt < GEMM_MTILES; mt++) {
+                        const typename P::Word *row[2];
+                        bool ok[2];
                         for (int hr = 0; hr < 2; hr++) {
-                            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
-                            w[hr] = r < batch ? r_bits[r * words + ks] : 0u;
+                            const u64 r = row0 + 16 * mt + acc_row(g, 2 * hr);
+                            ok[hr] = r < rows;
+                            row[hr] = op.row(ok[hr] ? r : 0);
                         }
-                        af[mt][l][0] = pk_a_frag(w[0], t, 0);
-                        af[mt][l][1] = pk_a_frag(w[1], t, 0);
-                        af[mt][l][2] = pk_a_frag(w[0], t, 1);
-                        af[mt][l][3] = pk_a_frag(w[1], t, 1);
+                        op.a_frag(row, ok, ks, t, af[mt][l]);
                     }
                 }
-                for (int mt = 0; mt < PK_MTILES; mt++)
-                    for (int p = 0; p < 4; p++) mma_m16n8k32_u8(af[mt], bf[p], acc[p][mt]);
+                for (int mt = 0; mt < GEMM_MTILES; mt++)
+                    for (int nt = 0; nt < NT; nt++)
+                        for (int p = 0; p < 4; p++) mma_m16n8k32(P::SIGNED_A, af[mt], bf[nt][p], A(p, mt, nt));
             }
             for (int l = 0; l < 32; l++) {
                 const int g = l >> 2, t = l & 3;
-                for (int mt = 0; mt < PK_MTILES; mt++)
-                    for (int i = 0; i < 4; i++) {
-                        const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
-                        const u32 col = col0 + pk_acc_col(t, i);
-                        if (row >= batch) continue;
-                        const u32 v = pk_combine(acc[0][mt][l][i], acc[1][mt][l][i], acc[2][mt][l][i], acc[3][mt][l][i]);
-                        if (col < n) out_a[row * n + col] = (i32)v;
-                        else if (col == n) out_b[row] = (i32)(v + (u32)mus[row]);
-                        else if (col == n + 1) out_cv[row] = (float)acc[0][mt][l][i] * row_variance;
-                    }
+                for (int mt = 0; mt < GEMM_MTILES; mt++)
+                    for (int nt = 0; nt < NT; nt++)
+                        for (int i = 0; i < 4; i++) {
+                            const u64 row = row0 + 16 * mt + acc_row(g, i);
+                            if (row >= rows) continue;
+                            const u32 col = col0 + 8 * nt + acc_col(t, i);
+                            op.store(row, col, combine(A(0, mt, nt)[l][i], A(1, mt, nt)[l][i], A(2, mt, nt)[l][i],
+                                                       A(3, mt, nt)[l][i]), A(0, mt, nt)[l][i]);
+                        }
             }
         }
+}
+
+// Public-key encryption (pk_layout.cuh): nb_pk_prepare, then nb_pk_encrypt.
+void emul_pk_encrypt(const u32 *r_bits, const i32 *a, const i32 *b, size_t m, size_t n, const i32 *mus,
+                     float row_variance, i32 *out_a, i32 *out_b, float *out_cv, size_t batch)
+{
+    emul_plane_gemm(PkGemm{r_bits, (u32)m, (u32)n, mus, row_variance, out_a, out_b, out_cv}, PkSource{a, b, (u32)m, (u32)n},
+                    batch);
 }
 
 // Result packing (pack_layout.cuh): the digits of `count` mask words (out[2 c + j] = digit j of a[c]), the 16-bit mod
@@ -622,91 +639,11 @@ void emul_compact_extract(const uint16_t *data, int k, u32 p, i32 *a, i32 *b)
     *b = (i32)pack_unround16(data[k * PACK_N + p]);
 }
 
-// Tree-based programmable bootstrapping (tree_layout.cuh).  emul_tree_keyswitch: tree_prepare_kernel's planes, then
-// tree_keyswitch_kernel's tile loop with a scalar model of mma.sync.m16n8k32.row.col.s32.s8.u8.s32 that places each
-// register byte by the PTX ISA's fragment layout (A bytes signed, B bytes unsigned).
-static void mma_m16n8k32_s8u8(const u32 a[32][4], const u32 b[32][2], i32 c[32][4])
-{
-    i32 A[16][32];
-    u32 B[32][8];
-    for (int l = 0; l < 32; l++) {
-        const int g = l >> 2, t = l & 3;
-        for (int j = 0; j < 16; j++) {
-            const int row = g + ((j < 4 || (j >= 8 && j < 12)) ? 0 : 8), k = 4 * t + (j & 3) + (j >= 8 ? 16 : 0);
-            A[row][k] = (int8_t)((a[l][j >> 2] >> (8 * (j & 3))) & 0xFF);
-        }
-        for (int j = 0; j < 8; j++) {
-            const int k = 4 * t + (j & 3) + (j >= 4 ? 16 : 0);
-            B[k][g] = (b[l][j >> 2] >> (8 * (j & 3))) & 0xFF;
-        }
-    }
-    i32 D[16][8] = {};
-    for (int r = 0; r < 16; r++) {
-        bool any = false;
-        for (int k = 0; k < 32; k++) any |= A[r][k] != 0;
-        if (!any) continue;
-        for (int c2 = 0; c2 < 8; c2++) {
-            i32 s = 0;
-            for (int k = 0; k < 32; k++) s += A[r][k] * (i32)B[k][c2];
-            D[r][c2] = s;
-        }
-    }
-    for (int l = 0; l < 32; l++) {
-        const int g = l >> 2, t = l & 3;
-        for (int i = 0; i < 4; i++) c[l][i] += D[g + (i >= 2 ? 8 : 0)][2 * t + (i & 1)];
-    }
-}
-
+// Tree-based programmable bootstrapping (tree_layout.cuh).  emul_tree_keyswitch: nb_tree_prepare, then
+// nb_tree_keyswitch.
 void emul_tree_keyswitch(const i32 *a, const i32 *masks, const i32 *body, size_t n, int k, i32 *out, size_t rows)
 {
-    const u32 kpad = tree_k_padded((u32)n), cols = (u32)(k + 1) * PACK_N, ksteps = kpad >> 5;
-    std::vector<uint8_t> planes((size_t)4 * kpad * cols);
-    for (u32 col = 0; col < cols; col++)
-        for (u32 kk = 0; kk < kpad; kk++) {
-            const u32 w = tree_key_word(masks, body, (u32)n, (u32)k, kk, col);
-            for (int p = 0; p < 4; p++) planes[tree_plane_offset(p, col, kk, kpad, cols)] = (uint8_t)(w >> (8 * p));
-        }
-    auto load32 = [&](u64 off) { u32 v; memcpy(&v, planes.data() + off, 4); return v; };
-    const u64 plane_stride = tree_plane_offset(1, 0, 0, kpad, cols);
-    std::vector<i32> acc((size_t)4 * TREE_MTILES * 32 * 4);
-    auto A = [&](int p, int mt) { return reinterpret_cast<i32 (*)[4]>(&acc[((size_t)p * TREE_MTILES + mt) * 128]); };
-    for (u64 row0 = 0; row0 < rows; row0 += 16 * TREE_MTILES)      // one warp
-        for (u32 col0 = 0; col0 < cols; col0 += 8) {                 // one n8 tile
-            std::fill(acc.begin(), acc.end(), 0);
-            for (u32 ks = 0; ks < ksteps; ks++) {
-                u32 bf[4][32][2], af[TREE_MTILES][32][4];
-                for (int l = 0; l < 32; l++) {
-                    const int g = l >> 2, t = l & 3;
-                    const u64 bcol = tree_plane_offset(0, col0 + g, 0, kpad, cols);
-                    for (int p = 0; p < 4; p++)
-                        for (int h = 0; h < 2; h++) bf[p][l][h] = load32(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h));
-                    const u32 i0 = 16 * ks + 4 * t;
-                    for (int mt = 0; mt < TREE_MTILES; mt++) {
-                        i32 w[2][4];
-                        for (int hr = 0; hr < 2; hr++) {
-                            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
-                            for (int q = 0; q < 4; q++) w[hr][q] = (r < rows && i0 + q < n) ? a[r * n + i0 + q] : 0;
-                        }
-                        af[mt][l][0] = tree_a_frag(w[0][0], w[0][1]);
-                        af[mt][l][1] = tree_a_frag(w[1][0], w[1][1]);
-                        af[mt][l][2] = tree_a_frag(w[0][2], w[0][3]);
-                        af[mt][l][3] = tree_a_frag(w[1][2], w[1][3]);
-                    }
-                }
-                for (int mt = 0; mt < TREE_MTILES; mt++)
-                    for (int p = 0; p < 4; p++) mma_m16n8k32_s8u8(af[mt], bf[p], A(p, mt));
-            }
-            for (int l = 0; l < 32; l++) {
-                const int g = l >> 2, t = l & 3;
-                for (int mt = 0; mt < TREE_MTILES; mt++)
-                    for (int i = 0; i < 4; i++) {
-                        const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
-                        if (row >= rows) continue;
-                        const u32 col = col0 + pk_acc_col(t, i);
-                        out[row * cols + col] = (i32)pk_combine(A(0, mt)[l][i], A(1, mt)[l][i], A(2, mt)[l][i], A(3, mt)[l][i]);
-                    }
-            }
-        }
+    emul_plane_gemm(TreeGemm{a, (u32)n, (u32)(k + 1) * PACK_N, out}, TreeSource{masks, body, (u32)n, (u32)k}, rows);
 }
 
 // emul_tree_assemble: tree_assemble_kernel's arithmetic, one (test vector, polynomial) after the other, with a serial

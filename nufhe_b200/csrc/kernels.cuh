@@ -1706,97 +1706,114 @@ __global__ void __launch_bounds__(SEEDED_THREADS) seeded_uniform_kernel(i32 *__r
     }
 }
 
-// ---- public-key encryption (DESIGN.md section 11; index arithmetic in pk_layout.cuh).
-// nb_pk_prepare: the 4 byte planes of W = [A | b | 1] (m x n), one thread per (column, 4 consecutive k): it reads W
-// once and writes one 32-bit word to each plane.
-__global__ void pk_prepare_kernel(const i32 *__restrict__ a, const i32 *__restrict__ b, u32 m, u32 n,
-                                  uint8_t *__restrict__ planes)
+// ---- the byte-plane GEMM of public-key encryption (DESIGN.md section 11) and the tree key switch (section 13); layout
+// and index arithmetic in plane_gemm.cuh, the operands in pk_layout.cuh (PkSource, PkGemm) and tree_layout.cuh
+// (TreeSource, TreeGemm).  Both kernels take the fields of their source or policy as separate parameters, typed by the
+// caller with __restrict__ on the pointers: as one struct parameter they make ptxas spill in the encryption GEMM, and
+// without __restrict__ its loads of mus leave the read-only path.
+// nb_pk_prepare, nb_tree_prepare: the 4 byte planes of W (K x cols), one thread per (column, 4 consecutive k): it reads
+// 4 words of W and writes one 32-bit word to each plane.
+template <class Src, class... Fields>
+__global__ void plane_prepare_kernel(uint8_t *__restrict__ planes, Fields... fields)
 {
-    const u32 npad = pk_cols_padded(n), quads = m >> 2;
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < (u64)npad * quads; i += (u64)gridDim.x * blockDim.x) {
+    const Src src{fields...};
+    const u32 K = src.K(), cols = src.cols(), quads = K >> 2;
+    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < (u64)cols * quads; i += (u64)gridDim.x * blockDim.x) {
         const u32 col = (u32)(i / quads), k = (u32)(i % quads) * 4;
         u32 w[4];
 #pragma unroll
-        for (int j = 0; j < 4; j++) w[j] = pk_source_word(a, b, n, k + j, col);
+        for (int j = 0; j < 4; j++) w[j] = src(k + j, col);
 #pragma unroll
         for (int p = 0; p < 4; p++) {
             u32 v = 0;
 #pragma unroll
             for (int j = 0; j < 4; j++) v |= ((w[j] >> (8 * p)) & 0xFFu) << (8 * j);
-            *(u32 *)(planes + pk_plane_offset(p, col, k, m, npad)) = v;
+            *(u32 *)(planes + plane_offset(p, col, k, K, cols)) = v;
         }
     }
 }
 
-__device__ __forceinline__ void pk_mma(i32 *c, const u32 *a, const u32 *b)
+template <bool SIGNED_A> NB_D void mma_m16n8k32(i32 *c, const u32 *a, const u32 *b)
 {
-    asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    if constexpr (SIGNED_A)
+        asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    else
+        asm("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// nb_pk_encrypt: one GEMM R (batch x m, packed bits) x W (m x npad, 4 byte planes).  CTA = PK_WARPS warps on the
-// same 8 columns (blockIdx.y), each warp PK_MTILES m16 tiles of rows.  Per k-step of 32 a lane loads the R word of its
-// 2 * PK_MTILES rows and 2 words of each plane, and issues the 4 planes' MMAs with the same A fragment, so the four
-// sums of one output word sit in one thread.  The planes (33 MB for the default key) stay in L2 across CTAs.
-__global__ void __launch_bounds__(PK_WARPS * 32) pk_encrypt_kernel(
-    const u32 *__restrict__ r_bits, const uint8_t *__restrict__ planes, u32 m, u32 n, const i32 *__restrict__ mus,
-    float row_variance, i32 *__restrict__ out_a, i32 *__restrict__ out_b, float *__restrict__ out_cv, u64 batch)
+// nb_pk_encrypt, nb_tree_keyswitch: OUT (rows x cols) = A (rows x K) x W (K x cols, 4 byte planes) for the operand
+// policy P.  CTA = GEMM_WARPS warps on the same P::NTILES n8 column tiles (blockIdx.y), each warp GEMM_MTILES m16 tiles
+// of rows.  Per k-step of 32 a lane loads 2 words of each plane and column tile, forms the A fragment of each of its
+// row tiles in registers (P::a_frag), and issues every plane's and column tile's MMA with that fragment, so the four
+// plane sums of one output word sit in one thread.  The planes stay in L2 across CTAs.
+template <class P, class... Fields>
+__global__ void __launch_bounds__(GEMM_WARPS * 32) plane_gemm_kernel(const uint8_t *__restrict__ planes, u64 rows,
+                                                                     Fields... fields)
 {
+    const P op{fields...};
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const u64 row0 = ((u64)blockIdx.x * PK_WARPS + (threadIdx.x >> 5)) * (16 * PK_MTILES);
-    if (row0 >= batch) return;
-    const u32 npad = pk_cols_padded(n), words = m >> 5, col0 = blockIdx.y * 8;
-    const uint8_t *bcol = planes + pk_plane_offset(0, col0 + g, 0, m, npad);
-    const u64 plane_stride = pk_plane_offset(1, 0, 0, m, npad);
-    const u32 *rrow[PK_MTILES][2];
-    bool rok[PK_MTILES][2];
+    const u64 row0 = ((u64)blockIdx.x * GEMM_WARPS + (threadIdx.x >> 5)) * (16 * GEMM_MTILES);
+    if (row0 >= rows) return;
+    const u32 K = op.K(), cols = op.cols(), ksteps = K >> 5, col0 = blockIdx.y * (8 * P::NTILES);
+    const uint8_t *bcol = planes + plane_offset(0, col0 + g, 0, K, cols);
+    const u64 plane_stride = plane_offset(1, 0, 0, K, cols);
+    const typename P::Word *arow[GEMM_MTILES][2];
+    bool rok[GEMM_MTILES][2];
 #pragma unroll
-    for (int mt = 0; mt < PK_MTILES; mt++)
+    for (int mt = 0; mt < GEMM_MTILES; mt++)
 #pragma unroll
         for (int hr = 0; hr < 2; hr++) {
-            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
-            rok[mt][hr] = r < batch;
-            rrow[mt][hr] = r_bits + (rok[mt][hr] ? r : 0) * words;
+            const u64 r = row0 + 16 * mt + acc_row(g, 2 * hr);
+            rok[mt][hr] = r < rows;
+            arow[mt][hr] = op.row(rok[mt][hr] ? r : 0);
         }
-    i32 acc[4][PK_MTILES][4];
+    i32 acc[4][GEMM_MTILES][P::NTILES][4];
 #pragma unroll
     for (int p = 0; p < 4; p++)
 #pragma unroll
-        for (int mt = 0; mt < PK_MTILES; mt++)
+        for (int mt = 0; mt < GEMM_MTILES; mt++)
 #pragma unroll
-            for (int i = 0; i < 4; i++) acc[p][mt][i] = 0;
+            for (int nt = 0; nt < P::NTILES; nt++)
+#pragma unroll
+                for (int i = 0; i < 4; i++) acc[p][mt][nt][i] = 0;
 
-#pragma unroll 2
-    for (u32 ks = 0; ks < words; ks++) {
-        u32 bf[4][2];
+#pragma unroll P::UNROLL
+    for (u32 ks = 0; ks < ksteps; ks++) {
+        u32 bf[P::NTILES][4][2];
 #pragma unroll
-        for (int p = 0; p < 4; p++)
+        for (int nt = 0; nt < P::NTILES; nt++)
 #pragma unroll
-            for (int h = 0; h < 2; h++)
-                bf[p][h] = __ldg((const u32 *)(bcol + p * plane_stride + 32 * ks + pk_frag_k(t, h)));
+            for (int p = 0; p < 4; p++)
 #pragma unroll
-        for (int mt = 0; mt < PK_MTILES; mt++) {
-            const u32 w0 = rok[mt][0] ? __ldg(rrow[mt][0] + ks) : 0u;     // row g of the tile
-            const u32 w1 = rok[mt][1] ? __ldg(rrow[mt][1] + ks) : 0u;     // row g + 8
-            const u32 af[4] = {pk_a_frag(w0, t, 0), pk_a_frag(w1, t, 0), pk_a_frag(w0, t, 1), pk_a_frag(w1, t, 1)};
+                for (int h = 0; h < 2; h++)
+                    bf[nt][p][h] = __ldg((const u32 *)(bcol + (u64)8 * nt * K + p * plane_stride + 32 * ks + frag_k(t, h)));
 #pragma unroll
-            for (int p = 0; p < 4; p++) pk_mma(acc[p][mt], af, bf[p]);
+        for (int mt = 0; mt < GEMM_MTILES; mt++) {
+            u32 af[4];
+            op.a_frag(arow[mt], rok[mt], ks, t, af);
+#pragma unroll
+            for (int nt = 0; nt < P::NTILES; nt++)
+#pragma unroll
+                for (int p = 0; p < 4; p++) mma_m16n8k32<P::SIGNED_A>(acc[p][mt][nt], af, bf[nt][p]);
         }
     }
 
 #pragma unroll
-    for (int mt = 0; mt < PK_MTILES; mt++)
+    for (int mt = 0; mt < GEMM_MTILES; mt++)
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
-            const u32 col = col0 + pk_acc_col(t, i);
-            if (row >= batch) continue;
-            const u32 v = pk_combine(acc[0][mt][i], acc[1][mt][i], acc[2][mt][i], acc[3][mt][i]);
-            if (col < n) out_a[row * n + col] = (i32)v;
-            else if (col == n) out_b[row] = (i32)(v + (u32)mus[row]);
-            else if (col == n + 1) out_cv[row] = (float)acc[0][mt][i] * row_variance;   // the popcount of R's row
-        }
+        for (int nt = 0; nt < P::NTILES; nt++)
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const u64 row = row0 + 16 * mt + acc_row(g, i);
+                const u32 col = col0 + 8 * nt + acc_col(t, i);
+                if (row >= rows) continue;
+                op.store(row, col, combine(acc[0][mt][nt][i], acc[1][mt][nt][i], acc[2][mt][nt][i], acc[3][mt][nt][i]),
+                         acc[0][mt][nt][i]);
+            }
 }
 
 // ---- result packing (DESIGN.md section 12; slot mapping, digits and rounding in pack_layout.cuh).
@@ -1905,108 +1922,7 @@ __global__ void pack_finish_kernel(const i32 *__restrict__ c, const i32 *__restr
     }
 }
 
-// ---- tree-based programmable bootstrapping (DESIGN.md section 13; layout and index arithmetic in tree_layout.cuh).
-// nb_tree_prepare: the 4 byte planes of the tree key T (n t rows padded to kpad, (k+1) N columns), one thread per
-// (column, 4 consecutive rows): it reads 4 key words and writes one 32-bit word to each plane.
-__global__ void tree_prepare_kernel(const i32 *__restrict__ masks, const i32 *__restrict__ body, u32 n, u32 k,
-                                    uint8_t *__restrict__ planes)
-{
-    const u32 kpad = tree_k_padded(n), cols = (k + 1) * PACK_N, quads = kpad >> 2;
-    for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < (u64)cols * quads; i += (u64)gridDim.x * blockDim.x) {
-        const u32 col = (u32)(i / quads), kk = (u32)(i % quads) * 4;
-        u32 w[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) w[j] = tree_key_word(masks, body, n, k, kk + j, col);
-#pragma unroll
-        for (int p = 0; p < 4; p++) {
-            u32 v = 0;
-#pragma unroll
-            for (int j = 0; j < 4; j++) v |= ((w[j] >> (8 * p)) & 0xFFu) << (8 * j);
-            *(u32 *)(planes + tree_plane_offset(p, col, kk, kpad, cols)) = v;
-        }
-    }
-}
-
-__device__ __forceinline__ void tree_mma(i32 *c, const u32 *a, const u32 *b)
-{
-    asm("mma.sync.aligned.m16n8k32.row.col.s32.s8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-
-// nb_tree_keyswitch: V (rows x cols) = D (rows x kpad, signed digits of the masks) x T (4 byte planes), the pk_encrypt
-// tiling with TREE_NTILES n8 tiles per CTA: per k-step of 32 a lane reads 4 mask words of each of its 2 * TREE_MTILES
-// rows, forms their digits in registers (tree_a_frag) and issues every plane and column tile with the same A fragment,
-// so the four plane sums of one output word sit in one thread.  Every plane sum is at most kpad * 128 * 255 < 2^31.
-__global__ void __launch_bounds__(TREE_WARPS * 32) tree_keyswitch_kernel(
-    const i32 *__restrict__ a, const uint8_t *__restrict__ planes, u32 n, u32 cols, i32 *__restrict__ out, u64 rows)
-{
-    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const u64 row0 = ((u64)blockIdx.x * TREE_WARPS + (threadIdx.x >> 5)) * (16 * TREE_MTILES);
-    if (row0 >= rows) return;
-    const u32 kpad = tree_k_padded(n), ksteps = kpad >> 5, col0 = blockIdx.y * (8 * TREE_NTILES);
-    const u64 plane_stride = tree_plane_offset(1, 0, 0, kpad, cols);
-    const uint8_t *bcol = planes + tree_plane_offset(0, col0 + g, 0, kpad, cols);
-    const i32 *arow[TREE_MTILES][2];
-    bool rok[TREE_MTILES][2];
-#pragma unroll
-    for (int mt = 0; mt < TREE_MTILES; mt++)
-#pragma unroll
-        for (int hr = 0; hr < 2; hr++) {
-            const u64 r = row0 + 16 * mt + pk_acc_row(g, 2 * hr);
-            rok[mt][hr] = r < rows;
-            arow[mt][hr] = a + (rok[mt][hr] ? r : 0) * n;
-        }
-    i32 acc[4][TREE_MTILES][TREE_NTILES][4];
-#pragma unroll
-    for (int p = 0; p < 4; p++)
-#pragma unroll
-        for (int mt = 0; mt < TREE_MTILES; mt++)
-#pragma unroll
-            for (int nt = 0; nt < TREE_NTILES; nt++)
-#pragma unroll
-                for (int i = 0; i < 4; i++) acc[p][mt][nt][i] = 0;
-
-    for (u32 ks = 0; ks < ksteps; ks++) {
-        u32 bf[TREE_NTILES][4][2];
-#pragma unroll
-        for (int nt = 0; nt < TREE_NTILES; nt++)
-#pragma unroll
-            for (int p = 0; p < 4; p++)
-#pragma unroll
-                for (int h = 0; h < 2; h++)
-                    bf[nt][p][h] = __ldg((const u32 *)(bcol + (u64)8 * nt * kpad + p * plane_stride + 32 * ks + pk_frag_k(t, h)));
-        const u32 i0 = 16 * ks + 4 * t;      // mask words i0, i0 + 1 feed half 0, i0 + 2, i0 + 3 half 1
-#pragma unroll
-        for (int mt = 0; mt < TREE_MTILES; mt++) {
-            i32 w[2][4];
-#pragma unroll
-            for (int hr = 0; hr < 2; hr++)
-#pragma unroll
-                for (int q = 0; q < 4; q++) w[hr][q] = (rok[mt][hr] && i0 + q < n) ? __ldg(arow[mt][hr] + i0 + q) : 0;
-            const u32 af[4] = {tree_a_frag(w[0][0], w[0][1]), tree_a_frag(w[1][0], w[1][1]),
-                               tree_a_frag(w[0][2], w[0][3]), tree_a_frag(w[1][2], w[1][3])};
-#pragma unroll
-            for (int nt = 0; nt < TREE_NTILES; nt++)
-#pragma unroll
-                for (int p = 0; p < 4; p++) tree_mma(acc[p][mt][nt], af, bf[nt][p]);
-        }
-    }
-
-#pragma unroll
-    for (int mt = 0; mt < TREE_MTILES; mt++)
-#pragma unroll
-        for (int nt = 0; nt < TREE_NTILES; nt++)
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const u64 row = row0 + 16 * mt + pk_acc_row(g, i);
-                if (row >= rows) continue;
-                const u32 col = col0 + 8 * nt + pk_acc_col(t, i);
-                out[row * cols + col] = (i32)pk_combine(acc[0][mt][nt][i], acc[1][mt][nt][i], acc[2][mt][nt][i],
-                                                        acc[3][mt][nt][i]);
-            }
-}
-
+// ---- tree-based programmable bootstrapping (DESIGN.md section 13; index arithmetic in tree_layout.cuh).
 // nb_tree_assemble: one CTA per (test vector, polynomial u).  Z_u = sum_m X^(o_m) G_m,u in shared memory, its
 // exclusive prefix sums (4 coefficients per thread, a warp scan, then the warp totals), then every coefficient of
 // Q_P Z_u as the difference of two prefix sums.  All sums wrap mod 2^32, which is exact.

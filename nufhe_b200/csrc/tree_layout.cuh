@@ -1,26 +1,19 @@
 // tree_layout.cuh -- the index and sign arithmetic of tree-based programmable bootstrapping (DESIGN.md section 13),
 // kept apart from the kernels so that g++ compiles it into the host emulator (host_emul.cpp) and the CPU suite checks
 // it:
-//   * the LWE -> GLWE key switch V (R, k+1, N) = D (R, n t) x T (n t, (k+1) N) mod 2^32 as an exact byte-plane GEMM:
-//     the plane layout nb_tree_prepare writes, the signed 8-bit digit fragments a lane forms from two mask words, and
-//     the row / column of each accumulator (the m16n8k32 fragment layout is the one of pk_layout.cuh);
+//   * the LWE -> GLWE key switch V (R, k+1, N) = D (R, n t) x T (n t, (k+1) N) mod 2^32 as the byte-plane GEMM of
+//     plane_gemm.cuh: the key words nb_tree_prepare splits into planes, and the signed 8-bit digit fragments a lane
+//     forms from two mask words;
 //   * the test-vector assembly tv_u = sum_m X^(o_m) Q_P G_m,u (negacyclic) with Q_P = 1 + X + ... + X^(box - 1):
 //     Z_u = sum_m X^(o_m) G_m,u first, then the box sum of Z_u from its prefix sums.
 #pragma once
 #include "pack_layout.cuh"
-#include "pk_layout.cuh"
+#include "plane_gemm.cuh"
 
 namespace nb {
 
-constexpr int TREE_WARPS = 4;     // warps per CTA, each its own 64-row slice, all on the same TREE_NTILES * 8 columns
-constexpr int TREE_MTILES = 4;    // m16 tiles per warp
-constexpr int TREE_NTILES = 2;    // n8 tiles per CTA
-
 // digit rows n t padded to whole k-steps of 32 (the padding rows of the key planes are zero)
 NB_HD u32 tree_k_padded(u32 n) { return (n * PACK_LEVELS + 31u) & ~31u; }
-
-// Plane p is column-major kpad x cols (the `.col` B operand): byte (kk, col) at ((p * cols + col) * kpad + kk).
-NB_HD u64 tree_plane_offset(u32 p, u32 col, u32 kk, u32 kpad, u32 cols) { return ((u64)p * cols + col) * kpad + kk; }
 
 // T[kk][col], kk = i t + j, col = u N + x: mask u < k of key row kk (masks (n, t, k, N)) or its body (bodies (n, t, N))
 NB_HD u32 tree_key_word(const i32 *masks, const i32 *body, u32 n, u32 k, u32 kk, u32 col)
@@ -30,7 +23,7 @@ NB_HD u32 tree_key_word(const i32 *masks, const i32 *body, u32 n, u32 k, u32 kk,
     return u < k ? (u32)masks[((u64)kk * k + u) * PACK_N + x] : (u32)body[(u64)kk * PACK_N + x];
 }
 
-// The A fragment register of K values kb .. kb + 3 (kb = 32 ks + pk_frag_k(t, h), even): the digits d_0, d_1 of mask
+// The A fragment register of K values kb .. kb + 3 (kb = 32 ks + frag_k(t, h), even): the digits d_0, d_1 of mask
 // words kb / 2 and kb / 2 + 1 as four signed bytes, lowest first.  Byte 3 - j of pack_digit_word is d_j + 128, so the
 // signed byte is that byte with its top bit flipped.
 NB_HD u32 tree_a_frag(i32 a0, i32 a1)
@@ -39,6 +32,47 @@ NB_HD u32 tree_a_frag(i32 a0, i32 a1)
     const u32 v = (w0 >> 24) | (((w0 >> 16) & 0xFFu) << 8) | ((w1 >> 24) << 16) | (((w1 >> 16) & 0xFFu) << 24);
     return v ^ 0x80808080u;
 }
+
+// The source of nb_tree_prepare's planes: K = tree_k_padded(n) rows, (k + 1) N columns.
+struct TreeSource {
+    const i32 *masks, *body;
+    u32 n, k;
+    NB_HD u32 K() const { return tree_k_padded(n); }
+    NB_HD u32 cols() const { return (k + 1) * PACK_N; }
+    NB_HD u32 operator()(u32 kk, u32 col) const { return tree_key_word(masks, body, n, k, kk, col); }
+};
+
+// The operand policy of nb_tree_keyswitch: A rows are LWE masks of n words, each giving t = 2 signed digits.  Every
+// plane sum is at most K * 128 * 255.
+struct TreeGemm {
+    static constexpr int NTILES = 2;          // n8 column tiles per CTA
+    static constexpr bool SIGNED_A = true;    // signed digits: mma .s8.u8
+    static constexpr int UNROLL = 1;          // unroll of the k-step loop
+    typedef i32 Word;
+    const i32 *a;
+    u32 n, ncols;
+    i32 *out;
+
+    NB_HD u32 K() const { return tree_k_padded(n); }
+    NB_HD u32 cols() const { return ncols; }
+    NB_HD const i32 *row(u64 r) const { return a + r * n; }
+    // The A registers of k-step ks for rows g (row[0]) and g + 8 (row[1]) of a tile: mask words i0, i0 + 1 feed half 0,
+    // i0 + 2, i0 + 3 half 1.  A row past the batch, and a word past n, is zero.
+    NB_HD void a_frag(const i32 *const row[2], const bool ok[2], u32 ks, int t, u32 af[4]) const
+    {
+        const u32 i0 = 16 * ks + 4 * t;
+        i32 w[2][4];
+#pragma unroll
+        for (int hr = 0; hr < 2; hr++)
+#pragma unroll
+            for (int q = 0; q < 4; q++) w[hr][q] = (ok[hr] && i0 + q < n) ? ldg(row[hr] + i0 + q) : 0;
+        af[0] = tree_a_frag(w[0][0], w[0][1]);
+        af[1] = tree_a_frag(w[1][0], w[1][1]);
+        af[2] = tree_a_frag(w[0][2], w[0][3]);
+        af[3] = tree_a_frag(w[1][2], w[1][3]);
+    }
+    NB_HD void store(u64 row, u32 col, u32 v, i32) const { out[row * ncols + col] = (i32)v; }
+};
 
 // ---- assembly
 NB_HD int tree_box(int bits) { return PACK_N >> bits; }

@@ -1,5 +1,5 @@
-"""Public-key encryption on the CPU: the kernel's tile loop and index arithmetic (csrc/pk_layout.cuh, through the host
-emulator's scalar model of the m16n8k32 u8 MMA) against an independent NumPy restatement (pk_ref.py), and the Python
+"""Public-key encryption on the CPU: the kernel's tile loop and index arithmetic (csrc/plane_gemm.cuh, pk_layout.cuh,
+through the host emulator's scalar model of the m16n8k32 u8 MMA) against an independent NumPy restatement (pk_ref.py), and the Python
 layer (nufhe_b200/public_key.py) on an oracle-backed engine double: draw order, the phase error of every ciphertext,
 variances, decryption, serialization, a gate, and the noise bound of DESIGN.md section 11."""
 import ctypes

@@ -1,5 +1,5 @@
 """Tree-based programmable bootstrapping on the CPU: the key switch and assembly of csrc/tree_layout.cuh (through the
-host emulator's scalar models of tree_keyswitch_kernel and tree_assemble_kernel) against the NumPy restatement
+host emulator's scalar models of plane_gemm_kernel and tree_assemble_kernel) against the NumPy restatement
 (tree_ref.py), the tree key (draw order, row phases, pickles), the noise rule, and vm.lut_tree end to end on an
 oracle-backed engine double."""
 import ctypes
