@@ -148,6 +148,40 @@ int nb_ks_prepare(nb_ctx *ctx, const int32_t *ks_a, const int32_t *ks_b, uint8_t
                   int log2_base, int *registered);
 int nb_ks_forget(nb_ctx *ctx, const int32_t *ks_a);
 
+/* ---- multi-key calls (DESIGN.md section 17): one launch over ciphertexts of several cloud keys ("tenants").
+ * Each takes the arguments of the single-key call of the same name, with the key replaced by HOST arrays of one entry
+ * per tenant (`tenants` entries): the key pointers, and counts[t], the number of consecutive ciphertexts of the batch
+ * that belong to tenant t, in tenant order; the counts add up to `batch` (for extract2 they apply to each job, so job
+ * A is [0, batch) and job B [batch, 2 batch), both split by the same counts; for the key switch of the 2^L samples of
+ * nb_mk_bootstrap_lut_extract pass counts * 2^L).  A count may be 0.  Every output row is bit-identical to the
+ * single-key call on that tenant's segment with that tenant's key.  The bootstrap runs in the 2-ciphertext FP64 shape
+ * at every batch size; every key must lie inside one engine key prepared by nb_bk_prepare on this context with FP64
+ * spectra.  The key switch runs each tenant whose segment would take the tensor-core GEMM in nb_keyswitch exactly as
+ * there, and all the others in one launch of the gather kernel whose tiles never cross a tenant boundary; it takes
+ * in = 1024, n = 500, t = 8, base 4 only.  The library uploads the per-ciphertext tenant table and the tile table into
+ * context scratch; these calls are not for graph capture.
+ * NB_EINVAL for a NULL argument, counts that do not add up to `batch`, or a key that is not inside a prepared engine
+ * key of this context; NB_EUNSUPPORTED for a multi-bit key, a context with the FP64 step disabled (NUFHE_B200_FFT=0),
+ * an LWE dimension out of range or other key-switch sizes. */
+int nb_mk_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                            const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
+                            const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants, size_t n,
+                            int32_t *out_a, int32_t *out_b, size_t batch);
+int nb_mk_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
+                             const int32_t *a2_b, int32_t a_c, int32_t a_s1, int32_t a_s2, const int32_t *b1_a,
+                             const int32_t *b1_b, const int32_t *b2_a, const int32_t *b2_b, int32_t b_c, int32_t b_s1,
+                             int32_t b_s2, int32_t mu, const uint64_t *const *bk_int_host, const size_t *counts_host,
+                             size_t tenants, size_t n, int32_t *out_a, int32_t *out_b, size_t batch);
+int nb_mk_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                                const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv,
+                                size_t tv_stride, int log2_outputs, const uint64_t *const *bk_int_host,
+                                const size_t *counts_host, size_t tenants, size_t n, int32_t *out_a, int32_t *out_b,
+                                size_t batch);
+int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, const int32_t *src2_a,
+                    const int32_t *src2_b, int32_t c, const int32_t *const *ks_a_host, const int32_t *const *ks_b_host,
+                    const float *const *ks_cv_host, const size_t *counts_host, size_t tenants, size_t in_size, size_t n,
+                    int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv, size_t batch);
+
 /* ---- LweLinear / LweNoiselessTrivial (lwe.py:346-422): res = (0, c) + s1 * x1 + s2 * x2 ------- */
 int nb_lwe_affine(nb_ctx *ctx, int32_t *res_a, int32_t *res_b, const int32_t *x1_a, const int32_t *x1_b,
                   const int32_t *x2_a, const int32_t *x2_b, int32_t c, int32_t s1, int32_t s2, size_t batch,

@@ -77,6 +77,7 @@ from .index_lookup import (
     encrypt_index,
     lookup,
     )
+from .multikey import MultiKeyVirtualMachine
 from .performance import PerformanceParameters
 from .random_numbers import DeterministicRNG, SecureRNG
 from .computation_cache import clear_computation_cache

@@ -44,6 +44,13 @@ SIGNATURES = {
     'nb_bootstrap_extract2': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32,
                               _vp, _sz, _vp, _vp, _sz],
     'nb_keyswitch': [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp, _vp, _vp, _sz],
+    'nb_mk_bootstrap_extract': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _sz, _sz, _vp, _vp, _sz],
+    'nb_mk_bootstrap_extract2': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32,
+                                 _vp, _vp, _sz, _sz, _vp, _vp, _sz],
+    'nb_mk_bootstrap_lut_extract': [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _int, _vp, _vp, _sz, _sz, _vp,
+                                    _vp, _sz],
+    'nb_mk_keyswitch': [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _sz, _sz, _int, _int, _vp, _vp, _vp,
+                        _sz],
     'nb_ks_prepared_bytes': [],
     'nb_ks_prepare': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp],
     'nb_ks_forget': [_vp, _vp],

@@ -180,6 +180,15 @@ class Context:
     def make_virtual_machine(self, cloud_key: NuFHECloudKey, perf_params: PerformanceParameters = None):
         return VirtualMachine(self.thread, cloud_key, perf_params=perf_params)
 
+    def make_multi_key_machine(self, cloud_keys, perf_params: PerformanceParameters = None):
+        """A MultiKeyVirtualMachine (nufhe_b200/multikey.py) for the list of cloud keys `cloud_keys`, one per tenant:
+        its gates and LUTs take one operand list aligned with it and bootstrap every tenant's ciphertexts in one launch,
+        bit-identical to each tenant's own VirtualMachine.  TypeError for anything but NuFHECloudKey objects, ValueError
+        for keys of different parameters, multi-bit keys, single_kernel_bootstrap=False and keys the fused FP64 step
+        cannot run."""
+        from .multikey import MultiKeyVirtualMachine
+        return MultiKeyVirtualMachine(self.thread, cloud_keys, perf_params=perf_params)
+
     def load_ciphertext(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
             return LweSampleArray.loads(file_or_bytestring, self.thread)

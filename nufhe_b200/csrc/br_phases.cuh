@@ -165,6 +165,7 @@ using BrDefault = BrCfg<BR2_CT, BR2_THREADS, NB_BR_CTAS, NB_BR_TWD_GLOBAL != 0>;
 using BrWide = BrCfg<1, 256>;
 using BrWide2 = BrCfg<1, 512, 1>;                 // lowest latency: one ciphertext per SM, 16 warps in step
 using BrFft = BrCfg<2, 256, 2, true, true>;      // throughput shape, FP64 step
+struct BrFftMk : BrFft {};                         // the same with one key per ciphertext (multi-key launches)
 constexpr int BR2_POLYS = BrDefault::POLYS;
 // Engine bootstrap-key row: 8 planes [(mi*2+j)*2+mo][row*64 + stored column] of plain field values plus
 // 2 correction planes K[mo] = 512 * NTT(1,...,1) * sum_{mi,j} plane, because the forward transforms run

@@ -50,6 +50,8 @@ struct nb_ctx {
     size_t cv_words;
     int force_chunks;                    // developer knob: chunk count of every multi-wave launch (0 = automatic)
     int stagger_cycles;                  // start-up offset of the second CTA per SM in single-wave launches
+    void *d_mk;                          // multi-key calls: the uploaded tenant tables (nb_mk_*)
+    size_t mk_bytes;
     std::string err;
 };
 
@@ -132,6 +134,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     ctx->d_sched = nullptr; ctx->d_state = nullptr; ctx->sched_words = ctx->state_words = 0;
     ctx->d_cv_blocks = nullptr; ctx->cv_words = 0;
     ctx->d_index_tmp = nullptr; ctx->index_tmp_words = 0;
+    ctx->d_mk = nullptr; ctx->mk_bytes = 0;
     *out = ctx;   // returned even on failure so that nb_last_error() can be read; caller destroys it
     NB_ON_DEVICE(ctx);
     cudaDeviceProp prop;
@@ -178,6 +181,8 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
                      "cudaFuncSetAttribute(blind_rotate pair)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)KS_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch)"));
+    NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)KS_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch_grouped)"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(keyswitch_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)KM_SMEM_BYTES), "cudaFuncSetAttribute(keyswitch_mma)"));
     {
@@ -190,6 +195,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check_resident<BrWide2>(ctx));
     NB_TRY(check_resident<BrFft>(ctx));
     NB_TRY((check_resident<BrFft, true>(ctx)));
+    NB_TRY(check_resident<BrFftMk>(ctx));
     for (auto kernel : {index_lookup_kernel<false>, index_lookup_kernel<true>})
         NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<BrFft>()),
                      "cudaFuncSetAttribute(index_lookup)"));
@@ -251,6 +257,7 @@ void nb_ctx_destroy(nb_ctx *ctx)
     if (ctx->d_state) cudaFree(ctx->d_state);
     if (ctx->d_cv_blocks) cudaFree(ctx->d_cv_blocks);
     if (ctx->d_index_tmp) cudaFree(ctx->d_index_tmp);
+    if (ctx->d_mk) cudaFree(ctx->d_mk);
     delete ctx;
 }
 
@@ -653,6 +660,23 @@ int nb_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b,
     return launch_blind_rotate(ctx, p);
 }
 
+}  // extern "C"
+
+// The prepared planes of (ks_a, ks_b) when a fast-path key switch of `batch` ciphertexts runs as the tensor-core GEMM
+// (registered key, batch from ks_mma_min, rows aligned for its loads and stores), else null
+static const uint8_t *ks_gemm_planes(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src2_a, const int32_t *ks_a,
+                                     const int32_t *ks_b, const int32_t *res_a, size_t batch)
+{
+    const uint8_t *planes = nullptr;
+    if (batch >= ctx->ks_mma_min &&
+        (((uintptr_t)src1_a | (uintptr_t)(src2_a ? src2_a : src1_a)) & 15) == 0 && ((uintptr_t)res_a & 7) == 0)
+        for (const auto &k : ctx->ks_keys)
+            if (k.ks_a == ks_a && k.ks_b == ks_b) planes = k.planes;
+    return planes;
+}
+
+extern "C" {
+
 int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, const int32_t *src2_a,
                  const int32_t *src2_b, int32_t c, const int32_t *ks_a, const int32_t *ks_b, const float *ks_cv,
                  size_t in_size, size_t n, int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv,
@@ -672,11 +696,7 @@ int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, cons
     p.ks_a = ks_a; p.ks_b = ks_b; p.ks_cv = ks_cv; p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
     p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch;
     const bool fast = t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N;
-    const uint8_t *planes = nullptr;
-    if (fast && batch >= ctx->ks_mma_min &&
-        (((uintptr_t)src1_a | (uintptr_t)(src2_a ? src2_a : src1_a)) & 15) == 0 && ((uintptr_t)res_a & 7) == 0)
-        for (const auto &k : ctx->ks_keys)
-            if (k.ks_a == ks_a && k.ks_b == ks_b) planes = k.planes;
+    const uint8_t *planes = fast ? ks_gemm_planes(ctx, src1_a, src2_a, ks_a, ks_b, res_a, batch) : nullptr;
     if (planes) {
         // the GEMM: tiles of 256 ciphertexts x 32 output columns; K is split over blockIdx.z (partial sums meet in
         // integer atomics) while a launch would leave half of the SMs idle
@@ -1206,6 +1226,204 @@ int nb_compact_extract(nb_ctx *ctx, const uint16_t *data, int mask_size, int32_t
     const dim3 grid(PACK_N / CX_ROWS, (unsigned)groups, (unsigned)mask_size);
     compact_extract_kernel<<<grid, CX_THREADS, 0, ctx->stream>>>(data, (u32)mask_size, (u64)rows, out_a, out_b);
     return launch_check(ctx, "compact_extract_kernel");
+}
+
+}  // extern "C"
+
+// ---- multi-key calls (DESIGN.md section 17) --------------------------------------------------------------------
+
+// counts[0 .. tenants) must add up to `batch`
+static int mk_check_counts(nb_ctx *ctx, const char *what, const size_t *counts, size_t tenants, size_t batch)
+{
+    size_t sum = 0;
+    for (size_t t = 0; t < tenants; t++) sum += counts[t];
+    if (sum != batch)
+        return fail(ctx, NB_EINVAL, std::string(what) + ": the counts add up to " + std::to_string(sum) + ", not the batch " +
+                                        std::to_string(batch));
+    return NB_OK;
+}
+
+// copy `bytes` of host data into the context's multi-key scratch (stream-ordered after every earlier launch that reads it)
+static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
+{
+    NB_TRY(reserve_words(ctx, &ctx->d_mk, &ctx->mk_bytes, bytes, 1));
+    return check(ctx, cudaMemcpyAsync(ctx->d_mk, host, bytes, cudaMemcpyHostToDevice, ctx->stream), "cudaMemcpyAsync(multi-key tables)");
+}
+
+// The common part of the multi-key bootstraps: p carries everything but the keys, for a batch of jobs x sum(counts)
+// ciphertexts whose job j covers rows [j B, (j + 1) B), split into tenants by the same counts.  Every tenant's key must lie
+// inside an engine key with FP64 spectra prepared on this context, since the multi-key kernel runs the FP64 step.
+static int mk_blind_rotate(nb_ctx *ctx, const char *what, BlindRotateArgs &p, const uint64_t *const *bk,
+                           const size_t *counts, size_t tenants, size_t job_batch, int jobs)
+{
+    if (p.n <= 0 || p.n > LWE_N_MAX) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": LWE dimension out of range");
+    if (!ctx->fft) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": multi-key launches run the FP64 step, which NUFHE_B200_FFT=0 disables");
+    for (size_t t = 0; t < tenants; t++) {
+        const u64 *key = (const u64 *)bk[t];
+        if (!key) return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(t));
+        for (const auto &k : ctx->multibit_keys)
+            if (k.first <= key && key < k.second)
+                return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": tenant " + std::to_string(t) + " has a multi-bit key");
+        bool spectral = false;
+        for (const auto &k : ctx->spectral_keys) spectral |= k.first <= key && key + (size_t)p.n * BK_ROW_U64 <= k.second;
+        if (!spectral)
+            return fail(ctx, NB_EINVAL, std::string(what) + ": the key of tenant " + std::to_string(t) +
+                                            " is not inside an engine key with FP64 spectra prepared on this context");
+    }
+    if (p.batch == 0) return NB_OK;
+    // [tenant key pointers][tenant of each ciphertext]
+    std::vector<unsigned char> host(tenants * sizeof(const u64 *) + p.batch * sizeof(unsigned));
+    memcpy(host.data(), bk, tenants * sizeof(const u64 *));
+    unsigned *tenant_of = reinterpret_cast<unsigned *>(host.data() + tenants * sizeof(const u64 *));
+    for (int j = 0; j < jobs; j++) {
+        size_t c = (size_t)j * job_batch;
+        for (size_t t = 0; t < tenants; t++)
+            for (size_t i = 0; i < counts[t]; i++) tenant_of[c++] = (unsigned)t;
+    }
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_blind_rotate");
+    NB_TRY(mk_upload(ctx, host.data(), host.size()));
+    p.bk = nullptr;
+    p.mk_bk = reinterpret_cast<const u64 *const *>(ctx->d_mk);
+    p.mk_tenant = reinterpret_cast<const unsigned *>(reinterpret_cast<unsigned char *>(ctx->d_mk) + tenants * sizeof(const u64 *));
+    NB_TRY(launch_br_cfg<BrFftMk>(ctx, p));
+    return launch_check(ctx, "blind_rotate_kernel(multi-key)");
+}
+
+extern "C" {
+
+int nb_mk_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                            const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
+                            const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants, size_t n,
+                            int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    const char *what = "nb_mk_bootstrap_extract";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
+    if (batch && (!in1_a || !in1_b || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": in2_a/in2_b must come together");
+    BlindRotateArgs p{};
+    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
+    p.c = c; p.s1 = s1; p.s2 = s2; p.mu = mu;
+    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
+    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
+}
+
+int nb_mk_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
+                             const int32_t *a2_b, int32_t a_c, int32_t a_s1, int32_t a_s2, const int32_t *b1_a,
+                             const int32_t *b1_b, const int32_t *b2_a, const int32_t *b2_b, int32_t b_c, int32_t b_s1,
+                             int32_t b_s2, int32_t mu, const uint64_t *const *bk_int_host, const size_t *counts_host,
+                             size_t tenants, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    const char *what = "nb_mk_bootstrap_extract2";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
+    if (batch && (!a1_a || !a1_b || !b1_a || !b1_b || !out_a || !out_b))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if ((a2_a == nullptr) != (a2_b == nullptr) || (b2_a == nullptr) != (b2_b == nullptr))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": a/b parts must come together");
+    BlindRotateArgs p{};
+    p.in1_a = a1_a; p.in1_b = a1_b; p.in2_a = a2_a; p.in2_b = a2_b; p.c = a_c; p.s1 = a_s1; p.s2 = a_s2;
+    p.j2_in1_a = b1_a; p.j2_in1_b = b1_b; p.j2_in2_a = b2_a; p.j2_in2_b = b2_b; p.j2_c = b_c; p.j2_s1 = b_s1; p.j2_s2 = b_s2;
+    p.mu = mu; p.job_batch = batch;
+    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = 2 * batch;
+    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 2);
+}
+
+int nb_mk_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                                const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv,
+                                size_t tv_stride, int log2_outputs, const uint64_t *const *bk_int_host,
+                                const size_t *counts_host, size_t tenants, size_t n, int32_t *out_a, int32_t *out_b,
+                                size_t batch)
+{
+    const char *what = "nb_mk_bootstrap_lut_extract";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
+    if (batch && (!in1_a || !in1_b || !tv || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": in2_a/in2_b must come together");
+    if (tv_stride != 0 && tv_stride != (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tv_stride must be 0 or 1024");
+    if (log2_outputs < 0 || log2_outputs > 2) return fail(ctx, NB_EINVAL, std::string(what) + ": log2_outputs must be 0, 1 or 2");
+    BlindRotateArgs p{};
+    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
+    p.c = c; p.s1 = s1; p.s2 = s2;
+    p.tv = tv; p.tv_stride = tv_stride; p.log2_outputs = log2_outputs;
+    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
+    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
+}
+
+int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, const int32_t *src2_a,
+                    const int32_t *src2_b, int32_t c, const int32_t *const *ks_a_host, const int32_t *const *ks_b_host,
+                    const float *const *ks_cv_host, const size_t *counts_host, size_t tenants, size_t in_size, size_t n,
+                    int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv, size_t batch)
+{
+    const char *what = "nb_mk_keyswitch";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!ks_a_host || !ks_b_host || !ks_cv_host || !counts_host))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
+    if (batch && (!src1_a || !src1_b || !res_a || !res_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if ((src2_a == nullptr) != (src2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": src2_a/src2_b must come together");
+    for (size_t k = 0; k < tenants; k++)
+        if (!ks_a_host[k] || !ks_b_host[k] || !ks_cv_host[k])
+            return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(k));
+    if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N))
+        return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the grouped key switch is for in = 1024, n = 500, t = 8, base 4 only");
+    if (batch == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_keyswitch");
+    // tenants whose segment nb_keyswitch would run as the GEMM go there; the others become tiles of the gather kernel
+    std::vector<KsTile> tiles;
+    std::vector<std::pair<size_t, size_t>> gemm;      // (tenant, first row)
+    size_t row = 0;
+    for (size_t k = 0; k < tenants; row += counts_host[k], k++) {
+        const size_t cnt = counts_host[k];
+        if (cnt && ks_gemm_planes(ctx, src1_a + row * KS_IN, src2_a ? src2_a + row * KS_IN : nullptr, ks_a_host[k],
+                                  ks_b_host[k], res_a + row * KS_N, cnt)) {
+            gemm.emplace_back(k, row);
+            continue;
+        }
+        for (size_t q = 0; q < cnt; q += KS_TILE)
+            tiles.push_back({ks_a_host[k], ks_b_host[k], ks_cv_host[k], row + q, (int)std::min<size_t>(KS_TILE, cnt - q)});
+    }
+    if (!tiles.empty()) {
+        // the split rule of nb_keyswitch over the tile count; every output row is exact integer arithmetic and its
+        // variance the fixed-shape sum, so the split changes no bit
+        KeyswitchArgs p{};
+        p.src1_a = src1_a; p.src1_b = src1_b; p.src2_a = src2_a; p.src2_b = src2_b; p.c = c;
+        p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
+        p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch; p.tile = KS_TILE;
+        int splits = (int)std::min<size_t>(128, (size_t)ctx->sm_count / tiles.size());
+        if (splits < 1) splits = 1;
+        p.splits = splits;
+        if (splits > 1) {
+            // (the GEMM segments are written after this, by their own launches)
+            NB_TRY(check(ctx, cudaMemsetAsync(res_a, 0, batch * n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+            NB_TRY(check(ctx, cudaMemsetAsync(res_b, 0, batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+            if (res_cv) {
+                NB_TRY(reserve_words(ctx, (void **)&ctx->d_cv_blocks, &ctx->cv_words, batch * KS_CV_BLOCKS, sizeof(float)));
+                p.cv_blocks = ctx->d_cv_blocks;
+            }
+        }
+        NB_TRY(mk_upload(ctx, tiles.data(), tiles.size() * sizeof(KsTile)));
+        keyswitch_grouped_kernel<<<dim3((unsigned)tiles.size(), splits), KS_THREADS, KS_SMEM_BYTES, ctx->stream>>>(
+            p, reinterpret_cast<const KsTile *>(ctx->d_mk));
+        NB_TRY(launch_check(ctx, "keyswitch_grouped_kernel"));
+        if (p.cv_blocks) {
+            // over the whole batch: the rows of GEMM segments get their variances from ks_cv_kernel after this
+            ks_cv_finalize_kernel<<<(int)((batch + 127) / 128), 128, 0, ctx->stream>>>(res_cv, p.cv_blocks, batch);
+            NB_TRY(launch_check(ctx, "ks_cv_finalize_kernel"));
+        }
+    }
+    for (const auto &g : gemm) {
+        const size_t k = g.first, r = g.second;
+        NB_TRY(nb_keyswitch(ctx, src1_a + r * KS_IN, src1_b + r, src2_a ? src2_a + r * KS_IN : nullptr,
+                            src2_b ? src2_b + r : nullptr, c, ks_a_host[k], ks_b_host[k], ks_cv_host[k], in_size, n, t,
+                            log2_base, res_a + r * KS_N, res_b + r, res_cv ? res_cv + r : nullptr, counts_host[k]));
+    }
+    return NB_OK;
 }
 
 }  // extern "C"

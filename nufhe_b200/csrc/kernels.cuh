@@ -19,6 +19,7 @@
 // section 4 for the measurements behind each choice.
 #pragma once
 #include <cuda_runtime.h>
+#include <type_traits>
 #include "ntt_lane.cuh"
 #include "br_phases.cuh"
 #include "lut_index.cuh"
@@ -366,6 +367,10 @@ struct BlindRotateArgs {
     const i32 *tv;
     size_t tv_stride;       // 0: one test vector for the batch, NTT_N: one per ciphertext, 2 NTT_N: one GLWE per ciphertext
     int log2_outputs;
+    // multi-key launches (the BrFftMk instantiation of blind_rotate_kernel; bk unused): the engine key of tenant t starts at mk_bk[t], and
+    // ciphertext c of the batch belongs to tenant mk_tenant[c]
+    const u64 *const *mk_bk;
+    const unsigned *mk_tenant;
 };
 constexpr int BR_SCHED_HEADER = 32;      // the ticket counter has a 128-byte line of its own
 
@@ -611,11 +616,17 @@ template <bool MB> NB_D int br_chain_steps(const BlindRotateArgs &p)
 // LUT: the programmable bootstrap (BlindRotateArgs::tv); its own instantiation, so that the gate kernels keep their code.
 // MB: a multi-bit key (BrFft only): a chain is p.n / 2 groups of two key bits instead of p.n steps, p.bk holds 3 rows of
 // BK_FFT_U64 per group, and s.rot holds both rotation amounts of the group per ciphertext ([parity][CT][2]).
+// Cfg = BrFftMk: the multi-key instantiation -- ciphertexts under different keys (BlindRotateArgs::mk_bk).  Chains are
+// consecutive pairs of the batch as always, so the two slots of a CTA may belong to two tenants.  Only pass 3 of the
+// FP64 step reads the key, and fft_phase_mac serves slot tid & 1 from the pointer its thread passes (as
+// index_lookup_kernel does), so each thread passes the key of its own slot's tenant, looked up again for every work item.
 template <class Cfg, bool LUT = false, bool MB = false>
 __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_kernel(BlindRotateArgs p, const u64 *__restrict__ twd_fwd_g,
                                                                        const u64 *__restrict__ twd_inv_g)
 {
+    constexpr bool MK = std::is_same<Cfg, BrFftMk>::value;
     static_assert(!MB || Cfg::FFT, "multi-bit keys run the FP64 step");
+    static_assert(!MK || !MB, "multi-key launches take standard keys");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Br2Smem s = br2_carve<Cfg>(smem_raw);
     __shared__ unsigned s_item, s_entry;
@@ -700,12 +711,16 @@ __global__ void __launch_bounds__(Cfg::THREADS, Cfg::CTAS_PER_SM) blind_rotate_k
                 __syncthreads();
             }
         } else {
+            const u64 *mk_bk = nullptr;       // MK: the key of this thread's pass-3 slot
+            if constexpr (MK) mk_bk = p.mk_bk[p.mk_tenant[ct_of(tid & 1)]];
             if (tid < Cfg::CT) s.rot[(step0 & 1) * Cfg::CT + tid] = br_rotation<LUT>(p, ct_of(tid), step0);
             __syncthreads();
             for (int i = step0; i < step1; i++) {
                 int next = 0;
                 if (tid < Cfg::CT && i + 1 < step1) next = br_rotation<LUT>(p, ct_of(tid), i + 1);
-                if constexpr (Cfg::FFT)
+                if constexpr (MK)
+                    br_fft_step<true, Cfg>(s, mk_bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid, p.fft_tab);
+                else if constexpr (Cfg::FFT)
                     br_fft_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid, p.fft_tab);
                 else
                     br2_step<true, Cfg>(s, p.bk + (size_t)i * BK_ROW_U64, s.rot + (i & 1) * Cfg::CT, tid,
@@ -1117,8 +1132,19 @@ NB_D void bulk_g2s(void *dst, const void *src, u32 bytes, u64 *bar)
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// One tile of the grouped key switch (keyswitch_grouped_kernel): ciphertexts ct0 .. ct0 + nct - 1 (nct <= KS_TILE) of
+// the batch, all of one tenant, switched with that tenant's key
+struct KsTile {
+    const i32 *ks_a, *ks_b;
+    const float *ks_cv;
+    size_t ct0;
+    int nct;
+};
+
 // Fast path: in = 1024, n = 500, t = 8, base = 4 (the scheme's parameters, api_low_level.py:49-56).
-__global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs p)
+// GROUPED: CTA x takes tiles[x] (its ciphertexts and key) instead of ciphertexts x * p.tile .. with p's key.
+template <bool GROUPED>
+NB_D void keyswitch_body(const KeyswitchArgs &p, const KsTile *__restrict__ tiles)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     unsigned char *ring = smem_raw;                                               // [slot][k & 3][row][2000 B]
@@ -1127,8 +1153,14 @@ __global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs 
     u64 *empty = full + KS_SLOTS;
 
     const int tid = threadIdx.x;
-    const size_t ct0 = (size_t)blockIdx.x * p.tile;
-    const int nct = (int)min((size_t)p.tile, p.batch - ct0);
+    size_t ct0 = (size_t)blockIdx.x * p.tile;
+    int nct = (int)min((size_t)p.tile, p.batch - ct0);
+    const i32 *ks_a = p.ks_a, *ks_b = p.ks_b;
+    const float *ks_cv = p.ks_cv;
+    if constexpr (GROUPED) {
+        const KsTile &t = tiles[blockIdx.x];
+        ct0 = t.ct0; nct = t.nct; ks_a = t.ks_a; ks_b = t.ks_b; ks_cv = t.ks_cv;
+    }
     // slice of the input coefficients handled by this CTA (small batches: split-j over blockIdx.y so that
     // one ciphertext does not stream the whole 65 MB key through a single SM); always an even number of j
     const int j_per = ((KS_IN + p.splits - 1) / p.splits + KS_CV_BLOCK_J - 1) & ~(KS_CV_BLOCK_J - 1);
@@ -1161,14 +1193,14 @@ __global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs 
         const int q = tid - (KS_CONSUMERS + 32);
         u32 accb = 0;
         float cv = 0.f;
-        int4 kb = __ldg(reinterpret_cast<const int4 *>(p.ks_b));
-        float4 kc = __ldg(reinterpret_cast<const float4 *>(p.ks_cv));
-        kb = __ldg(reinterpret_cast<const int4 *>(p.ks_b) + min(j_begin * 8, KS_IN * 8 - 1));
-        kc = __ldg(reinterpret_cast<const float4 *>(p.ks_cv) + min(j_begin * 8, KS_IN * 8 - 1));
+        int4 kb = __ldg(reinterpret_cast<const int4 *>(ks_b));
+        float4 kc = __ldg(reinterpret_cast<const float4 *>(ks_cv));
+        kb = __ldg(reinterpret_cast<const int4 *>(ks_b) + min(j_begin * 8, KS_IN * 8 - 1));
+        kc = __ldg(reinterpret_cast<const float4 *>(ks_cv) + min(j_begin * 8, KS_IN * 8 - 1));
         float blk = 0.f;
         for (int jk = j_begin * 8; jk < j_end * 8; jk++) {
-            const int4 kb_next = __ldg(reinterpret_cast<const int4 *>(p.ks_b) + min(jk + 1, KS_IN * 8 - 1));
-            const float4 kc_next = __ldg(reinterpret_cast<const float4 *>(p.ks_cv) + min(jk + 1, KS_IN * 8 - 1));
+            const int4 kb_next = __ldg(reinterpret_cast<const int4 *>(ks_b) + min(jk + 1, KS_IN * 8 - 1));
+            const float4 kc_next = __ldg(reinterpret_cast<const float4 *>(ks_cv) + min(jk + 1, KS_IN * 8 - 1));
             const u32 bits = digits[(jk >> 3) * KS_TILE + q];
             const u32 d = (bits >> (14 - 2 * (jk & 7))) & 3u;
             accb -= d == 0 ? (u32)kb.x : d == 1 ? (u32)kb.y : d == 2 ? (u32)kb.z : (u32)kb.w;
@@ -1201,7 +1233,7 @@ __global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs 
                     const int slot = 2 * (j & 1) + h;
                     mbar_wait(&empty[slot], parity);  // first pass: passes immediately (phase -1 "complete")
                     mbar_expect_tx(&full[slot], KS_SLOT_BYTES);
-                    bulk_g2s(ring + slot * KS_SLOT_BYTES, p.ks_a + (size_t)(j * 8 + 4 * h) * 4 * KS_N, KS_SLOT_BYTES,
+                    bulk_g2s(ring + slot * KS_SLOT_BYTES, ks_a + (size_t)(j * 8 + 4 * h) * 4 * KS_N, KS_SLOT_BYTES,
                              &full[slot]);
                 }
             }
@@ -1267,6 +1299,14 @@ __global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs 
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_kernel(KeyswitchArgs p) { keyswitch_body<false>(p, nullptr); }
+
+// the grouped key switch (nb_mk_keyswitch): one tile table entry per CTA
+__global__ void __launch_bounds__(KS_THREADS, 1) keyswitch_grouped_kernel(KeyswitchArgs p, const KsTile *__restrict__ tiles)
+{
+    keyswitch_body<true>(p, tiles);
 }
 
 // second half of the fixed-shape variance sum for split launches: one thread per ciphertext adds its block sums in order

@@ -237,6 +237,82 @@ class Engine:
                    _ptr(res_cv), B)
         return res_a, res_b, res_cv
 
+    # --- multi-key calls (nb_mk_*, DESIGN.md section 17): tenant t owns counts[t] consecutive ciphertexts of the batch
+    @staticmethod
+    def _host_array(ctype, values):
+        return (ctype * max(len(values), 1))(*values)
+
+    def _mk_keys(self, bk_ints, counts):
+        return (self._host_array(ctypes.c_void_p, [k.data_ptr() for k in bk_ints]),
+                self._host_array(ctypes.c_size_t, [int(c) for c in counts]), len(bk_ints))
+
+    def mk_bootstrap_extract(self, x1, x2, c, s1, s2, mu, bk_ints, counts):
+        """bootstrap_extract over the ciphertexts of several keys: bk_ints[t] (bk_prepare) serves the counts[t]
+        ciphertexts of tenant t, which follow those of tenant t - 1 (nb_mk_bootstrap_extract)."""
+        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
+        a2 = b2 = None
+        if x2 is not None:
+            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
+        B = b1.numel()
+        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
+        keys, cnt, T = self._mk_keys(bk_ints, counts)
+        self._call('nb_mk_bootstrap_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
+                   int(mu), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
+        return out_a, out_b
+
+    def mk_bootstrap_lut_extract(self, x1, x2, c, s1, s2, tv, log2_outputs, bk_ints, counts):
+        """bootstrap_lut_extract over the ciphertexts of several keys, split as for mk_bootstrap_extract
+        (nb_mk_bootstrap_lut_extract); tv (1024,) serves the whole batch."""
+        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
+        a2 = b2 = None
+        if x2 is not None:
+            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
+        tv = self._dense(tv, torch.int32)
+        assert tuple(tv.shape) == (N,), tuple(tv.shape)
+        B = b1.numel()
+        rows = B << int(log2_outputs)
+        out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
+        keys, cnt, T = self._mk_keys(bk_ints, counts)
+        self._call('nb_mk_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
+                   _ptr(tv), 0, int(log2_outputs), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
+        return out_a, out_b
+
+    def mk_bootstrap_extract2(self, job_a, job_b, mu, bk_ints, counts):
+        """bootstrap_extract2 over the ciphertexts of several keys: both jobs are split by the same counts
+        (nb_mk_bootstrap_extract2).  Returns the two samples as views of one allocation."""
+        def parts(job):
+            x1, x2, c, s1, s2 = job
+            a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
+            a2 = b2 = None
+            if x2 is not None:
+                a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
+            return a1, b1, a2, b2, int(c), int(s1), int(s2)
+        pa, pb = parts(job_a), parts(job_b)
+        B = pa[1].numel()
+        out_a, out_b = self.empty((2 * B, N), torch.int32), self.empty((2 * B,), torch.int32)
+        keys, cnt, T = self._mk_keys(bk_ints, counts)
+        self._call('nb_mk_bootstrap_extract2', _ptr(pa[0]), _ptr(pa[1]), _ptr(pa[2]), _ptr(pa[3]), pa[4], pa[5], pa[6],
+                   _ptr(pb[0]), _ptr(pb[1]), _ptr(pb[2]), _ptr(pb[3]), pb[4], pb[5], pb[6], int(mu), keys, cnt, T,
+                   pa[0].shape[-1], _ptr(out_a), _ptr(out_b), B)
+        return (out_a[:B], out_b[:B]), (out_a[B:], out_b[B:])
+
+    def mk_keyswitch(self, keys, counts, src1, src2=None, c=0, want_cv=False):
+        """keyswitch over the ciphertexts of several keys: keys[t] = (ks_a, ks_b, ks_cv) of tenant t serves its counts[t]
+        rows (nb_mk_keyswitch).  Returns res_a (B, n), res_b (B,) and the variances (B,) or None."""
+        in_size, t, base, n = keys[0][0].shape if keys else (0, 0, 0, 0)
+        a1, b1 = self._dense(src1[0], torch.int32), self._dense(src1[1], torch.int32)
+        a2 = b2 = None
+        if src2 is not None:
+            a2, b2 = self._dense(src2[0], torch.int32), self._dense(src2[1], torch.int32)
+        B = b1.numel()
+        res_a, res_b = self.empty((B, n), torch.int32), self.empty((B,), torch.int32)
+        res_cv = self.empty((B,), torch.float32) if want_cv else None
+        ks = [self._host_array(ctypes.c_void_p, [k[i].data_ptr() for k in keys]) for i in range(3)]
+        self._call('nb_mk_keyswitch', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), ks[0], ks[1], ks[2],
+                   self._host_array(ctypes.c_size_t, [int(x) for x in counts]), len(keys), in_size, n, t,
+                   int(base).bit_length() - 1, _ptr(res_a), _ptr(res_b), _ptr(res_cv), B)
+        return res_a, res_b, res_cv
+
     def ks_prepare(self, ks_a, ks_b):
         """Lay a key-switch key (in = 1024, n = 500, t = 8, base 4) into the byte planes of the tensor-core key switch
         and register them for (ks_a, ks_b) on this engine (nb_ks_prepare).  Returns the planes, which must stay alive
