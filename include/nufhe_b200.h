@@ -181,6 +181,21 @@ int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, c
                     const int32_t *src2_b, int32_t c, const int32_t *const *ks_a_host, const int32_t *const *ks_b_host,
                     const float *const *ks_cv_host, const size_t *counts_host, size_t tenants, size_t in_size, size_t n,
                     int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv, size_t batch);
+/* The multi-key forms of tree LUTs and result packing (DESIGN.md section 18), with the conventions above.
+ * nb_mk_bootstrap_glwe_lut_extract: nb_bootstrap_glwe_lut_extract with per-tenant keys and counts, as
+ *     nb_mk_bootstrap_extract (same refusals).
+ * nb_mk_tree_keyswitch: nb_tree_keyswitch with per-tenant planes (nb_tree_prepare) and counts of rows; a CTA covers up
+ *     to 256 rows of one tenant.  NB_EINVAL also for a NULL planes pointer and the sizes nb_tree_keyswitch refuses.
+ * nb_mk_ntt_mac: nb_ntt_mac with per-tenant key spectra and group_counts[t], the number of consecutive groups of x
+ *     that belong to tenant t (they add up to `groups`).  NB_EINVAL also for a NULL key and the sizes nb_ntt_mac
+ *     refuses. */
+int nb_mk_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
+                                     const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants,
+                                     size_t n, int32_t *out_a, int32_t *out_b, size_t batch);
+int nb_mk_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *const *planes_host, const size_t *counts_host,
+                         size_t tenants, size_t n, int mask_size, int32_t *out, size_t rows);
+int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_host, const size_t *group_counts_host,
+                  size_t tenants, uint64_t *out, size_t rows, size_t outs, size_t groups);
 
 /* ---- LweLinear / LweNoiselessTrivial (lwe.py:346-422): res = (0, c) + s1 * x1 + s2 * x2 ------- */
 int nb_lwe_affine(nb_ctx *ctx, int32_t *res_a, int32_t *res_b, const int32_t *x1_a, const int32_t *x1_b,

@@ -51,6 +51,9 @@ SIGNATURES = {
                                     _vp, _sz],
     'nb_mk_keyswitch': [_vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _sz, _sz, _int, _int, _vp, _vp, _vp,
                         _sz],
+    'nb_mk_bootstrap_glwe_lut_extract': [_vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _sz],
+    'nb_mk_tree_keyswitch': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _vp, _sz],
+    'nb_mk_ntt_mac': [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _sz, _sz],
     'nb_ks_prepared_bytes': [],
     'nb_ks_prepare': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp],
     'nb_ks_forget': [_vp, _vp],

@@ -1426,4 +1426,71 @@ int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, c
     return NB_OK;
 }
 
+int nb_mk_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
+                                     const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants,
+                                     size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    const char *what = "nb_mk_bootstrap_glwe_lut_extract";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
+    if (batch && (!in_a || !in_b || !tv || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    BlindRotateArgs p{};
+    p.in1_a = in_a; p.in1_b = in_b; p.c = 0; p.s1 = 1; p.s2 = 0;
+    p.tv = tv; p.tv_stride = 2 * (size_t)NTT_N; p.log2_outputs = 0;
+    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
+    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
+}
+
+int nb_mk_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *const *planes_host, const size_t *counts_host,
+                         size_t tenants, size_t n, int mask_size, int32_t *out, size_t rows)
+{
+    const char *what = "nb_mk_tree_keyswitch";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!planes_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, rows));
+    if (rows && (!a || !out)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    for (size_t t = 0; t < tenants; t++)
+        if (!planes_host[t]) return fail(ctx, NB_EINVAL, std::string(what) + ": null planes of tenant " + std::to_string(t));
+    NB_TRY(tree_check_shape(ctx, n, mask_size, what));
+    if (rows == 0) return NB_OK;
+    std::vector<TreeTile> tiles(mk_tree_tiles(counts_host, tenants, planes_host, nullptr));
+    if (tiles.size() > 0x7fffffffu) return fail(ctx, NB_EINVAL, std::string(what) + ": too many rows");
+    mk_tree_tiles(counts_host, tenants, planes_host, tiles.data());
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_tree_keyswitch");
+    NB_TRY(mk_upload(ctx, tiles.data(), tiles.size() * sizeof(TreeTile)));
+    const u32 cols = (u32)(mask_size + 1) * PACK_N;
+    const dim3 grid((unsigned)tiles.size(), cols / (8 * TreeGemm::NTILES));
+    tree_gemm_mk_kernel<<<grid, GEMM_WARPS * 32, 0, ctx->stream>>>(reinterpret_cast<const TreeTile *>(ctx->d_mk), a,
+                                                                   (u32)n, cols, out);
+    return launch_check(ctx, "tree_gemm_mk_kernel");
+}
+
+int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_host, const size_t *group_counts_host,
+                  size_t tenants, uint64_t *out, size_t rows, size_t outs, size_t groups)
+{
+    const char *what = "nb_mk_ntt_mac";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!key_host || !group_counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(mk_check_counts(ctx, what, group_counts_host, tenants, groups));
+    if (groups && (!x || !out)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    for (size_t t = 0; t < tenants; t++)
+        if (!key_host[t]) return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(t));
+    if (rows == 0 || outs == 0 || rows > (1u << 24) || outs > (1u << 16))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": rows must be in [1, 2^24] and outputs in [1, 2^16]");
+    if (groups == 0) return NB_OK;
+    const size_t ctas = groups * (PACK_N / MAC_POINTS);
+    if (ctas > 0x7fffffffu) return fail(ctx, NB_EINVAL, std::string(what) + ": too many groups");
+    std::vector<const u64 *> group_keys(groups);
+    mk_group_keys(group_counts_host, tenants, reinterpret_cast<const u64 *const *>(key_host), group_keys.data());
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_ntt_mac");
+    NB_TRY(mk_upload(ctx, group_keys.data(), groups * sizeof(const u64 *)));
+    const dim3 grid((unsigned)ctas, (unsigned)((outs + MAC_OUTS - 1) / MAC_OUTS));
+    ntt_mac_mk_kernel<<<grid, MAC_WARPS * 32, 0, ctx->stream>>>((const u64 *)x, reinterpret_cast<const u64 *const *>(ctx->d_mk),
+                                                               (u64 *)out, (u32)rows, (u32)outs);
+    return launch_check(ctx, "ntt_mac_mk_kernel");
+}
+
 }  // extern "C"

@@ -13,6 +13,7 @@
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
 #include "compact_layout.cuh"
+#include "mk_layout.cuh"
 
 using namespace nb;
 
@@ -644,6 +645,34 @@ void emul_compact_extract(const uint16_t *data, int k, u32 p, i32 *a, i32 *b)
 void emul_tree_keyswitch(const i32 *a, const i32 *masks, const i32 *body, size_t n, int k, i32 *out, size_t rows)
 {
     emul_plane_gemm(TreeGemm{a, (u32)n, (u32)(k + 1) * PACK_N, out}, TreeSource{masks, body, (u32)n, (u32)k}, rows);
+}
+
+// Multi-key tables (mk_layout.cuh).  emul_mk_tree_tiles: the tiles of nb_mk_tree_keyswitch (first row, rows, tenant),
+// written when the arrays are not null; returns their number.  emul_mk_tree_keyswitch: nb_mk_tree_keyswitch, every tile
+// run as tree_gemm_mk_kernel runs it, with its tenant's masks[t] / body[t].  emul_mk_group_tenants: the tenant of every
+// group of nb_mk_ntt_mac.
+u64 emul_mk_tree_tiles(const size_t *counts, size_t tenants, u64 *row0, u32 *rows, u32 *tenant)
+{
+    std::vector<TreeTile> tiles(mk_tree_tiles(counts, tenants, nullptr, nullptr));
+    mk_tree_tiles(counts, tenants, nullptr, tiles.data());
+    for (size_t i = 0; i < tiles.size() && row0; i++) { row0[i] = tiles[i].row0; rows[i] = tiles[i].rows; tenant[i] = tiles[i].tenant; }
+    return tiles.size();
+}
+void emul_mk_tree_keyswitch(const i32 *a, const i32 *const *masks, const i32 *const *body, const size_t *counts,
+                            size_t tenants, size_t n, int k, i32 *out)
+{
+    const u32 cols = (u32)(k + 1) * PACK_N;
+    std::vector<TreeTile> tiles(mk_tree_tiles(counts, tenants, nullptr, nullptr));
+    mk_tree_tiles(counts, tenants, nullptr, tiles.data());
+    for (const TreeTile &t : tiles)
+        emul_plane_gemm(TreeGemm{a + t.row0 * n, (u32)n, cols, out + t.row0 * cols},
+                        TreeSource{masks[t.tenant], body[t.tenant], (u32)n, (u32)k}, t.rows);
+}
+u64 emul_mk_group_tenants(const size_t *group_counts, size_t tenants, u32 *out)
+{
+    std::vector<u32> ids(tenants);
+    for (size_t t = 0; t < tenants; t++) ids[t] = (u32)t;
+    return mk_group_keys(group_counts, tenants, ids.data(), out);
 }
 
 // emul_tree_assemble: tree_assemble_kernel's arithmetic, one (test vector, polynomial) after the other, with a serial

@@ -27,6 +27,7 @@
 #include "pk_layout.cuh"
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
+#include "mk_layout.cuh"
 
 namespace nb {
 
@@ -1790,13 +1791,12 @@ template <bool SIGNED_A> NB_D void mma_m16n8k32(i32 *c, const u32 *a, const u32 
 // of rows.  Per k-step of 32 a lane loads 2 words of each plane and column tile, forms the A fragment of each of its
 // row tiles in registers (P::a_frag), and issues every plane's and column tile's MMA with that fragment, so the four
 // plane sums of one output word sit in one thread.  The planes stay in L2 across CTAs.
-template <class P, class... Fields>
-__global__ void __launch_bounds__(GEMM_WARPS * 32) plane_gemm_kernel(const uint8_t *__restrict__ planes, u64 rows,
-                                                                     Fields... fields)
+// plane_gemm_cta is the work of CTA `cta` (rows from cta * MK_TILE_ROWS); nb_mk_tree_keyswitch runs it on a tile.
+template <class P>
+__device__ __forceinline__ void plane_gemm_cta(const P &op, const uint8_t *__restrict__ planes, u64 rows, u64 cta)
 {
-    const P op{fields...};
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    const u64 row0 = ((u64)blockIdx.x * GEMM_WARPS + (threadIdx.x >> 5)) * (16 * GEMM_MTILES);
+    const u64 row0 = (cta * GEMM_WARPS + (threadIdx.x >> 5)) * (16 * GEMM_MTILES);
     if (row0 >= rows) return;
     const u32 K = op.K(), cols = op.cols(), ksteps = K >> 5, col0 = blockIdx.y * (8 * P::NTILES);
     const uint8_t *bcol = planes + plane_offset(0, col0 + g, 0, K, cols);
@@ -1856,6 +1856,23 @@ __global__ void __launch_bounds__(GEMM_WARPS * 32) plane_gemm_kernel(const uint8
             }
 }
 
+template <class P, class... Fields>
+__global__ void __launch_bounds__(GEMM_WARPS * 32) plane_gemm_kernel(const uint8_t *__restrict__ planes, u64 rows,
+                                                                     Fields... fields)
+{
+    plane_gemm_cta(P{fields...}, planes, rows, blockIdx.x);
+}
+
+// nb_mk_tree_keyswitch: the tree key switch of several tenants' rows, CTA x on tile x (mk_layout.cuh), which holds at
+// most one CTA's rows of one tenant and that tenant's planes.
+__global__ void __launch_bounds__(GEMM_WARPS * 32) tree_gemm_mk_kernel(const TreeTile *__restrict__ tiles,
+                                                                       const i32 *__restrict__ a, u32 n, u32 cols,
+                                                                       i32 *__restrict__ out)
+{
+    const TreeTile tile = tiles[blockIdx.x];
+    plane_gemm_cta(TreeGemm{a + tile.row0 * n, n, cols, out + tile.row0 * cols}, tile.planes, tile.rows, 0);
+}
+
 // ---- result packing (DESIGN.md section 12; slot mapping, digits and rounding in pack_layout.cuh).
 // nb_pack_digits: LWE masks a (batch, n) row-major -> digit polynomials (groups, n t, N), row i t + j of group g holding
 // digit j of a[g N + p][i] at coefficient p.  A transpose: a CTA stages a 32 x 32 tile (32 inputs x 32 mask words) in
@@ -1897,13 +1914,13 @@ constexpr int MAC_WARPS = 16;
 constexpr int MAC_POINTS = 64;
 constexpr int MAC_OUTS = 2;
 
-__global__ void __launch_bounds__(MAC_WARPS * 32) ntt_mac_kernel(const u64 *__restrict__ x, const u64 *__restrict__ key,
-                                                                 u64 *__restrict__ out, u32 R, u32 U)
+// ntt_mac_group is the work of a CTA of group g with the key spectra `key`.
+__device__ __forceinline__ void ntt_mac_group(const u64 *__restrict__ x, const u64 *__restrict__ key,
+                                              u64 *__restrict__ out, u32 R, u32 U, u64 g)
 {
 #if defined(__CUDA_ARCH__)          // (mac128 and the limb fold exist on the device only)
     __shared__ u64 part[MAC_WARPS][MAC_OUTS][MAC_POINTS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const u64 g = blockIdx.x / (PACK_N / MAC_POINTS);
     const u32 pt0 = (blockIdx.x % (PACK_N / MAC_POINTS)) * MAC_POINTS, pt = pt0 + 2 * lane;
     const u32 u0 = blockIdx.y * MAC_OUTS, outs = U - u0 < (u32)MAC_OUTS ? U - u0 : (u32)MAC_OUTS;
     u32 acc[MAC_OUTS][2][5];
@@ -1946,6 +1963,21 @@ __global__ void __launch_bounds__(MAC_WARPS * 32) ntt_mac_kernel(const u64 *__re
         }
     }
 #endif
+}
+
+__global__ void __launch_bounds__(MAC_WARPS * 32) ntt_mac_kernel(const u64 *__restrict__ x, const u64 *__restrict__ key,
+                                                                 u64 *__restrict__ out, u32 R, u32 U)
+{
+    ntt_mac_group(x, key, out, R, U, blockIdx.x / (PACK_N / MAC_POINTS));
+}
+
+// nb_mk_ntt_mac: the same with the key spectra of group g at group_keys[g] (mk_layout.cuh: mk_group_keys).
+__global__ void __launch_bounds__(MAC_WARPS * 32) ntt_mac_mk_kernel(const u64 *__restrict__ x,
+                                                                    const u64 *const *__restrict__ group_keys,
+                                                                    u64 *__restrict__ out, u32 R, u32 U)
+{
+    const u64 g = blockIdx.x / (PACK_N / MAC_POINTS);
+    ntt_mac_group(x, group_keys[g], out, R, U, g);
 }
 
 // nb_pack_finish: out (G, k+1, N) uint16 = round_16(-C) for the masks, round_16(b_c - C) at the slots of the body.

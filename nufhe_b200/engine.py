@@ -262,20 +262,69 @@ class Engine:
 
     def mk_bootstrap_lut_extract(self, x1, x2, c, s1, s2, tv, log2_outputs, bk_ints, counts):
         """bootstrap_lut_extract over the ciphertexts of several keys, split as for mk_bootstrap_extract
-        (nb_mk_bootstrap_lut_extract); tv (1024,) serves the whole batch."""
+        (nb_mk_bootstrap_lut_extract); tv (1024,) serves the whole batch, tv (B, 1024) holds one per ciphertext."""
         a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
         a2 = b2 = None
         if x2 is not None:
             a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
         tv = self._dense(tv, torch.int32)
-        assert tuple(tv.shape) == (N,), tuple(tv.shape)
         B = b1.numel()
+        stride = 0 if tv.dim() == 1 else N
+        assert tuple(tv.shape) == ((N,) if stride == 0 else (B, N)), (tuple(tv.shape), B)
         rows = B << int(log2_outputs)
         out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
         keys, cnt, T = self._mk_keys(bk_ints, counts)
         self._call('nb_mk_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
-                   _ptr(tv), 0, int(log2_outputs), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
+                   _ptr(tv), stride, int(log2_outputs), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
         return out_a, out_b
+
+    def mk_bootstrap_glwe_lut_extract(self, x, tv, bk_ints, counts):
+        """bootstrap_glwe_lut_extract over the ciphertexts of several keys, split as for mk_bootstrap_extract
+        (nb_mk_bootstrap_glwe_lut_extract)."""
+        a, b = self._dense(x[0], torch.int32), self._dense(x[1], torch.int32)
+        tv = self._dense(tv, torch.int32)
+        B = b.numel()
+        n = a.shape[-1]
+        if tuple(tv.shape) != (B, 2, N) or a.numel() != B * n:
+            raise ValueError('mk_bootstrap_glwe_lut_extract: tv %s for %d ciphertexts' % (tuple(tv.shape), B))
+        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
+        keys, cnt, T = self._mk_keys(bk_ints, counts)
+        self._call('nb_mk_bootstrap_glwe_lut_extract', _ptr(a), _ptr(b), _ptr(tv), keys, cnt, T, n, _ptr(out_a),
+                   _ptr(out_b), B)
+        return out_a, out_b
+
+    def mk_tree_keyswitch(self, a, planes, counts, mask_size):
+        """tree_keyswitch over the rows of several tenants: planes[t] (tree_prepare) serves the counts[t] rows of tenant
+        t (nb_mk_tree_keyswitch).  Returns V (R, k+1, N)."""
+        a = self._dense(a, torch.int32)
+        rows, n = a.shape
+        want = self.lib.nb_tree_planes_bytes(n, int(mask_size))
+        for t, p in enumerate(planes):
+            if p.numel() != want:
+                raise ValueError('mk_tree_keyswitch: tenant %d: %d plane bytes do not fit n = %d, k = %d'
+                                 % (t, p.numel(), n, mask_size))
+        out = self.empty((rows, mask_size + 1, N), torch.int32)
+        self._call('nb_mk_tree_keyswitch', _ptr(a), self._host_array(ctypes.c_void_p, [p.data_ptr() for p in planes]),
+                   self._host_array(ctypes.c_size_t, [int(c) for c in counts]), len(planes), n, int(mask_size),
+                   _ptr(out), rows)
+        return out
+
+    def mk_ntt_mac(self, x, keys, group_counts):
+        """ntt_mac over the groups of several tenants: keys[t] (R, U, N) serves the group_counts[t] groups of tenant t
+        (nb_mk_ntt_mac).  Returns (G, U, N)."""
+        x = self._dense(x, torch.int64)
+        keys = [self._dense(k, torch.int64) for k in keys]
+        if x.dim() != 3 or x.shape[2] != N or not keys or any(tuple(k.shape) != tuple(keys[0].shape) for k in keys) \
+                or keys[0].dim() != 3 or keys[0].shape[2] != N or x.shape[1] != keys[0].shape[0]:
+            raise ValueError('mk_ntt_mac: x %s and keys %s are not (G, R, N) and (R, U, N)'
+                             % (tuple(x.shape), [tuple(k.shape) for k in keys]))
+        groups, rows = x.shape[:2]
+        outs = keys[0].shape[1]
+        out = self.empty((groups, outs, N), torch.int64)
+        self._call('nb_mk_ntt_mac', _ptr(x), self._host_array(ctypes.c_void_p, [k.data_ptr() for k in keys]),
+                   self._host_array(ctypes.c_size_t, [int(c) for c in group_counts]), len(keys), _ptr(out), rows, outs,
+                   groups)
+        return out
 
     def mk_bootstrap_extract2(self, job_a, job_b, mu, bk_ints, counts):
         """bootstrap_extract2 over the ciphertexts of several keys: both jobs are split by the same counts

@@ -12,18 +12,23 @@ import torch
 from .api_low_level import NuFHECloudKey, empty_ciphertext
 from .gates import MU, _BINARY_GATES, check_shape, get_shape, result_shape
 from .lwe import LweSampleArray
-from .lut import _check_config, _check_margin, _sigma
+from .lut import LookupTable, _check_config, _check_margin, _sigma
 from .numeric_functions import phase_to_t32
 from .performance import PerformanceParameters
 from .tgsw import engine_format, fused_kernel_supported
-from . import gates
+from .tree_lut import NuFHETreeKey, TreeLookupTable
+from .packing import NuFHEPackingKey, PackedLweSampleArray
+from .compact import CompactLweSampleArray
+from .index_lookup import EncryptedIndexArray, IndexTable
+from . import compact, gates, index_lookup, packing, tree_lut
 
 # gates that need no key: run per tenant
 _KEYLESS = {'not': 1, 'copy': 1, 'constant': 1}
 
 
 class MultiKeyVirtualMachine:
-    """Executes gates and one-table LUTs on the ciphertexts of several cloud keys at once.
+    """Executes gates, LUTs, tree LUTs, packing, expansion and index lookups on the ciphertexts of several cloud keys at
+    once.
 
     Every operand is a list aligned with `cloud_keys`: entry t holds tenant t's ciphertexts (of any shape, broadcast per
     tenant as VirtualMachine does), or None when tenant t has no work, in which case all its operands must be None.
@@ -205,13 +210,44 @@ class MultiKeyVirtualMachine:
         raise AttributeError(name)
 
     # --- lookup tables -------------------------------------------------------------------------
+    def _tenant_tables(self, tables, active):
+        """A list of per-tenant LookupTables: the table of tenant 0's kind, after checking that every active tenant has
+        one and that they share bits, log2_outputs and out."""
+        if len(tables) != self.tenants:
+            raise ValueError('tables must be one LookupTable or a list of %d, one per tenant' % self.tenants)
+        ref = None
+        for t in active:
+            table = tables[t]
+            if not isinstance(table, LookupTable):
+                raise TypeError('tenant %d: a LookupTable is needed (vm.make_lut), got %s' % (t, type(table).__name__))
+            if table.batch_shape:
+                raise ValueError('tenant %d: the multi-key machine takes one table per tenant, not one per ciphertext' % t)
+            if ref is None:
+                ref = table
+            elif (table.bits, table.log2_outputs, table.out) != (ref.bits, ref.log2_outputs, ref.out):
+                raise ValueError('tenant %d: the tables must share bits, log2_outputs and out (%s, got %s)'
+                                 % (t, (ref.bits, ref.log2_outputs, ref.out), (table.bits, table.log2_outputs, table.out)))
+        return ref
+
     def lut(self, table, xs, ys=None, shift=0, dest=None):
         """f(x), or f(x * 2^shift + y), for every tenant's ciphertexts with one LookupTable (VirtualMachine.make_lut)
-        shared by all tenants.  Entry t of the result is one ciphertext array, or a list of 2^L of them for a table with
-        several outputs.  ValueError for a configuration without enough noise margin (lut.check_noise) and for tables
-        with one entry per ciphertext."""
+        shared by all tenants, or a list of one table per tenant (None for idle tenants), all with the same bits,
+        log2_outputs and out.  Entry t of the result is one ciphertext array, or a list of 2^L of them for a table with
+        several outputs.  ValueError for a configuration without enough noise margin (lut.check_noise), for tables
+        with one entry per ciphertext and for per-tenant tables that differ in bits, log2_outputs or out."""
+        if isinstance(table, (list, tuple)):
+            tables = list(table)
+            operand_lists = (xs,) if ys is None else (xs, ys)
+            active, _ = self._active(operand_lists, None)
+            table = self._tenant_tables(tables, active)
+            if table is None:
+                return [None] * self.tenants
+            return self._lut(table, xs, ys, shift, dest, tables)
         if table.batch_shape:
             raise ValueError('the multi-key machine takes one table for every ciphertext, not one per ciphertext')
+        return self._lut(table, xs, ys, shift, dest, None)
+
+    def _lut(self, table, xs, ys, shift, dest, tables):
         operand_lists = (xs,) if ys is None else (xs, ys)
         K = table.outputs
         L = table.log2_outputs
@@ -237,7 +273,10 @@ class MultiKeyVirtualMachine:
         p1 = self._concat(xs, active, shapes)
         p2 = self._concat(ys, active, shapes) if ys is not None else None
         s1 = 1 << shift if ys is not None else 1
-        ea, eb = self.thread.mk_bootstrap_lut_extract(p1, p2, 0, s1, 1, table.tv, L, self._bk_ints, counts)
+        tv = table.tv
+        if tables is not None:      # one test vector per ciphertext: its tenant's
+            tv = torch.cat([tables[t].tv.reshape(1, -1).expand(counts[t], -1) for t in active])
+        ea, eb = self.thread.mk_bootstrap_lut_extract(p1, p2, 0, s1, 1, tv, L, self._bk_ints, counts)
         ra, rb, rcv = self._keyswitch([c * K for c in counts], (ea, eb))
         # sample j of ciphertext c is row c * K + j: one contiguous block per output
         total = rb.numel() // K
@@ -249,4 +288,318 @@ class MultiKeyVirtualMachine:
                       for j in range(K)]
         for t in active:
             out[t] = per_output[0][t] if K == 1 else [per_output[j][t] for j in range(K)]
+        return out
+
+    # --- per-tenant extras (DESIGN.md section 18) --------------------------------------------------
+    def _tenant_objects(self, objs, active, cls, what, hint=''):
+        """Check a list of per-tenant objects (keys, compact ciphertexts, indices): aligned with the tenants, an
+        instance of `cls` made for this machine's parameters for every active tenant."""
+        if not isinstance(objs, (list, tuple)) or len(objs) != self.tenants:
+            raise ValueError('%s must be a list of %d entries, one per tenant' % (what, self.tenants))
+        for t in active:
+            if not isinstance(objs[t], cls):
+                raise TypeError('tenant %d: %s needs a %s%s, got %s' % (t, what, cls.__name__, hint, type(objs[t]).__name__))
+            if objs[t].params != self.params:
+                raise ValueError('tenant %d: the %s was made for other parameters than the cloud keys' % (t, what))
+        return list(objs)
+
+    @staticmethod
+    def _pass_counts(counts, c0, c1, *per_tenant):
+        """The rows of [c0, c1) of the concatenated batch that each tenant owns (counts: rows per tenant, in order), for
+        the tenants that own some, and their entries of each list in `per_tenant`."""
+        hi = numpy.cumsum(counts, dtype=numpy.int64)
+        own = numpy.clip(numpy.minimum(hi, c1) - numpy.maximum(hi - counts, c0), 0, None)
+        idx = numpy.nonzero(own)[0]
+        return ([int(own[i]) for i in idx],) + tuple([lst[i] for i in idx] for lst in per_tenant)
+
+    def _per_tenant(self, dest, active, K, what):
+        """dest as a list of lists of K results (None for idle tenants)."""
+        if dest is None:
+            return None
+        if not isinstance(dest, (list, tuple)) or len(dest) != self.tenants:
+            raise ValueError('dest must be a list of %d entries, one per tenant' % self.tenants)
+        out = [None if d is None else ([d] if isinstance(d, LweSampleArray) else list(d)) for d in dest]
+        active_set = set(active)
+        for t in range(self.tenants):
+            if (t in active_set) != (out[t] is not None):
+                raise ValueError('tenant %d: a destination is needed exactly for a tenant with operands' % t)
+            if out[t] is not None and len(out[t]) != K:
+                raise ValueError('tenant %d: %s writes %d results, got %d' % (t, what, K, len(out[t])))
+        return out
+
+    def lut_tree(self, tree_keys, table, digits, dest=None):
+        """f(d_{D-1}, ..., d_0) for every tenant (VirtualMachine.lut_tree): `digits` is a list of D operand lists
+        (highest digit first), `tree_keys` the list of the tenants' NuFHETreeKeys (None for idle tenants), `table` one
+        TreeLookupTable shared by all tenants.  Every level runs once over the concatenated batch of all tenants.  Entry
+        t of the result is one ciphertext array, or a list of F for a table of F functions."""
+        if not isinstance(table, TreeLookupTable):
+            raise TypeError('lut_tree needs a TreeLookupTable (vm.make_tree_lut), got %s' % type(table).__name__)
+        if table.params != self.params or table.multi_bit != 1:
+            raise ValueError('the table was made for other parameters or another kind of bootstrap key')
+        digits = list(digits)
+        if len(digits) != table.digits:
+            raise ValueError('the table takes %d digits, got %d' % (table.digits, len(digits)))
+        F = table.functions
+        active, shapes = self._active(digits, None)
+        tree_keys = self._tenant_objects(tree_keys, active, NuFHETreeKey, 'tree key',
+                                         ' (ctx.make_cloud_key(sk, tree_key=True))')
+        dest_lists = self._per_tenant(dest, active, F, 'a table of %d functions' % F)
+        for t in active:
+            for d in digits:
+                if tuple(d[t].shape) != tuple(digits[0][t].shape):
+                    raise ValueError('tenant %d: all digits must have one shape, got %s and %s'
+                                     % (t, tuple(digits[0][t].shape), tuple(d[t].shape)))
+            if dest_lists is not None:
+                for r in dest_lists[t]:
+                    check_shape(r, *[d[t] for d in digits])
+                shapes[t] = tuple(dest_lists[t][0].shape)
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        all_counts = self._counts(active, shapes)
+        counts = [all_counts[t] for t in active]
+        bks = [self._bk_ints[t] for t in active]
+        kss = [self._ks[t] for t in active]
+        planes = [tree_keys[t].planes(thr) for t in active]
+        flat = [self._concat(d, active, shapes) for d in reversed(digits)]        # d_0 first
+        B = sum(counts)
+        n = self.params.in_out_params.size
+        out_a = thr.empty((B, F, n), torch.int32)
+        out_b = thr.empty((B, F), torch.int32)
+        step = max(1, tree_lut.ROWS_PER_PASS // table.groups)
+        for c0 in range(0, B, step):
+            c1 = min(B, c0 + step)
+            cnt, pbks, pkss, pplanes = self._pass_counts(counts, c0, c1, bks, kss, planes)
+            part = [(a[c0:c1], b[c0:c1]) for a, b in flat]
+            cur = self._tree_level1(table, part[0], pbks, pkss, cnt)
+            for level in range(1, table.digits):
+                cur = self._tree_level(table, pplanes, cur, part[level], pbks, pkss, cnt)
+            out_a[c0:c1].copy_(cur[0])
+            out_b[c0:c1].copy_(cur[1])
+        # function f of every tenant: views of one (F, B) allocation
+        out_a, out_b = out_a.transpose(0, 1).contiguous(), out_b.t().contiguous()
+        out_cv = thr.empty((F, B), torch.float32).fill_(float(tree_lut.output_variance(table.params, table.bits,
+                                                                                        table.digits)))
+        row = 0
+        for t, rows in zip(active, counts):
+            shape, r = shapes[t], slice(row, row + rows)
+            res = [LweSampleArray(self.params.in_out_params, out_a[f, r].reshape(shape + (n,)),
+                                  out_b[f, r].reshape(shape), out_cv[f, r].reshape(shape)) for f in range(F)]
+            row += rows
+            if dest_lists is not None:
+                for d, x in zip(dest_lists[t], res):
+                    d.a.copy_(x.a)
+                    d.b.copy_(x.b)
+                    d.current_variances.copy_(x.current_variances)
+                res = dest_lists[t]
+            out[t] = res[0] if table.single else res
+        return out
+
+    def _tree_level1(self, table, d0, bks, kss, cnt):
+        """tree_lut._level1 over the concatenated batch: cnt[i] ciphertexts of the i-th active tenant."""
+        a, b = d0
+        B, n = a.shape
+        Q, L = table.groups, table.log2_outputs
+        K = 1 << L
+        ea_ = a[:, None, :].expand(B, Q, n).reshape(B * Q, n)
+        eb_ = b[:, None].expand(B, Q).reshape(B * Q)
+        tv = table.tv.reshape(Q, -1)[None].expand(B, Q, table.tv.shape[-1]).reshape(B * Q, -1)
+        ea, eb = self.thread.mk_bootstrap_lut_extract((ea_, eb_), None, 0, 1, 1, tv, L, bks, [c * Q for c in cnt])
+        ra, rb, _ = self.thread.mk_keyswitch(kss, [c * Q * K for c in cnt], (ea, eb))
+        return ra.reshape(B, Q * K, n)[:, :table.columns], rb.reshape(B, Q * K)[:, :table.columns]
+
+    def _tree_level(self, table, planes, cur, digit, bks, kss, cnt):
+        """tree_lut._level over the concatenated batch: the tree key switch with each tenant's planes, one assembly,
+        the GLWE-test-vector bootstrap and the key switch with each tenant's keys."""
+        thr = self.thread
+        ca, cb = cur
+        B, W, n = ca.shape
+        M = 1 << table.bits
+        k = self.params.tgsw_params.tlwe_params.mask_size
+        T = B * (W // M)
+        v = thr.mk_tree_keyswitch(ca.reshape(B * W, n), planes, [c * W for c in cnt], k)
+        tv = thr.tree_assemble(v.reshape(T, M, k + 1, -1), cb.reshape(T, M), table.bits)
+        da, db = digit
+        xa = da[:, None, :].expand(B, W // M, n).reshape(T, n)
+        xb = db[:, None].expand(B, W // M).reshape(T)
+        per = [c * (W // M) for c in cnt]
+        ea, eb = thr.mk_bootstrap_glwe_lut_extract((xa, xb), tv, bks, per)
+        ra, rb, _ = thr.mk_keyswitch(kss, per, (ea, eb))
+        return ra.reshape(B, W // M, n), rb.reshape(B, W // M)
+
+    def pack(self, packing_keys, results_list):
+        """Pack every tenant's results (VirtualMachine.pack) with its NuFHEPackingKey: a list of PackedLweSampleArrays
+        (None for idle tenants), each byte-identical to the tenant's own vm.pack.  Each tenant's results start at a
+        group boundary, so a group never mixes tenants; the rows that pad a tenant's last group are zero, which packs
+        exactly as an empty slot.  The MAC of all groups runs in one launch per pass, each group with its tenant's key."""
+        active, shapes = self._active((results_list,), None)
+        packing_keys = self._tenant_objects(packing_keys, active, NuFHEPackingKey, 'packing key')
+        for t in active:
+            if results_list[t].params != self.params.in_out_params:
+                raise ValueError('tenant %d: the ciphertexts do not have the LWE parameters of the packing key' % t)
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        tl = self.params.tgsw_params.tlwe_params
+        k, N = tl.mask_size, tl.polynomial_degree
+        n = self.params.in_out_params.size
+        counts = [int(numpy.prod(shapes[t], dtype=numpy.int64)) for t in active]
+        groups = [-(-c // N) for c in counts]
+        G = sum(groups)
+        # padded row r of group g holds row src[g N + slot] of the concatenated batch, or the zero row B
+        B = sum(counts)
+        src = numpy.full(G * N, B, numpy.int64)
+        g0 = c0 = 0
+        for c, g in zip(counts, groups):
+            src[g0 * N:g0 * N + c] = numpy.arange(c0, c0 + c)
+            g0, c0 = g0 + g, c0 + c
+        a_all = torch.cat([results_list[t].a.reshape(-1, n) for t in active] + [thr.empty((1, n), torch.int32).zero_()])
+        b_all = torch.cat([results_list[t].b.reshape(-1) for t in active] + [thr.empty((1,), torch.int32).zero_()])
+        src = thr.to_device(src)
+        keys = [packing_keys[t].spectra(thr) for t in active]
+        data = thr.empty((G, k + 1, N), torch.uint16)
+        step = packing.groups_per_pass(self.params)
+        for p0 in range(0, G, step):
+            p1 = min(G, p0 + step)
+            idx = src[p0 * N:p1 * N]
+            spec = thr.ntt_forward_i32(thr.pack_digits(a_all.index_select(0, idx)))
+            cnt, pkeys = self._pass_counts(groups, p0, p1, keys)
+            part = thr.pack_finish(thr.ntt_inverse_i32(thr.mk_ntt_mac(spec, pkeys, cnt)), b_all.index_select(0, idx))
+            del spec
+            data.view(torch.int16)[p0:p1].copy_(part.view(torch.int16))
+        g0 = 0
+        for t, g in zip(active, groups):
+            out[t] = PackedLweSampleArray(self.params, shapes[t], data[g0:g0 + g])
+            g0 += g
+        return out
+
+    def expand(self, compacts):
+        """The LweSampleArrays of every tenant's compact ciphertexts (VirtualMachine.expand): one extraction over all
+        tenants' groups, then one multi-key key switch, a few groups per pass (compact.PASS_BYTES).  A list aligned with
+        the tenants (None for idle tenants)."""
+        if not isinstance(compacts, (list, tuple)) or len(compacts) != self.tenants:
+            raise ValueError('compacts must be a list of %d entries, one per tenant' % self.tenants)
+        active = [t for t in range(self.tenants) if compacts[t] is not None]
+        compacts = self._tenant_objects(compacts, active, CompactLweSampleArray, 'compact ciphertext')
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        tl = self.params.tgsw_params.tlwe_params
+        N = tl.polynomial_degree
+        io_params = self.params.in_out_params
+        n = io_params.size
+        counts = [compacts[t].size for t in active]
+        groups = [-(-c // N) for c in counts]
+        B, G = sum(counts), sum(groups)
+        res_a, res_b = thr.empty((B, n), torch.int32), thr.empty((B,), torch.int32)
+        res_cv = thr.empty((B,), torch.float32)
+        # slot s of the concatenated groups is row keep[s] of the batch, or padding (-1)
+        keep = numpy.full(G * N, -1, numpy.int64)
+        g0 = c0 = 0
+        for c, g in zip(counts, groups):
+            keep[g0 * N:g0 * N + c] = numpy.arange(c0, c0 + c)
+            g0, c0 = g0 + g, c0 + c
+        data = torch.cat([compacts[t].data.to(thr.device) for t in active]) if G else None
+        kss = [self._ks[t] for t in active]
+        fresh, mask_rnd, body_rnd, _ = compact.noise_terms(self.params)
+        step = compact.groups_per_pass(self.params)
+        for p0 in range(0, G, step):
+            p1 = min(G, p0 + step)
+            slots = keep[p0 * N:p1 * N]
+            rows = numpy.nonzero(slots >= 0)[0]
+            r0, r1 = int(slots[rows[0]]), int(slots[rows[-1]]) + 1      # the rows of a pass are consecutive
+            ea, eb = thr.compact_extract(data[p0:p1], (p1 - p0) * N)
+            if len(rows) < (p1 - p0) * N:
+                sel = thr.to_device(rows)
+                ea, eb = ea.index_select(0, sel), eb.index_select(0, sel)
+            cnt, pkss = self._pass_counts(counts, r0, r1, kss)
+            ra, rb, rcv = thr.mk_keyswitch(pkss, cnt, (ea, eb), want_cv=True)
+            del ea, eb
+            res_a[r0:r1], res_b[r0:r1] = ra, rb
+            res_cv[r0:r1] = rcv + (fresh + mask_rnd + body_rnd)
+        row = 0
+        for t, c in zip(active, counts):
+            shape = compacts[t].shape
+            out[t] = LweSampleArray(io_params, res_a[row:row + c].reshape(shape + (n,)), res_b[row:row + c].reshape(shape),
+                                    res_cv[row:row + c].reshape(shape))
+            row += c
+        return out
+
+    def lookup(self, indexes, table, dest=None):
+        """table[idx] for every tenant's EncryptedIndexArray (VirtualMachine.lookup) with one IndexTable shared by all
+        tenants: the queries of all tenants go through one CMux tree and rotation per pass, then one multi-key key
+        switch.  Entry t of the result is one ciphertext array of the tenant's index shape, or a list of W for a table
+        of W columns."""
+        if not isinstance(table, IndexTable):
+            raise TypeError('lookup needs an IndexTable (vm.make_index_table), got %s' % type(table).__name__)
+        if not isinstance(indexes, (list, tuple)) or len(indexes) != self.tenants:
+            raise ValueError('indexes must be a list of %d entries, one per tenant' % self.tenants)
+        active = [t for t in range(self.tenants) if indexes[t] is not None]
+        indexes = self._tenant_objects(indexes, active, EncryptedIndexArray, 'encrypted index',
+                                       ' (decompress() a compressed one first)')
+        if table.params != self.params:
+            raise ValueError('the table was made for other parameters than the cloud keys')
+        for t in active:
+            if indexes[t].bits != table.bits:
+                raise ValueError('tenant %d: the table takes %d-bit indices, got %d bits' % (t, table.bits, indexes[t].bits))
+        m, W = table.bits, table.columns
+        dest_lists = self._per_tenant(dest, active, W, 'a table of %d columns' % W)
+        for t in active:
+            if dest_lists is not None and any(tuple(d.shape) != indexes[t].shape for d in dest_lists[t]):
+                raise ValueError('tenant %d: lookup writes %d results of shape %s' % (t, W, indexes[t].shape))
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        n = self.params.in_out_params.size
+        counts = [int(numpy.prod(indexes[t].shape, dtype=numpy.int64)) for t in active]
+        offsets = numpy.concatenate([[0], numpy.cumsum(counts)]).astype(numpy.int64)
+        B = int(offsets[-1])
+        sels = [indexes[t].samples.reshape(c, m, 2, 2, 2, index_lookup.N) for t, c in zip(active, counts)]
+        kss = [self._ks[t] for t in active]
+        # column w of query q (of the concatenated batch) at row w B + q
+        res_a, res_b = thr.empty((W * B, n), torch.int32), thr.empty((W * B,), torch.int32)
+        step = index_lookup.queries_per_pass(m, W)
+        for q0 in range(0, B, step):
+            q1 = min(B, q0 + step)
+            Q = q1 - q0
+            cnt, pkss, psels, plos = self._pass_counts(counts, q0, q1, kss, sels, offsets[:-1])
+            pieces = [s[max(q0, lo) - lo:][:c] for s, lo, c in zip(psels, plos, cnt)]
+            spec = thr.index_prepare(torch.cat(pieces) if len(pieces) > 1 else pieces[0]).reshape(Q, m, -1)
+            cur = table.polys
+            for j in range(index_lookup.ROTATE_BITS, m):
+                cur = thr.index_cmux_level(cur, spec, j, Q)
+            a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
+            del spec, cur
+            # rows (w, q) are column-major; the key switch wants each tenant's W c rows together, in vm.lookup's order
+            perm, lo = [], 0
+            for c in cnt:
+                perm.append((numpy.arange(W)[:, None] * Q + numpy.arange(lo, lo + c)[None, :]).reshape(-1))
+                lo += c
+            perm = numpy.concatenate(perm)
+            sel = thr.to_device(perm)
+            ra, rb, _ = thr.mk_keyswitch(pkss, [W * c for c in cnt], (a.reshape(W * Q, -1).index_select(0, sel),
+                                                                      b.reshape(W * Q).index_select(0, sel)))
+            dst = thr.to_device((perm // Q) * B + q0 + perm % Q)
+            res_a.index_copy_(0, dst, ra)
+            res_b.index_copy_(0, dst, rb)
+        res_cv = thr.empty((W * B,), torch.float32).fill_(float(index_lookup.output_variance(self.params, m)))
+        for i, t in enumerate(active):
+            shape, lo, c = indexes[t].shape, int(offsets[i]), counts[i]
+            cols = []
+            for w in range(W):
+                r = slice(w * B + lo, w * B + lo + c)
+                x = LweSampleArray(self.params.in_out_params, res_a[r].reshape(shape + (n,)), res_b[r].reshape(shape),
+                                   res_cv[r].reshape(shape))
+                if dest_lists is not None:
+                    d = dest_lists[t][w]
+                    d.a.copy_(x.a)
+                    d.b.copy_(x.b)
+                    d.current_variances.copy_(x.current_variances)
+                    x = d
+                cols.append(x)
+            out[t] = cols[0] if table.single else cols
         return out
