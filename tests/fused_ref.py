@@ -223,8 +223,16 @@ class Mode:
             assert (g[sel] == w[:k]).all(), (what, self.name, B, 'output', i)
 
     def equal(self, got, B):
+        return self.row_equal(got, B)[1].all()
+
+    def row_equal(self, got, B):
+        """(the compared rows below B, whether every output of each equals the oracle)"""
         k = int(numpy.searchsorted(self.rows, B))
-        return all((g[self.rows[:k]] == w[:k]).all() for g, w in zip(got, self.want))
+        sel = self.rows[:k]
+        eq = numpy.ones(k, bool)
+        for g, w in zip(got, self.want):
+            eq &= (g[sel] == w[:k]).all(axis=tuple(range(1, g.ndim)))
+        return sel, eq
 
 
 def gate_mode(name, n, bk, c, s1, s2, mu, two, seed, B, rows=None, x=None, ref=STANDARD, layout=cycled):
