@@ -196,6 +196,26 @@ int nb_mk_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *const *pl
                          size_t tenants, size_t n, int mask_size, int32_t *out, size_t rows);
 int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_host, const size_t *group_counts_host,
                   size_t tenants, uint64_t *out, size_t rows, size_t outs, size_t groups);
+/* Expansion of compressed cloud keys into slots of the multi-key machine (DESIGN.md section 19).  seeds_host holds 8
+ * words per tenant, the seed of its compressed key; the other per-tenant arrays are HOST arrays of device pointers.
+ * Neither call allocates (beyond the multi-key scratch) or synchronises.
+ * nb_mk_bk_expand: slot t (n rows of nb_bk_row_u64() uint64) receives the FP64 part of the engine key of the bootstrap
+ *     key whose masks are the stream (seed t, nonce 1) laid out (n, k+1, l, k, N) (nb_seeded_uniform_i32) and whose
+ *     bodies are bodies_host[t] (n, k+1, l, N) int32: word for word what nb_bk_prepare stores there for that key.  The
+ *     NTT planes of the rows are not written, so the slot is registered for the nb_mk_* bootstraps only (it replaces any
+ *     earlier registration of the range); nb_mk_slot_release(ctx, slot) drops it, before the slot's memory is freed.
+ *     k = 1, l = 2, N = 1024 and 1 <= n <= 1024 only (NB_EUNSUPPORTED otherwise).
+ * nb_mk_ks_expand: ks_a_host[t] (in, t, base, n) int32 receives the masks of the stream (seed t, nonce 2) laid out
+ *     (in, t, base-1, n) in its rows h >= 1 and zeros in its rows h = 0, as CompressedCloudKey.decompress() lays them
+ *     out; a GEMM registration (nb_ks_prepare) of that ks_a is dropped.  in = 1024, n = 500, t = 8, base 4 only
+ *     (NB_EUNSUPPORTED otherwise).
+ * NB_EINVAL for a NULL pointer; tenants = 0 is a no-op. */
+int nb_mk_bk_expand(nb_ctx *ctx, const uint32_t *seeds_host, const int32_t *const *bodies_host,
+                    uint64_t *const *slots_host, size_t tenants, size_t n, int mask_size, int decomp_length,
+                    size_t poly_degree);
+int nb_mk_ks_expand(nb_ctx *ctx, const uint32_t *seeds_host, int32_t *const *ks_a_host, size_t tenants, size_t in_size,
+                    int t, int log2_base, size_t n);
+int nb_mk_slot_release(nb_ctx *ctx, const uint64_t *slot);
 
 /* ---- LweLinear / LweNoiselessTrivial (lwe.py:346-422): res = (0, c) + s1 * x1 + s2 * x2 ------- */
 int nb_lwe_affine(nb_ctx *ctx, int32_t *res_a, int32_t *res_b, const int32_t *x1_a, const int32_t *x1_b,

@@ -54,6 +54,9 @@ SIGNATURES = {
     'nb_mk_bootstrap_glwe_lut_extract': [_vp, _vp, _vp, _vp, _vp, _vp, _sz, _sz, _vp, _vp, _sz],
     'nb_mk_tree_keyswitch': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _vp, _sz],
     'nb_mk_ntt_mac': [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _sz, _sz],
+    'nb_mk_bk_expand': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _sz],
+    'nb_mk_ks_expand': [_vp, _vp, _vp, _sz, _sz, _int, _int, _sz],
+    'nb_mk_slot_release': [_vp, _vp],
     'nb_ks_prepared_bytes': [],
     'nb_ks_prepare': [_vp, _vp, _vp, _vp, _sz, _sz, _int, _int, _vp],
     'nb_ks_forget': [_vp, _vp],

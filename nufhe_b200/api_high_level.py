@@ -180,14 +180,18 @@ class Context:
     def make_virtual_machine(self, cloud_key: NuFHECloudKey, perf_params: PerformanceParameters = None):
         return VirtualMachine(self.thread, cloud_key, perf_params=perf_params)
 
-    def make_multi_key_machine(self, cloud_keys, perf_params: PerformanceParameters = None):
+    def make_multi_key_machine(self, cloud_keys, perf_params: PerformanceParameters = None, resident_tenants=None):
         """A MultiKeyVirtualMachine (nufhe_b200/multikey.py) for the list of cloud keys `cloud_keys`, one per tenant:
         its gates and LUTs take one operand list aligned with it and bootstrap every tenant's ciphertexts in one launch,
         bit-identical to each tenant's own VirtualMachine.  TypeError for anything but NuFHECloudKey objects, ValueError
         for keys of different parameters, multi-bit keys, single_kernel_bootstrap=False and keys the fused FP64 step
-        cannot run."""
+        cannot run.
+        resident_tenants=R (an int >= 1) takes CompressedCloudKey objects with their bodies on this context's device
+        (load_compressed_cloud_key) instead, and keeps at most R of them expanded on the device, about 164 MB each
+        (DESIGN.md section 19): an operation on more active tenants runs in rounds of at most R, with the same results.
+        TypeError for anything but CompressedCloudKey objects, ValueError for R < 1 and for the keys refused above."""
         from .multikey import MultiKeyVirtualMachine
-        return MultiKeyVirtualMachine(self.thread, cloud_keys, perf_params=perf_params)
+        return MultiKeyVirtualMachine(self.thread, cloud_keys, perf_params=perf_params, resident_tenants=resident_tenants)
 
     def load_ciphertext(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):

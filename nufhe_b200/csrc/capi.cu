@@ -29,6 +29,9 @@ struct nb_ctx {
     // multi-bit keys prepared on this context (nb_bk_prepare_multibit): 3 rows of spectra per group of two key bits,
     // which every launch with them runs on the FP64 step (begin, end of the key's rows)
     std::vector<std::pair<const u64 *, const u64 *>> multibit_keys;
+    // slots of the multi-key machine filled by nb_mk_bk_expand: engine key rows whose FP64 part only is written (their
+    // NTT planes are garbage), so only the nb_mk_* bootstraps accept them (begin, end of the slot's rows)
+    std::vector<std::pair<const u64 *, const u64 *>> mk_slots;
     int fft;                             // developer knob: 0 keeps the NTT step for every key
     int sm_count;
     size_t wide_max;                     // largest batch launched in the wide (1 ciphertext / 256 threads) shape
@@ -368,7 +371,7 @@ size_t nb_bk_multibit_row_u64(void) { return BK_FFT_U64; }
 // forget the registrations of keys that [begin, end) overwrites
 static void forget_keys(nb_ctx *ctx, const u64 *begin, const u64 *end)
 {
-    for (auto *keys : {&ctx->spectral_keys, &ctx->multibit_keys})
+    for (auto *keys : {&ctx->spectral_keys, &ctx->multibit_keys, &ctx->mk_slots})
         for (size_t i = 0; i < keys->size();) {
             if ((*keys)[i].first < end && begin < (*keys)[i].second) keys->erase(keys->begin() + i);
             else i++;
@@ -1252,7 +1255,8 @@ static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
 
 // The common part of the multi-key bootstraps: p carries everything but the keys, for a batch of jobs x sum(counts)
 // ciphertexts whose job j covers rows [j B, (j + 1) B), split into tenants by the same counts.  Every tenant's key must lie
-// inside an engine key with FP64 spectra prepared on this context, since the multi-key kernel runs the FP64 step.
+// inside an engine key with FP64 spectra prepared on this context, or inside a slot nb_mk_bk_expand filled, since the
+// multi-key kernel runs the FP64 step.  The keys are checked before an empty batch returns.
 static int mk_blind_rotate(nb_ctx *ctx, const char *what, BlindRotateArgs &p, const uint64_t *const *bk,
                            const size_t *counts, size_t tenants, size_t job_batch, int jobs)
 {
@@ -1265,10 +1269,12 @@ static int mk_blind_rotate(nb_ctx *ctx, const char *what, BlindRotateArgs &p, co
             if (k.first <= key && key < k.second)
                 return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": tenant " + std::to_string(t) + " has a multi-bit key");
         bool spectral = false;
-        for (const auto &k : ctx->spectral_keys) spectral |= k.first <= key && key + (size_t)p.n * BK_ROW_U64 <= k.second;
+        for (auto *keys : {&ctx->spectral_keys, &ctx->mk_slots})
+            for (const auto &k : *keys) spectral |= k.first <= key && key + (size_t)p.n * BK_ROW_U64 <= k.second;
         if (!spectral)
             return fail(ctx, NB_EINVAL, std::string(what) + ": the key of tenant " + std::to_string(t) +
-                                            " is not inside an engine key with FP64 spectra prepared on this context");
+                                            " is not inside an engine key with FP64 spectra prepared on this context "
+                                            "or a slot filled by nb_mk_bk_expand");
     }
     if (p.batch == 0) return NB_OK;
     // [tenant key pointers][tenant of each ciphertext]
@@ -1491,6 +1497,92 @@ int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_hos
     ntt_mac_mk_kernel<<<grid, MAC_WARPS * 32, 0, ctx->stream>>>((const u64 *)x, reinterpret_cast<const u64 *const *>(ctx->d_mk),
                                                                (u64 *)out, (u32)rows, (u32)outs);
     return launch_check(ctx, "ntt_mac_mk_kernel");
+}
+
+// ---- multi-key expansion of compressed cloud keys (DESIGN.md section 19) ----
+
+int nb_mk_bk_expand(nb_ctx *ctx, const uint32_t *seeds_host, const int32_t *const *bodies_host,
+                    uint64_t *const *slots_host, size_t tenants, size_t n, int mask_size, int decomp_length,
+                    size_t poly_degree)
+{
+    const char *what = "nb_mk_bk_expand";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!seeds_host || !bodies_host || !slots_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (mask_size != 1 || decomp_length != 2 || poly_degree != (size_t)NTT_N || n == 0 || n > (size_t)LWE_N_MAX)
+        return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the expansion is for k = 1, l = 2, N = 1024 and 1 <= n <= " +
+                                              std::to_string(LWE_N_MAX) + " only");
+    for (size_t t = 0; t < tenants; t++)
+        if (!bodies_host[t] || !slots_host[t])
+            return fail(ctx, NB_EINVAL, std::string(what) + ": null bodies or slot of tenant " + std::to_string(t));
+    if (tenants == 0) return NB_OK;
+    if (tenants * n * 8 > 0x7fffffffu) return fail(ctx, NB_EINVAL, std::string(what) + ": too many rows in one call");
+    std::vector<MkBkTenant> table(tenants);
+    for (size_t t = 0; t < tenants; t++) {
+        memcpy(table[t].seed, seeds_host + 8 * t, sizeof(table[t].seed));
+        table[t].body = bodies_host[t];
+        table[t].slot = slots_host[t];
+    }
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_bk_expand");
+    NB_TRY(mk_upload(ctx, table.data(), tenants * sizeof(MkBkTenant)));
+    mk_bk_expand_kernel<<<(unsigned)(tenants * n * 8), 64, 0, ctx->stream>>>(reinterpret_cast<const MkBkTenant *>(ctx->d_mk),
+                                                                          (u32)n, ctx->d_fft_tab);
+    NB_TRY(launch_check(ctx, "mk_bk_expand_kernel"));
+    // a slot serves the nb_mk_* bootstraps only: its NTT planes are not written
+    for (size_t t = 0; t < tenants; t++) {
+        const u64 *begin = slots_host[t], *end = begin + n * BK_ROW_U64;
+        forget_keys(ctx, begin, end);
+        ctx->mk_slots.emplace_back(begin, end);
+    }
+    return NB_OK;
+}
+
+int nb_mk_ks_expand(nb_ctx *ctx, const uint32_t *seeds_host, int32_t *const *ks_a_host, size_t tenants, size_t in_size,
+                    int t, int log2_base, size_t n)
+{
+    const char *what = "nb_mk_ks_expand";
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!seeds_host || !ks_a_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N))
+        return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the expansion is for the multi-key key switch, in = 1024, "
+                                                             "n = 500, t = 8, base 4 only");
+    for (size_t k = 0; k < tenants; k++)
+        if (!ks_a_host[k]) return fail(ctx, NB_EINVAL, std::string(what) + ": null ks_a of tenant " + std::to_string(k));
+    if (tenants == 0) return NB_OK;
+    if (tenants > 65535) return fail(ctx, NB_EINVAL, std::string(what) + ": more than 65535 tenants in one call");
+    std::vector<MkKsTenant> table(tenants);
+    for (size_t k = 0; k < tenants; k++) {
+        memcpy(table[k].seed, seeds_host + 8 * k, sizeof(table[k].seed));
+        table[k].ks_a = ks_a_host[k];
+        // GEMM planes registered for a key that lived at this address no longer describe it
+        for (size_t i = 0; i < ctx->ks_keys.size();) {
+            if (ctx->ks_keys[i].ks_a == ks_a_host[k]) ctx->ks_keys.erase(ctx->ks_keys.begin() + i);
+            else i++;
+        }
+    }
+    const u32 base = 1u << log2_base;
+    const u64 rows = (u64)in_size * t, words = rows * (base - 1) * n;
+    const u64 blocks = (words + 15) / 16, per_tenant = (blocks + MK_KS_THREADS - 1) / MK_KS_THREADS;
+    u64 ctas = (u64)ctx->sm_count * 8 / tenants;
+    if (ctas < 1) ctas = 1;
+    if (ctas > per_tenant) ctas = per_tenant;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_ks_expand");
+    NB_TRY(mk_upload(ctx, table.data(), tenants * sizeof(MkKsTenant)));
+    mk_ks_expand_kernel<<<dim3((unsigned)ctas, (unsigned)tenants), MK_KS_THREADS, 0, ctx->stream>>>(
+        reinterpret_cast<const MkKsTenant *>(ctx->d_mk), words, rows, (u32)n, base);
+    return launch_check(ctx, "mk_ks_expand_kernel");
+}
+
+int nb_mk_slot_release(nb_ctx *ctx, const uint64_t *slot)
+{
+    if (!ctx) return NB_EINVAL;
+    if (!slot) return fail(ctx, NB_EINVAL, "nb_mk_slot_release: null slot");
+    for (size_t i = 0; i < ctx->mk_slots.size();) {
+        if (ctx->mk_slots[i].first == (const u64 *)slot) ctx->mk_slots.erase(ctx->mk_slots.begin() + i);
+        else i++;
+    }
+    return NB_OK;
 }
 
 }  // extern "C"

@@ -14,6 +14,7 @@
 #include "tree_layout.cuh"
 #include "compact_layout.cuh"
 #include "mk_layout.cuh"
+#include "mk_expand_layout.cuh"
 
 using namespace nb;
 
@@ -673,6 +674,36 @@ u64 emul_mk_group_tenants(const size_t *group_counts, size_t tenants, u32 *out)
     std::vector<u32> ids(tenants);
     for (size_t t = 0; t < tenants; t++) ids[t] = (u32)t;
     return mk_group_keys(group_counts, tenants, ids.data(), out);
+}
+
+// Expansion of compressed cloud keys (mk_expand_layout.cuh).  emul_mk_bk_mask_word / emul_mk_bk_body_offset: the index
+// functions themselves.  emul_mk_bk_mask_regroup: what mk_bk_expand_kernel's 64 threads hold after the regrouping for
+// mask polynomial (i, mi, j, mo) (N = 1024): out[n0 * 16 + jj] = the value thread n0 gives bk_spectra_transform as k[jj].
+// emul_mk_ks_expand: ks_a (in, t, base, n) as mk_ks_expand_kernel writes it, every stream word and zero row in turn.
+u64 emul_mk_bk_mask_word(u64 i, u32 mi, u32 j, u32 mo, u32 k, u32 l, u32 N) { return mk_bk_mask_word(i, mi, j, mo, k, l, N); }
+u64 emul_mk_bk_body_offset(u64 i, u32 mi, u32 j, u32 k, u32 l, u32 N) { return mk_bk_body_offset(i, mi, j, k, l, N); }
+void emul_mk_bk_mask_regroup(const u32 *seed, u64 i, u32 mi, u32 j, u32 mo, u32 k, u32 l, i32 *out)
+{
+    std::vector<u32> buf(MK_REGROUP_WORDS);
+    for (int n0 = 0; n0 < 64; n0++) {
+        u32 x[16];
+        chacha20_block(seed, (mk_bk_mask_word(i, mi, j, mo, k, l, NTT_N) >> 4) + n0, MK_NONCE_BK, x);
+        for (int w = 0; w < 16; w++) buf[mk_regroup_slot(16 * n0 + w)] = x[w];
+    }
+    for (int n0 = 0; n0 < 64; n0++)
+        for (int jj = 0; jj < 16; jj++) out[n0 * 16 + jj] = (i32)buf[mk_regroup_slot(mk_spectra_coef(n0, jj))];
+}
+void emul_mk_ks_expand(const u32 *seed, size_t in_size, int t, int log2_base, size_t n, i32 *ks_a)
+{
+    const u32 base = 1u << log2_base;
+    const u64 rows = (u64)in_size * t, words = rows * (base - 1) * n;
+    for (u64 b = 0; b < (words + 15) / 16; b++) {
+        u32 x[16];
+        chacha20_block(seed, b, MK_NONCE_KS, x);
+        for (int w = 0; w < 16 && b * 16 + w < words; w++) ks_a[mk_ks_a_word(b * 16 + w, n, base)] = (i32)x[w];
+    }
+    for (u64 r = 0; r < rows; r++)
+        for (u64 c = 0; c < n; c++) ks_a[mk_ks_zero_word(r, c, n, base)] = 0;
 }
 
 // emul_tree_assemble: tree_assemble_kernel's arithmetic, one (test vector, polynomial) after the other, with a serial

@@ -28,6 +28,7 @@
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
 #include "mk_layout.cuh"
+#include "mk_expand_layout.cuh"
 
 namespace nb {
 
@@ -282,9 +283,31 @@ __global__ void bk_plain_kernel(const u64 *__restrict__ bk_ref, u64 *__restrict_
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
         plain[i] = ff_mul(ff_canon(bk_ref[i]), FF_RINV);
 }
+// The key spectra of key polynomial m of a row, for a CTA of 64 threads: thread n0 holds the centred integer
+// coefficients k[j] = coefficient 64 j + n0; they are split into 16-bit halves and both halves transformed with the
+// passes of the bootstrap into `spec`, then stored to bk_int + row * row_u64 + row_offset (fft_key_pos).
+NB_D void bk_spectra_transform(const long long (&k)[16], cplx (&spec)[2][FFT_SPEC_CPLX], const cplx *__restrict__ tab,
+                               u64 *__restrict__ bk_int, size_t row, size_t row_u64, size_t row_offset, int m, int n0)
+{
+    {
+        double lo[16], hi[16];
+        fft_split_key(k, lo, hi);
+        fft_fwd1(n0, lo, spec[0], tab);
+        fft_fwd1(n0, hi, spec[1], tab);
+    }
+    __syncthreads();
+    fft_fwd2(n0 & 7, (n0 >> 3) & 3, spec[n0 >> 5]);      // 2 x 32 tasks (h, n2, k1)
+    __syncthreads();
+    for (int t = n0; t < 2 * FFT_M / 4; t += 64) fft_fwd3(t & 127, spec[t >> 7]);
+    __syncthreads();
+    cplx *out = reinterpret_cast<cplx *>(bk_int + row * row_u64 + row_offset);
+    for (int P = n0; P < FFT_M; P += 64)
+        for (int h = 0; h < 2; h++) out[fft_key_pos(m * 2 + h, P & 127, P >> 7)] = spec[h][fft_pass3_x(fft_pass3_group(P & 127), P >> 7)];
+}
+
 // One CTA of 64 threads per key polynomial (blockIdx.x = row * 8 + m): its coefficients mod p (natural order) must be
-// centred 32-bit integers; they are split into 16-bit halves and both halves transformed with the passes of the
-// bootstrap.  A coefficient outside [-2^31, 2^31) sets *not_integral (the key then keeps the NTT step everywhere).
+// centred 32-bit integers, transformed by bk_spectra_transform.  A coefficient outside [-2^31, 2^31) sets
+// *not_integral (the key then keeps the NTT step everywhere).
 // The spectra of row r go to bk_int + r * row_u64 + row_offset: after the NTT planes of an engine key row
 // (BK_ROW_U64, BK_NTT_U64), or alone (BK_FFT_U64, 0: a multi-bit key).
 __global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ coef, u64 *__restrict__ bk_int,
@@ -305,20 +328,96 @@ __global__ void __launch_bounds__(64) bk_spectra_kernel(const u64 *__restrict__ 
         else { k[j] = 0; bad = true; }
     }
     if (bad) atomicOr(not_integral, 1);
-    {
-        double lo[16], hi[16];
-        fft_split_key(k, lo, hi);
-        fft_fwd1(n0, lo, spec[0], tab);
-        fft_fwd1(n0, hi, spec[1], tab);
+    bk_spectra_transform(k, spec, tab, bk_int, row, row_u64, row_offset, m, n0);
+}
+
+// ---- multi-key expansion of compressed cloud keys (DESIGN.md section 19; index arithmetic in mk_expand_layout.cuh)
+// One tenant of nb_mk_bk_expand: its seed, bootstrap-key bodies (n, k+1, l, N) int32 and slot (n engine key rows)
+struct MkBkTenant {
+    u32 seed[8];
+    const i32 *body;
+    u64 *slot;
+};
+
+// The FP64 part of every row of every listed slot, k = 1, l = 2, N = 1024: one CTA of 64 threads per key polynomial,
+// blockIdx.x = (tenant * n + row) * 8 + m with m = (mi * 2 + j) * 2 + mo as in bk_spectra_kernel.  A mask polynomial
+// (mo = 0) is 64 ChaCha blocks, one per thread, regrouped through shared memory (aliased onto the spectra, which are
+// written only after the regrouped words are in registers); a body polynomial (mo = 1) is read from the bodies.  The
+// coefficients are the int32 values decompress() feeds nb_bk_prepare, so the spectra are the ones it stores.  The
+// NTT planes of the rows are not written.
+__global__ void __launch_bounds__(64) mk_bk_expand_kernel(const MkBkTenant *__restrict__ tenants, u32 n,
+                                                          const cplx *__restrict__ tab)
+{
+    __shared__ __align__(16) cplx spec[2][FFT_SPEC_CPLX];
+    static_assert(MK_REGROUP_WORDS * sizeof(u32) <= sizeof(spec), "the regrouping buffer lives in the spectra");
+    const u64 poly = blockIdx.x, row_all = poly >> 3;
+    const u32 tenant = (u32)(row_all / n);
+    const u64 row = row_all - (u64)tenant * n;
+    const int m = (int)(poly & 7), n0 = threadIdx.x;
+    const u32 mi = (u32)m >> 2, j = ((u32)m >> 1) & 1, mo = (u32)m & 1;
+    const MkBkTenant &t = tenants[tenant];
+    long long k[16];
+    if (mo == 0) {
+        u32 *buf = reinterpret_cast<u32 *>(&spec[0][0]);
+        u32 seed[8], x[16];
+#pragma unroll
+        for (int i = 0; i < 8; i++) seed[i] = t.seed[i];
+        chacha20_block(seed, (mk_bk_mask_word(row, mi, j, mo, 1, 2, NTT_N) >> 4) + n0, MK_NONCE_BK, x);
+#pragma unroll
+        for (int w = 0; w < 16; w++) buf[mk_regroup_slot(16 * n0 + w)] = x[w];
+        __syncthreads();
+#pragma unroll
+        for (int jj = 0; jj < 16; jj++) k[jj] = (i32)buf[mk_regroup_slot(mk_spectra_coef(n0, jj))];
+        __syncthreads();
+    } else {
+        const i32 *body = t.body + mk_bk_body_offset(row, mi, j, 1, 2, NTT_N);
+#pragma unroll
+        for (int jj = 0; jj < 16; jj++) k[jj] = body[mk_spectra_coef(n0, jj)];
     }
-    __syncthreads();
-    fft_fwd2(n0 & 7, (n0 >> 3) & 3, spec[n0 >> 5]);      // 2 x 32 tasks (h, n2, k1)
-    __syncthreads();
-    for (int t = n0; t < 2 * FFT_M / 4; t += 64) fft_fwd3(t & 127, spec[t >> 7]);
-    __syncthreads();
-    cplx *out = reinterpret_cast<cplx *>(bk_int + row * row_u64 + row_offset);
-    for (int P = n0; P < FFT_M; P += 64)
-        for (int h = 0; h < 2; h++) out[fft_key_pos(m * 2 + h, P & 127, P >> 7)] = spec[h][fft_pass3_x(fft_pass3_group(P & 127), P >> 7)];
+    bk_spectra_transform(k, spec, tab, t.slot, row, BK_ROW_U64, BK_NTT_U64, m, n0);
+}
+
+// One tenant of nb_mk_ks_expand
+struct MkKsTenant {
+    u32 seed[8];
+    i32 *ks_a;
+};
+
+constexpr int MK_KS_THREADS = 256;
+
+// ks_a (in, t, base, n) of tenant blockIdx.y: the `words` mask words of the stream (seed, nonce 2) into rows h >= 1
+// (mk_ks_a_word), as seeded_uniform_kernel writes a stream: a lane per block, a warp's 32 blocks staged through shared
+// memory so that each store instruction writes 32 consecutive stream words; then zeros into the `zero_rows` rows h = 0.
+__global__ void __launch_bounds__(MK_KS_THREADS) mk_ks_expand_kernel(const MkKsTenant *__restrict__ tenants, u64 words,
+                                                                     u64 zero_rows, u32 n, u32 base)
+{
+    __shared__ u32 stage[MK_KS_THREADS / 32][32 * 17];
+    const int lane = threadIdx.x & 31;
+    u32 *st = stage[threadIdx.x >> 5];
+    const MkKsTenant &tt = tenants[blockIdx.y];
+    i32 *out = tt.ks_a;
+    u32 seed[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) seed[i] = tt.seed[i];
+    const u64 blocks = (words + 15) >> 4;
+    const u64 thread = (u64)blockIdx.x * blockDim.x + threadIdx.x, threads = (u64)gridDim.x * blockDim.x;
+    for (u64 wb = (thread >> 5) * 32; wb < blocks; wb += (threads >> 5) * 32) {
+        if (wb + lane < blocks) {
+            u32 x[16];
+            chacha20_block(seed, wb + lane, MK_NONCE_KS, x);
+#pragma unroll
+            for (int j = 0; j < 16; j++) st[lane * 17 + j] = x[j];
+        }
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const int idx = j * 32 + lane;
+            const u64 w = wb * 16 + idx;
+            if (w < words) out[mk_ks_a_word(w, n, base)] = (i32)st[(idx >> 4) * 17 + (idx & 15)];
+        }
+        __syncwarp();
+    }
+    for (u64 i = thread; i < zero_rows * n; i += threads) out[mk_ks_zero_word(i / n, i % n, n, base)] = 0;
 }
 
 // mod-switch to [0, 2N) (numeric_functions_gpu.py:55-71)

@@ -362,6 +362,49 @@ class Engine:
                    int(base).bit_length() - 1, _ptr(res_a), _ptr(res_b), _ptr(res_cv), B)
         return res_a, res_b, res_cv
 
+    # --- expansion of compressed cloud keys into multi-key slots (DESIGN.md section 19)
+    def mk_bk_slot(self, n):
+        """An uninitialised slot for the bootstrap key of one tenant: n engine key rows (nb_bk_row_u64() words each).
+        Its registration on this engine, which mk_bk_expand makes, is dropped when the slot is freed
+        (nb_mk_slot_release), so that memory the allocator hands out again never passes for a key."""
+        slot = self.empty((n, self.lib.nb_bk_row_u64()), torch.int64)
+        weakref.finalize(slot, self._mk_slot_release, slot.data_ptr())
+        return slot
+
+    def _mk_slot_release(self, ptr):
+        if self.handle:
+            self.lib.nb_mk_slot_release(self.handle, ctypes.c_void_p(ptr))
+
+    @staticmethod
+    def _seeds(seeds):
+        seeds = numpy.ascontiguousarray(numpy.asarray(seeds).astype(numpy.int64).astype(numpy.uint32).reshape(-1, 8))
+        return seeds, seeds.ctypes.data_as(ctypes.c_void_p)
+
+    def mk_bk_expand(self, seeds, bodies, slots, params):
+        """The FP64 part of the engine key of every listed tenant into its slot (mk_bk_slot), in one launch
+        (nb_mk_bk_expand): seeds (T, 8) of the compressed keys, bodies[t] (n, k+1, l, N) int32 on this device; the slots'
+        contents equal bk_prepare of the decompressed key's FP64 part, word for word."""
+        seeds, seeds_p = self._seeds(seeds)
+        bodies = [self._dense(b, torch.int32) for b in bodies]
+        n = params.in_out_params.size
+        for b, s in zip(bodies, slots):
+            assert b.shape[0] == n and s.is_contiguous() and s.shape == (n, self.lib.nb_bk_row_u64()), (b.shape, s.shape)
+        tl = params.tgsw_params.tlwe_params
+        self._call('nb_mk_bk_expand', seeds_p, self._host_array(ctypes.c_void_p, [b.data_ptr() for b in bodies]),
+                   self._host_array(ctypes.c_void_p, [s.data_ptr() for s in slots]), len(slots), n, tl.mask_size,
+                   params.tgsw_params.decomp_length, tl.polynomial_degree)
+
+    def mk_ks_expand(self, seeds, ks_as):
+        """The masks of every listed tenant's key-switch key into its ks_a (in, t, base, n) int32, rows h = 0 zero, in
+        one launch (nb_mk_ks_expand): byte-identical to CompressedCloudKey.decompress()'s ks_a."""
+        seeds, seeds_p = self._seeds(seeds)
+        if not ks_as:
+            return
+        in_size, t, base, n = ks_as[0].shape
+        assert all(k.is_contiguous() and k.shape == ks_as[0].shape for k in ks_as)
+        self._call('nb_mk_ks_expand', seeds_p, self._host_array(ctypes.c_void_p, [k.data_ptr() for k in ks_as]),
+                   len(ks_as), in_size, t, int(base).bit_length() - 1, n)
+
     def ks_prepare(self, ks_a, ks_b):
         """Lay a key-switch key (in = 1024, n = 500, t = 8, base 4) into the byte planes of the tensor-core key switch
         and register them for (ks_a, ks_b) on this engine (nb_ks_prepare).  Returns the planes, which must stay alive

@@ -5,11 +5,20 @@ A VirtualMachine per key would bootstrap each handful in a launch of its own, le
 MultiKeyVirtualMachine concatenates the operands of every tenant and runs one multi-key bootstrap (each ciphertext with
 its own tenant's bootstrapping key) and one multi-key key switch.  Every output is bit-identical to what that tenant's
 own VirtualMachine returns for the same operands.
+
+With `resident_tenants=R` the machine takes compressed cloud keys instead and keeps at most R of them expanded on the
+device (DESIGN.md section 19): an operation runs in rounds of at most R tenants, each round first expanding the keys it
+lacks into slots freed by the least recently used tenants.
 """
+import collections
+import functools
+import inspect
+
 import numpy
 import torch
 
 from .api_low_level import NuFHECloudKey, empty_ciphertext
+from .compressed import CompressedCloudKey
 from .gates import MU, _BINARY_GATES, check_shape, get_shape, result_shape
 from .lwe import LweSampleArray
 from .lut import LookupTable, _check_config, _check_margin, _sigma
@@ -26,6 +35,105 @@ from . import compact, gates, index_lookup, packing, tree_lut
 _KEYLESS = {'not': 1, 'copy': 1, 'constant': 1}
 
 
+def _in_rounds(operands, masked=()):
+    """Run a method of a machine on compressed keys in rounds (DESIGN.md section 19).  `operands` name the arguments
+    that hold one entry per tenant whose non-None entries make a tenant active (`digits`: a list of such lists);
+    `masked` name further per-tenant arguments.  Each round calls the method with every per-tenant argument masked to
+    the round's tenants and the round's keys in place; tenants are independent, so the rounds do not change a result.
+    A call whose per-tenant arguments are malformed goes straight to the method, which raises."""
+    def wrap(method):
+        sig = inspect.signature(method)
+
+        @functools.wraps(method)
+        def run(self, *args, **kwds):
+            if self._pool is None:
+                return method(self, *args, **kwds)
+            call = sig.bind(self, *args, **kwds)
+            T = self.tenants
+
+            def lists(name):
+                x = call.arguments.get(name)
+                if x is None or (name == 'table' and not isinstance(x, (list, tuple))):
+                    return []
+                return list(x) if name == 'digits' else [x]
+            per_tenant = [x for name in operands + masked for x in lists(name)]
+            if any(not isinstance(x, (list, tuple)) or len(x) != T for x in per_tenant):
+                return method(self, *args, **kwds)
+            active = [t for t in range(T) if any(x[t] is not None for name in operands for x in lists(name))]
+            out = [None] * T
+            for keep in self._pool.rounds(active):
+                self._pool.fill(self, keep)
+                keep = set(keep)
+                masked_call = sig.bind(self, *args, **kwds)
+                for name in operands + masked:
+                    x = masked_call.arguments.get(name)
+                    if not lists(name):
+                        continue
+                    mask = lambda lst: [v if t in keep else None for t, v in enumerate(lst)]
+                    masked_call.arguments[name] = [mask(d) for d in x] if name == 'digits' else mask(x)
+                res = method(*masked_call.args, **masked_call.kwargs)
+                for t in keep:
+                    out[t] = res[t]
+            return out
+        return run
+    return wrap
+
+
+class _SlotPool:
+    """The expanded keys of a machine on compressed cloud keys: at most R slots, each the engine-row bootstrap key
+    (FP64 part only) and the key-switch masks of one tenant, allocated lazily and reused in least-recently-used order.
+    While a round runs, the machine's per-tenant key lists point at the round's slots.  The pool holds no reference to
+    its machine, so the slots go with the machine."""
+
+    def __init__(self, keys, R):
+        self.keys = keys
+        self.R = R
+        self.lru = collections.OrderedDict()           # tenant -> (bk slot, ks_a), least recently used first
+        self.slots = 0
+        # ks_cv of decompress(): 0 for rows h = 0, the key's variance elsewhere; one per distinct variance
+        self.ks_cv = {}
+        for key in keys:
+            if key.ks_variance not in self.ks_cv:
+                cv = torch.zeros(tuple(key.ks_b.shape), dtype=torch.float32, device=key.ks_b.device)
+                cv[:, :, 1:] = key.ks_variance
+                self.ks_cv[key.ks_variance] = cv
+
+    def rounds(self, active):
+        """The active tenants that hold a slot, in tenant order, then the others, R at a time."""
+        order = [t for t in active if t in self.lru] + [t for t in active if t not in self.lru]
+        return [order[i:i + self.R] for i in range(0, len(order), self.R)]
+
+    def fill(self, m, tenants):
+        """Expand the keys of `tenants` (at most R) that hold no slot, evicting the least recently used tenants outside
+        them, with one launch for the bootstrap keys and one for the key-switch keys; mark the round's tenants most
+        recently used, in tenant order; then point the machine's key lists at the round's slots."""
+        thr = m.thread
+        missing = [t for t in tenants if t not in self.lru]
+        if missing:
+            keep = set(tenants)
+            victims = [t for t in self.lru if t not in keep]
+            slots = []
+            for _ in missing:
+                if self.slots < self.R:
+                    in_size, t_, base = self.keys[0].ks_b.shape
+                    slots.append((thr.mk_bk_slot(m.params.in_out_params.size),
+                                  thr.empty((in_size, t_, base, m.params.in_out_params.size), torch.int32)))
+                    self.slots += 1
+                else:
+                    slots.append(self.lru.pop(victims.pop(0)))
+            seeds = numpy.stack([self.keys[t].seed for t in missing])
+            thr.mk_bk_expand(seeds, [self.keys[t].bk_body for t in missing], [s[0] for s in slots], m.params)
+            thr.mk_ks_expand(seeds, [s[1] for s in slots])
+            for t, slot in zip(missing, slots):
+                self.lru[t] = slot
+        for t in sorted(tenants):                     # the round's tenants become the most recently used
+            self.lru.move_to_end(t)
+        first = self.lru[tenants[0]]
+        m._bk_ints = [self.lru.get(t, first)[0] for t in range(m.tenants)]
+        m._ks = [(self.lru.get(t, first)[1], self.keys[t].ks_b, self.ks_cv[self.keys[t].ks_variance])
+                 for t in range(m.tenants)]
+
+
 class MultiKeyVirtualMachine:
     """Executes gates, LUTs, tree LUTs, packing, expansion and index lookups on the ciphertexts of several cloud keys at
     once.
@@ -34,13 +142,20 @@ class MultiKeyVirtualMachine:
     tenant as VirtualMachine does), or None when tenant t has no work, in which case all its operands must be None.
     The result is a list aligned the same way (None for idle tenants).
 
+    With `resident_tenants=R` every key is a CompressedCloudKey with its bodies on the machine's device, and at most R
+    tenants hold expanded keys at a time (DESIGN.md section 19); the results are the same.
+
     .. method:: gate_<operator>(*operand_lists, dest=None)
     """
 
-    def __init__(self, thread, cloud_keys, perf_params: PerformanceParameters = None):
+    def __init__(self, thread, cloud_keys, perf_params: PerformanceParameters = None, resident_tenants=None):
         cloud_keys = list(cloud_keys)
         if not cloud_keys:
             raise ValueError('a multi-key machine needs at least one cloud key')
+        self._pool = None
+        if resident_tenants is not None:
+            self._init_pool(thread, cloud_keys, perf_params, resident_tenants)
+            return
         for t, key in enumerate(cloud_keys):
             if not isinstance(key, NuFHECloudKey):
                 raise TypeError('tenant %d: a multi-key machine takes NuFHECloudKey objects (decompress a compressed key '
@@ -73,9 +188,45 @@ class MultiKeyVirtualMachine:
         except ValueError as e:
             raise ValueError('a cloud key cannot run in a multi-key launch: %s' % e) from None
 
+    def _init_pool(self, thread, keys, perf_params, R):
+        if isinstance(R, bool) or not isinstance(R, (int, numpy.integer)):
+            raise TypeError('resident_tenants must be an int, got %s' % type(R).__name__)
+        if R < 1:
+            raise ValueError('resident_tenants must be at least 1, got %d' % R)
+        for t, key in enumerate(keys):
+            if not isinstance(key, CompressedCloudKey):
+                raise TypeError('tenant %d: a multi-key machine with resident_tenants takes CompressedCloudKey objects '
+                                '(ctx.load_compressed_cloud_key), got %s' % (t, type(key).__name__))
+        params = keys[0].params
+        pp = (perf_params if perf_params is not None else PerformanceParameters(params)).for_device(thread.device_params)
+        n = params.in_out_params.size
+        for t, key in enumerate(keys):
+            if key.params != params:
+                raise ValueError('tenant %d: the cloud key was made for other parameters than tenant 0\'s' % t)
+            if key.bk_body.shape[0] != n:
+                raise ValueError('tenant %d: multi-bit bootstrap keys are not supported by the multi-key machine' % t)
+            if not pp.single_kernel_bootstrap or not fused_kernel_supported(params.tgsw_params):
+                raise ValueError('tenant %d: the multi-key machine runs the fused bootstrap only (single_kernel_bootstrap=True, '
+                                 'tlwe_mask_size=1)' % t)
+            if key.bk_body.device != thread.device or key.ks_b.device != thread.device:
+                raise ValueError('tenant %d: the compressed key\'s bodies are on %s, not on the machine\'s device %s'
+                                 % (t, key.bk_body.device, thread.device))
+        self.thread = thread
+        self.params = params
+        self.cloud_keys = keys
+        self.perf_params = pp
+        self._bk_ints = self._ks = None        # the keys of the current round (_SlotPool.fill)
+        self._pool = _SlotPool(keys, int(R))
+
     @property
     def tenants(self):
         return len(self.cloud_keys)
+
+    @property
+    def resident(self):
+        """The tenants whose keys are expanded on the device, least recently used first (resident_tenants mode; every
+        tenant otherwise)."""
+        return list(range(self.tenants)) if self._pool is None else list(self._pool.lru)
 
     def empty_ciphertext(self, shape):
         return empty_ciphertext(self.thread, self.params, shape)
@@ -150,6 +301,7 @@ class MultiKeyVirtualMachine:
         return out
 
     # --- gates ---------------------------------------------------------------------------------
+    @_in_rounds(('a', 'b'), ('dest',))
     def _binary(self, name, a, b, dest):
         active, shapes = self._active((a, b), dest)
         if not active:
@@ -160,6 +312,7 @@ class MultiKeyVirtualMachine:
                                                phase_to_t32(num, den), sa, sb, MU, self._bk_ints, counts)
         return self._results(self._keyswitch(counts, ext), active, shapes, counts, dest)
 
+    @_in_rounds(('a', 'b', 'c'), ('dest',))
     def _mux(self, a, b, c, dest):
         active, shapes = self._active((a, b, c), dest)
         if not active:
@@ -229,6 +382,7 @@ class MultiKeyVirtualMachine:
                                  % (t, (ref.bits, ref.log2_outputs, ref.out), (table.bits, table.log2_outputs, table.out)))
         return ref
 
+    @_in_rounds(('xs', 'ys'), ('table', 'dest'))
     def lut(self, table, xs, ys=None, shift=0, dest=None):
         """f(x), or f(x * 2^shift + y), for every tenant's ciphertexts with one LookupTable (VirtualMachine.make_lut)
         shared by all tenants, or a list of one table per tenant (None for idle tenants), all with the same bits,
@@ -262,10 +416,10 @@ class MultiKeyVirtualMachine:
         active, shapes = self._active(operand_lists, None if dest_lists is None else
                                       [None if d is None else d[0] for d in dest_lists])
         # the noise rule of VirtualMachine.lut (every tenant has the same parameters)
-        bk, ks = self.cloud_keys[0].bootstrap_key, self.cloud_keys[0].keyswitch_key
+        p = self.params
         sh = None if ys is None else shift
         _check_config(table.bits, L, sh)
-        _check_margin(_sigma(bk.in_out_params, bk.bk_params, ks.decomp_length, ks.log2_base, L, sh), table.bits, L, sh)
+        _check_margin(_sigma(p.in_out_params, p.tgsw_params, p.ks_decomp_length, p.ks_log2_base, L, sh), table.bits, L, sh)
         out = [None] * self.tenants
         if not active:
             return out
@@ -327,6 +481,7 @@ class MultiKeyVirtualMachine:
                 raise ValueError('tenant %d: %s writes %d results, got %d' % (t, what, K, len(out[t])))
         return out
 
+    @_in_rounds(('digits',), ('tree_keys', 'dest'))
     def lut_tree(self, tree_keys, table, digits, dest=None):
         """f(d_{D-1}, ..., d_0) for every tenant (VirtualMachine.lut_tree): `digits` is a list of D operand lists
         (highest digit first), `tree_keys` the list of the tenants' NuFHETreeKeys (None for idle tenants), `table` one
@@ -475,6 +630,7 @@ class MultiKeyVirtualMachine:
             g0 += g
         return out
 
+    @_in_rounds(('compacts',))
     def expand(self, compacts):
         """The LweSampleArrays of every tenant's compact ciphertexts (VirtualMachine.expand): one extraction over all
         tenants' groups, then one multi-key key switch, a few groups per pass (compact.PASS_BYTES).  A list aligned with
@@ -528,6 +684,7 @@ class MultiKeyVirtualMachine:
             row += c
         return out
 
+    @_in_rounds(('indexes',), ('dest',))
     def lookup(self, indexes, table, dest=None):
         """table[idx] for every tenant's EncryptedIndexArray (VirtualMachine.lookup) with one IndexTable shared by all
         tenants: the queries of all tenants go through one CMux tree and rotation per pass, then one multi-key key
