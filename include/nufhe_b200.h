@@ -364,6 +364,19 @@ int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_st
                             size_t sel_query_stride, int bits, size_t columns, int32_t *out_a, int32_t *out_b,
                             size_t queries);
 
+/* The same two levels with one table per query (encrypted tables, DESIGN.md section 20): `tables` holds table_count
+ * tables, table_stride int32 words apart, and query q reads table table_ids_host[q] (a host array of `queries` entries,
+ * uploaded by the call) where the calls above read in + q in_query_stride.  They serve the level that first reads a
+ * table: nb_index_cmux_level_indirect for bits > 10 (each table 2 nodes GLWE samples), nb_index_rotate_extract_indirect
+ * for bits <= 10 (each table `columns` accumulators for bits = 10, one below).  NB_EINVAL as above, and for an id
+ * >= table_count or a stride shorter than a table. */
+int nb_index_cmux_level_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
+                                 const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
+                                 int32_t *out, size_t nodes, size_t queries);
+int nb_index_rotate_extract_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
+                                     const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
+                                     int bits, size_t columns, int32_t *out_a, int32_t *out_b, size_t queries);
+
 /* ---- compact public-key encryption (DESIGN.md section 16; no reference counterpart).  B messages go into
  * G = ceil(B / 1024) GLWE samples under the bootstrap key's GLWE key S (k + 1 polynomials of N = 1024 coefficients),
  * message c in group c / 1024, slot c % 1024, every coefficient rounded to 16 bits.  Encryption: nb_ntt_forward_i32 of

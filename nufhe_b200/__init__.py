@@ -74,7 +74,10 @@ from .index_lookup import (
     EncryptedIndexArray,
     CompressedEncryptedIndexArray,
     IndexTable,
+    EncryptedIndexTable,
     encrypt_index,
+    encrypt_table,
+    make_encrypted_table,
     lookup,
     )
 from .multikey import MultiKeyVirtualMachine

@@ -85,6 +85,8 @@ SIGNATURES = {
     'nb_index_prepare': [_vp, _vp, _sz, _vp],
     'nb_index_cmux_level': [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _sz],
     'nb_index_rotate_extract': [_vp, _vp, _sz, _vp, _sz, _int, _sz, _vp, _vp, _sz],
+    'nb_index_cmux_level_indirect': [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _sz, _sz],
+    'nb_index_rotate_extract_indirect': [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _int, _sz, _vp, _vp, _sz],
     'nb_compact_finish': [_vp, _vp, _vp, _vp, _vp, _int, _vp, _sz],
     'nb_compact_extract': [_vp, _vp, _int, _vp, _vp, _sz],
 }

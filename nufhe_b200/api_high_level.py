@@ -12,8 +12,8 @@ from .compact import NuFHECompactPublicKey, CompactLweSampleArray, expand
 from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
                       decrypt_packed, decrypt_packed_int)
 from .tree_lut import NuFHETreeKey, TreeLookupTable, lut_tree
-from .index_lookup import (NuFHEIndexSecretKey, IndexTable, encrypt_index, load_encrypted_index, lookup,
-                           _check_params as check_index_params)
+from .index_lookup import (NuFHEIndexSecretKey, IndexTable, EncryptedIndexTable, encrypt_index, encrypt_table,
+                           make_encrypted_table, load_encrypted_index, lookup, _check_params as check_index_params)
 from .random_numbers import DeterministicRNG
 from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
@@ -140,6 +140,13 @@ class Context:
         `decompress()` to compute).  ValueError for bits or values out of range."""
         return encrypt_index(self.thread, self.rng, index_key, values, bits, compressed=compressed)
 
+    def encrypt_table(self, key, table, out='int', bits=None):
+        """An EncryptedIndexTable of `table` (shape (2^m,) or (W, 2^m), as make_index_table) for VirtualMachine.lookup:
+        the server stores it and reads it by encrypted index without learning any entry.  `key` is a
+        NuFHECompactPublicKey (whoever holds it can upload a table) or the owner's NuFHEIndexSecretKey; 4 bytes per
+        entry.  TypeError for any other key, ValueError for a table or bit count out of range."""
+        return encrypt_table(self.thread, self.rng, key, table, out=out, bits=bits)
+
     def make_public_key(self, secret_key: NuFHESecretKey):
         """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
         return NuFHEPublicKey.from_secret_key(self.thread, self.rng, secret_key)
@@ -254,6 +261,11 @@ class Context:
             file_or_bytestring = io.BytesIO(file_or_bytestring)
         return load_encrypted_index(file_or_bytestring, self.thread)
 
+    def load_encrypted_table(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return EncryptedIndexTable.loads(file_or_bytestring, self.thread)
+        return EncryptedIndexTable.load(file_or_bytestring, self.thread)
+
     def load_secret_key(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
             return NuFHESecretKey.loads(file_or_bytestring, self.thread)
@@ -353,11 +365,18 @@ class VirtualMachine:
         decrypt_int), out='bool' as gate bits."""
         return IndexTable(self.thread, self.params, table, out=out, bits=bits)
 
+    def make_encrypted_table(self, tree_key: NuFHETreeKey, columns, out='int', bits=None):
+        """An EncryptedIndexTable whose entries are ciphertexts this machine computed: `columns` is an LweSampleArray of
+        shape (2^m,) or (W, 2^m), or a list of W of shape (2^m,), packed under the bootstrap key's GLWE key with the
+        tree key (DESIGN.md section 20).  `out` / `bits` say how the entries are encoded (gate bits, or `bits`-bit
+        integers).  TypeError unless tree_key is a NuFHETreeKey, ValueError for other parameters or shapes."""
+        return make_encrypted_table(self.thread, self.params, tree_key, columns, out=out, bits=bits)
+
     def lookup(self, index, table, dest=None):
-        """table[idx] for every index of the EncryptedIndexArray `index`: one ciphertext array of the index's shape, or a
-        list of W for a table of W columns.  CMux gates only, no bootstrap (DESIGN.md section 15).  TypeError for
-        anything but an EncryptedIndexArray (decompress a compressed one first), ValueError for other parameters or a
-        bit count other than the table's."""
+        """table[idx] for every index of the EncryptedIndexArray `index` in an IndexTable or EncryptedIndexTable: one
+        ciphertext array of the index's shape, or a list of W for a table of W columns.  CMux gates only, no bootstrap
+        (DESIGN.md sections 15 and 20).  TypeError for anything but an EncryptedIndexArray (decompress a compressed one
+        first), ValueError for other parameters or a bit count other than the table's."""
         return lookup(self.thread, self.cloud_key.keyswitch_key, index, table, dest=dest)
 
     def int_add(self, x, y, dest=None):

@@ -199,7 +199,8 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check_resident<BrFft>(ctx));
     NB_TRY((check_resident<BrFft, true>(ctx)));
     NB_TRY(check_resident<BrFftMk>(ctx));
-    for (auto kernel : {index_lookup_kernel<false>, index_lookup_kernel<true>})
+    for (auto kernel : {index_lookup_kernel<false>, index_lookup_kernel<true>, index_lookup_kernel<false, true>,
+                        index_lookup_kernel<true, true>})
         NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<BrFft>()),
                      "cudaFuncSetAttribute(index_lookup)"));
     {   // batches that fit one wave of wide CTAs (one ciphertext on 256 threads) take the low-latency shape
@@ -678,6 +679,13 @@ static const uint8_t *ks_gemm_planes(nb_ctx *ctx, const int32_t *src1_a, const i
     return planes;
 }
 
+// copy `bytes` of host data into the context's multi-key scratch (stream-ordered after every earlier launch that reads it)
+static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
+{
+    NB_TRY(reserve_words(ctx, &ctx->d_mk, &ctx->mk_bytes, bytes, 1));
+    return check(ctx, cudaMemcpyAsync(ctx->d_mk, host, bytes, cudaMemcpyHostToDevice, ctx->stream), "cudaMemcpyAsync(multi-key tables)");
+}
+
 extern "C" {
 
 int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, const int32_t *src2_a,
@@ -1151,17 +1159,34 @@ int nb_index_prepare(nb_ctx *ctx, const int32_t *ggsw, size_t rows, uint64_t *sp
     return NB_OK;
 }
 
-static int index_launch(nb_ctx *ctx, IndexArgs &p, bool rotate, const char *what)
+static int index_launch(nb_ctx *ctx, IndexArgs &p, bool rotate, const char *what, const uint32_t *table_ids_host = nullptr,
+                        size_t tables = 0)
 {
     p.items = p.queries * p.nodes;
     const size_t ctas = (p.items + BrFft::CT - 1) / BrFft::CT;
     if (p.nodes > ((size_t)1 << 40) / p.queries || ctas > 0x7fffffffu)
         return fail(ctx, NB_EINVAL, std::string(what) + ": too many items");
+    if (table_ids_host)
+        for (size_t q = 0; q < p.queries; q++)
+            if (table_ids_host[q] >= tables)
+                return fail(ctx, NB_EINVAL, std::string(what) + ": query " + std::to_string(q) + " names table " +
+                                                std::to_string(table_ids_host[q]) + " of " + std::to_string(tables));
     NB_ON_DEVICE(ctx);
-    NvtxRange nvtx_range(rotate ? "nufhe_b200:index_rotate_extract" : "nufhe_b200:index_cmux_level");
+    NvtxRange nvtx_range(rotate ? (table_ids_host ? "nufhe_b200:index_rotate_extract_indirect" : "nufhe_b200:index_rotate_extract")
+                                : (table_ids_host ? "nufhe_b200:index_cmux_level_indirect" : "nufhe_b200:index_cmux_level"));
     p.fft_tab = ctx->d_fft_tab;
-    if (rotate) index_lookup_kernel<true><<<(unsigned)ctas, BrFft::THREADS, br_smem_bytes<BrFft>(), ctx->stream>>>(p);
-    else index_lookup_kernel<false><<<(unsigned)ctas, BrFft::THREADS, br_smem_bytes<BrFft>(), ctx->stream>>>(p);
+    const dim3 grid((unsigned)ctas);
+    const size_t smem = br_smem_bytes<BrFft>();
+    if (table_ids_host) {
+        NB_TRY(mk_upload(ctx, table_ids_host, p.queries * sizeof(u32)));
+        p.table_id = reinterpret_cast<const u32 *>(ctx->d_mk);
+        if (rotate) index_lookup_kernel<true, true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
+        else index_lookup_kernel<false, true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
+    } else if (rotate) {
+        index_lookup_kernel<true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
+    } else {
+        index_lookup_kernel<false><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
+    }
     return launch_check(ctx, what);
 }
 
@@ -1195,6 +1220,43 @@ int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_st
     p.steps = bits < 10 ? bits : 10;
     p.log2_stride = bits;
     return index_launch(ctx, p, true, "nb_index_rotate_extract");
+}
+
+int nb_index_cmux_level_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
+                                 const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
+                                 int32_t *out, size_t nodes, size_t queries)
+{
+    const char *what = "nb_index_cmux_level_indirect";
+    if (!ctx) return NB_EINVAL;
+    if (!tables || !table_ids_host || !sel || !out) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (table_stride < 4 * nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
+    if (nodes == 0 || queries == 0) return NB_OK;
+    IndexArgs p{};
+    p.in = tables; p.in_stride = table_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out = out; p.nodes = nodes; p.queries = queries;
+    return index_launch(ctx, p, false, what, table_ids_host, table_count);
+}
+
+int nb_index_rotate_extract_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
+                                     const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
+                                     int bits, size_t columns, int32_t *out_a, int32_t *out_b, size_t queries)
+{
+    const char *what = "nb_index_rotate_extract_indirect";
+    if (!ctx) return NB_EINVAL;
+    if (!tables || !table_ids_host || !sel || !out_a || !out_b) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
+    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    IndexArgs p{};
+    p.nodes = bits >= 10 ? columns : 1;
+    if (table_stride < 2 * p.nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
+    if (queries == 0) return NB_OK;
+    p.in = tables; p.in_stride = table_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out_a = out_a; p.out_b = out_b; p.queries = queries;
+    p.samples = bits >= 10 ? 1 : (int)columns;
+    p.steps = bits < 10 ? bits : 10;
+    p.log2_stride = bits;
+    return index_launch(ctx, p, true, what, table_ids_host, table_count);
 }
 
 // ---- compact public-key encryption (compact.cuh) ----
@@ -1244,13 +1306,6 @@ static int mk_check_counts(nb_ctx *ctx, const char *what, const size_t *counts, 
         return fail(ctx, NB_EINVAL, std::string(what) + ": the counts add up to " + std::to_string(sum) + ", not the batch " +
                                         std::to_string(batch));
     return NB_OK;
-}
-
-// copy `bytes` of host data into the context's multi-key scratch (stream-ordered after every earlier launch that reads it)
-static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
-{
-    NB_TRY(reserve_words(ctx, &ctx->d_mk, &ctx->mk_bytes, bytes, 1));
-    return check(ctx, cudaMemcpyAsync(ctx->d_mk, host, bytes, cudaMemcpyHostToDevice, ctx->stream), "cudaMemcpyAsync(multi-key tables)");
 }
 
 // The common part of the multi-key bootstraps: p carries everything but the keys, for a batch of jobs x sum(counts)

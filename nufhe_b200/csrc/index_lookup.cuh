@@ -8,6 +8,9 @@
 //   * CMux level: out[q][i] = in[q][2i] + C_j(q) [x] (in[q][2i+1] - in[q][2i]), one node per slot.
 //   * rotation + extraction: ACC <- ACC + C_j(q) [x] ((X^(-2^j) - 1) ACC) for j < min(m, 10), then sample extraction
 //     at coefficients w 2^m (m < 10) or 0 (m >= 10).
+// With INDIRECT, the level that first reads a table takes one table per query (the multi-key machine's per-tenant
+// encrypted tables, DESIGN.md section 20): query q reads its input at table_id[q] in_stride words from `in` instead of
+// q in_stride.  Every other level and the existing instantiations read as before.
 // Both round the gadget decomposition (fwd1 with ROUND = DIGIT_ROUND = 2^11) where the bootstrap truncates.  With
 // truncated digits every CMux whose selector bit is 1 shifts the phase by about -2^11 (1 + HW(S)) in 32-bit units,
 // -2.4e-4 of the torus, and those shifts add up coherently along a lookup's m CMuxes (DESIGN.md section 15).
@@ -38,7 +41,16 @@ struct IndexArgs {
     int steps;              // rotation: min(m, 10)
     int log2_stride;        // rotation: m, the distance between extracted coefficients
     int samples;            // rotation: samples extracted per accumulator
+    const u32 *table_id;    // INDIRECT: the table of each query, in_stride words apart from `in`
 };
+
+// the int32 words from p.in to the inputs of query q
+template <bool INDIRECT>
+NB_D size_t index_query_offset(const IndexArgs &p, size_t q)
+{
+    if constexpr (INDIRECT) return (size_t)p.table_id[q] * p.in_stride;
+    else return q * p.in_stride;
+}
 
 // the FP64 step (as br_fft_step) with a per-thread key row: the spectra of the selector of the slot this thread's
 // pass-3 task belongs to
@@ -63,7 +75,7 @@ NB_D void index_fft_step(const Br2Smem &s, const cplx *__restrict__ key, const i
 }
 
 // One CTA per two items (item = q * nodes + i); a slot beyond the batch replays the last item and stores nothing.
-template <bool ROTATE>
+template <bool ROTATE, bool INDIRECT = false>
 __global__ void __launch_bounds__(BrFft::THREADS, BrFft::CTAS_PER_SM) index_lookup_kernel(IndexArgs p)
 {
     using Cfg = BrFft;
@@ -80,7 +92,7 @@ __global__ void __launch_bounds__(BrFft::THREADS, BrFft::CTAS_PER_SM) index_look
         // the difference of the node pair
         for (int e = tid; e < ACC_WORDS; e += Cfg::THREADS) {
             const size_t it = item_of(e >> 11), q = it / p.nodes, i = it - q * p.nodes;
-            const i32 *d0 = p.in + q * p.in_stride + 2 * i * 2 * NTT_N;
+            const i32 *d0 = p.in + index_query_offset<INDIRECT>(p, q) + 2 * i * 2 * NTT_N;
             const int x = e & (2 * NTT_N - 1);
             s.acc[e] = (i32)((u32)d0[2 * NTT_N + x] - (u32)d0[x]);
         }
@@ -91,14 +103,14 @@ __global__ void __launch_bounds__(BrFft::THREADS, BrFft::CTAS_PER_SM) index_look
             const size_t it = item0 + (e >> 11);
             if (it >= p.items) continue;
             const size_t q = it / p.nodes, i = it - q * p.nodes;
-            const i32 *d0 = p.in + q * p.in_stride + 2 * i * 2 * NTT_N;
+            const i32 *d0 = p.in + index_query_offset<INDIRECT>(p, q) + 2 * i * 2 * NTT_N;
             const int x = e & (2 * NTT_N - 1);
             p.out[it * 2 * NTT_N + x] = (i32)((u32)s.acc[e] + (u32)d0[x]);
         }
     } else {
         for (int e = tid; e < ACC_WORDS; e += Cfg::THREADS) {
             const size_t it = item_of(e >> 11), q = it / p.nodes, c = it - q * p.nodes;
-            s.acc[e] = p.in[q * p.in_stride + c * 2 * NTT_N + (e & (2 * NTT_N - 1))];
+            s.acc[e] = p.in[index_query_offset<INDIRECT>(p, q) + c * 2 * NTT_N + (e & (2 * NTT_N - 1))];
         }
         for (int j = 0; j < p.steps; j++) {
             if (tid < Cfg::CT) s.rot[tid] = 2 * NTT_N - (1 << j);

@@ -743,6 +743,46 @@ class Engine:
                        _ptr(out_b), queries)
         return out_a, out_b
 
+    @staticmethod
+    def _index_tables(tables, table_ids, queries, what):
+        """(tables per call, nodes per table, stride, ids): tables (T, nodes, 2, N), table_ids (queries,) < T."""
+        ids = numpy.ascontiguousarray(table_ids, numpy.uint32).reshape(-1)
+        if tables.dim() != 4 or tables.shape[-2:] != (2, N) or ids.size != queries:
+            raise ValueError('%s: tables %s and %d table ids for %d queries' % (what, tuple(tables.shape), ids.size, queries))
+        return tables.shape[0], tables.shape[1], tables.shape[1] * 2 * N, ids
+
+    def index_cmux_level_indirect(self, tables, table_ids, sel, bit, queries):
+        """index_cmux_level with query q reading tables[table_ids[q]] (nb_index_cmux_level_indirect): tables
+        (T, 2 nodes, 2, N), table_ids a host array of `queries` ids.  Returns (queries, nodes, 2, N)."""
+        tables = self._dense(tables, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        count, pairs, stride, ids = self._index_tables(tables, table_ids, queries, 'index_cmux_level_indirect')
+        if pairs % 2:
+            raise ValueError('index_cmux_level_indirect: an odd node count %d' % pairs)
+        sp, sstride = self._index_sel(sel, bit, queries, 'index_cmux_level_indirect')
+        out = self.empty((queries, pairs // 2, 2, N), torch.int32)
+        if queries and pairs:
+            self._call('nb_index_cmux_level_indirect', _ptr(tables), stride, count, ids.ctypes.data_as(ctypes.c_void_p),
+                       sp, sstride, _ptr(out), pairs // 2, queries)
+        return out
+
+    def index_rotate_extract_indirect(self, tables, table_ids, sel, bits, columns, queries):
+        """index_rotate_extract with query q reading tables[table_ids[q]] (nb_index_rotate_extract_indirect): tables
+        (T, A, 2, N), A = columns for bits >= 10, else 1.  Returns a (columns, queries, N) and b (columns, queries)."""
+        tables = self._dense(tables, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        count, accs, stride, ids = self._index_tables(tables, table_ids, queries, 'index_rotate_extract_indirect')
+        if accs != (columns if bits >= 10 else 1) or sel.dim() != 3 or sel.shape[1] != bits:
+            raise ValueError('index_rotate_extract_indirect: %d accumulators and %s selector spectra for %d columns of %d '
+                             'bits' % (accs, tuple(sel.shape), columns, bits))
+        sp, sstride = self._index_sel(sel, 0, queries, 'index_rotate_extract_indirect')
+        out_a, out_b = self.empty((columns, queries, N), torch.int32), self.empty((columns, queries), torch.int32)
+        if queries:
+            self._call('nb_index_rotate_extract_indirect', _ptr(tables), stride, count,
+                       ids.ctypes.data_as(ctypes.c_void_p), sp, sstride, int(bits), columns, _ptr(out_a), _ptr(out_b),
+                       queries)
+        return out_a, out_b
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()

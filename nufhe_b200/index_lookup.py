@@ -23,13 +23,13 @@ import numpy
 import torch
 
 from .lwe import LweSampleArray
-from .tlwe import TLweKey, tlwe_encrypt_zero_with_masks
+from .tlwe import TLweKey, TLweSampleArray, tlwe_encrypt_zero, tlwe_encrypt_zero_with_masks
 from .tgsw import TGswKey, TGswSampleArray, tgsw_encrypt_int
 from .polynomials import IntPolynomialArray
-from .compressed import draw_seed, _check_tag, _variance, tgsw_add_message_seeded
+from .compressed import draw_seed, _check_tag, _variance, _wrap32, tgsw_add_message_seeded
 from .random_numbers import rand_gaussian_torus32
 from .gates import MU
-from . import lut
+from . import compact, lut, packing
 
 NONCE_INDEX = 6
 MAX_BITS = 20
@@ -44,6 +44,7 @@ PASS_BYTES = 2 << 30
 _SECRET_KEY_TAG = 'nufhe_b200.NuFHEIndexSecretKey/1'
 _INDEX_TAG = 'nufhe_b200.EncryptedIndexArray/1'
 _COMPRESSED_INDEX_TAG = 'nufhe_b200.CompressedEncryptedIndexArray/1'
+_ENCRYPTED_TABLE_TAG = 'nufhe_b200.EncryptedIndexTable/1'
 
 
 def _check_params(params):
@@ -96,6 +97,34 @@ def extracted_variance(params, m):
 
 def output_variance(params, m):
     return extracted_variance(params, m) + keyswitch_variance(params)
+
+
+def rounding_variance(params):
+    """The 16-bit rounding of a stored GLWE leaf: the k N mask coefficients, each multiplied by a key bit, and the body,
+    (k N / 2 + 1) 2^-32 / 12 (9.9e-9)."""
+    tl = params.tgsw_params.tlwe_params
+    return (tl.mask_size * tl.polynomial_degree / 2 + 1) * 2.0**-32 / 12
+
+
+def packing_variance(params):
+    """What packing LWE samples into a leaf adds (DESIGN.md section 12, with the tree key in place of the packing key):
+    the key noise n t N E[d^2] sigma^2, the 16-bit rounding of the input masks (n / 2) 2^-32 / 12 and the rounding of
+    the leaf (3.03e-7)."""
+    tl = params.tgsw_params.tlwe_params
+    n = params.in_out_params.size
+    e_d2 = (2**(2 * packing.PACK_LOG2_BASE) - 1) / 12 + 0.25        # digits uniform in [-128, 127]
+    key = n * packing.PACK_LEVELS * tl.polynomial_degree * e_d2 * tl.min_noise**2
+    return key + n / 2 * 2.0**-32 / 12 + rounding_variance(params)
+
+
+def lut_input_sigma(params, leaf_variance, m, log2_outputs=0, shift=None):
+    """Standard deviation of the rounded phase of a vm.lut input made of results of an m-bit lookup whose leaves carry
+    `leaf_variance`: lut.lut_sigma (measured where larger) plus whatever such a result carries beyond a LUT output,
+    weighted as the LUT weights its inputs.  For packed leaves (a LUT or gate output plus packing_variance) every
+    configuration of lut.ALLOWED keeps lut.MARGIN_SIGMAS (DESIGN.md section 20)."""
+    extra = max(0.0, leaf_variance + output_variance(params, m) - lut.bootstrap_variance(params))
+    weight = 1 if shift is None else 4**shift + 1
+    return (lut.lut_sigma(params, log2_outputs, shift)**2 + weight * extra)**0.5
 
 
 def output_sigma(params, m):
@@ -321,54 +350,213 @@ def encrypt_index(thr, rng, key: NuFHEIndexSecretKey, values, bits, compressed=F
 
 # ---------------------------------------------------------------- tables and lookups
 
+def _table_shape(shape):
+    """(W, m) of a table of shape (2^m,) or (W, 2^m), with the caps of the layout (ValueError otherwise)."""
+    if len(shape) not in (1, 2) or (len(shape) == 2 and shape[0] < 1):
+        raise ValueError('a table has shape (2^m,) or (W, 2^m), got %s' % (tuple(shape),))
+    W, size = (1,) + tuple(shape) if len(shape) == 1 else tuple(shape)
+    m = int(size).bit_length() - 1
+    if size != 1 << m or not 1 <= m <= MAX_BITS:
+        raise ValueError('a table has 2^m entries per column, 1 <= m <= %d, got %d' % (MAX_BITS, size))
+    if m < ROTATE_BITS and W << m > N:
+        raise ValueError('a table on %d index bits has at most %d columns, got %d' % (m, N >> m, W))
+    return W, m
+
+
+def _check_out(out, bits):
+    if out not in ('int', 'bool'):
+        raise ValueError("out must be 'int' or 'bool'")
+    if out == 'int' and bits is None:
+        raise ValueError("out='int' needs the message bits of the entries")
+
+
+def table_polys_count(m, columns):
+    """P, the GLWE samples of a table: W 2^(m-10) for m >= 10, else 1."""
+    return columns << (m - ROTATE_BITS) if m >= ROTATE_BITS else 1
+
+
+def _plain_layout(params, table, out, bits):
+    """(single, W, m, plain): the entries of `table` encoded for `out` and laid out as (P, N) int32 plaintext
+    polynomials (module docstring), 0 in the unused coefficients."""
+    _check_params(params)
+    _check_out(out, bits)
+    table = numpy.asarray(table)
+    W, m = _table_shape(table.shape)
+    single = table.ndim == 1
+    table = table.reshape(W, 1 << m)
+    if out == 'int':
+        enc = lut.encode_int(table, bits)
+    else:
+        enc = numpy.where(table != 0, int(MU), -int(MU)).astype(numpy.int32)
+    plain = numpy.zeros((table_polys_count(m, W), N), numpy.int32)
+    plain.reshape(-1)[:W << m] = enc.reshape(-1)
+    return single, W, m, plain
+
+
 class IndexTable:
     """W columns of 2^m entries encoded to Torus32 and laid out as GLWE plaintexts on the device (module docstring):
     `polys` (P, 2, N) int32 trivial samples (0, T), P = W 2^(m-10) for m >= 10, else 1.  out='int' encodes entries as
     `lut.encode_int(., bits)` (results feed vm.lut and decrypt_int), out='bool' as +-1/8 (results feed the gates)."""
 
     def __init__(self, thr, params, table, out='int', bits=None):
-        _check_params(params)
-        if out not in ('int', 'bool'):
-            raise ValueError("out must be 'int' or 'bool'")
-        table = numpy.asarray(table)
-        self.single = table.ndim == 1
-        if self.single:
-            table = table[None]
-        if table.ndim != 2 or table.shape[0] < 1:
-            raise ValueError('a table has shape (2^m,) or (W, 2^m), got %s' % (table.shape,))
-        W, size = table.shape
-        m = int(size).bit_length() - 1
-        if size != 1 << m or not 1 <= m <= MAX_BITS:
-            raise ValueError('a table has 2^m entries per column, 1 <= m <= %d, got %d' % (MAX_BITS, size))
-        if m < ROTATE_BITS and W << m > N:
-            raise ValueError('a table on %d index bits has at most %d columns, got %d' % (m, N >> m, W))
-        if out == 'int':
-            if bits is None:
-                raise ValueError("out='int' needs the message bits of the entries")
-            enc = lut.encode_int(table, bits)
-        else:
-            enc = numpy.where(table != 0, int(MU), -int(MU)).astype(numpy.int32)
+        self.single, W, m, plain = _plain_layout(params, table, out, bits)
         self.params = params
         self.out, self.bits_out = out, bits
         self.bits, self.columns = m, W
-        if m < ROTATE_BITS:
-            plain = numpy.zeros((1, N), numpy.int32)
-            plain[0, :W << m] = enc.reshape(-1)
-        else:
-            plain = enc.reshape(W << (m - ROTATE_BITS), N)
         polys = numpy.zeros((plain.shape[0], 2, N), numpy.int32)
         polys[:, 1] = plain
         self.polys = thr.to_device(polys)
 
 
-def queries_per_pass(m, columns):
-    """Queries per pass of `lookup`: as many as keep the selector spectra and the tree nodes within PASS_BYTES."""
+class EncryptedIndexTable:
+    """An IndexTable whose entries are encrypted: params, m (`bits`), W (`columns`), `out` / `bits_out` as IndexTable,
+    the variance of the leaves' noise, the wire form `data` (P, 2, N) uint16 (mask and body rounded to 16 bits, 4 bytes
+    per entry) and the device nodes `nodes` (P, 2, N) int32 = data << 16, laid out as IndexTable.polys.  Every leaf is a
+    GLWE sample under the bootstrap key's GLWE key S whose phase carries the entry at its coefficient; unused
+    coefficients encrypt 0.  Made by ctx.encrypt_table (client) or vm.make_encrypted_table (server); vm.lookup and
+    mk.lookup take it where they take an IndexTable."""
+
+    def __init__(self, thr, params, bits, columns, data, variance: float, out='int', bits_out=None, single=None):
+        _check_params(params)
+        _check_out(out, bits_out)
+        W, m = _table_shape((int(columns), 1 << _check_bits(bits)))
+        want = (table_polys_count(m, W), 2, N)
+        if tuple(data.shape) != want or data.dtype != torch.uint16:
+            raise ValueError('an encrypted table of %d columns on %d bits is uint16 %s, got %s %s'
+                             % (W, m, want, data.dtype, tuple(data.shape)))
+        self.params = params
+        self.bits, self.columns = m, W
+        self.out, self.bits_out = out, bits_out
+        self.single = W == 1 if single is None else bool(single)
+        self.variance = float(variance)
+        self.data = data
+        self.nodes = _wrap32((data.to(thr.device).view(torch.int16).to(torch.int64) & 0xffff) << 16).contiguous()
+
+    def dump(self, file_obj):
+        pickle.dump(_ENCRYPTED_TABLE_TAG, file_obj)
+        for x in (self.params, self.bits, self.columns, self.single, self.out, self.bits_out, self.variance):
+            pickle.dump(x, file_obj)
+        pickle.dump(self.data.cpu().numpy().astype('<u2').tobytes(), file_obj)
+
+    def dumps(self):
+        file_obj = io.BytesIO()
+        self.dump(file_obj)
+        return file_obj.getvalue()
+
+    @classmethod
+    def load(cls, file_obj, thr):
+        """ValueError for another pickle, a damaged one or data that does not fit the table's shape."""
+        _check_tag(file_obj, _ENCRYPTED_TABLE_TAG)
+        params, bits, columns, single, out, bits_out, variance, raw = compact._fields(file_obj, 8)
+        W, m = _table_shape((int(columns), 1 << _check_bits(bits)))
+        count = table_polys_count(m, W)
+        if not isinstance(raw, bytes) or len(raw) != count * 2 * N * 2:
+            raise ValueError('encrypted table data does not match %d columns on %d bits' % (W, m))
+        data = numpy.frombuffer(raw, '<u2').astype(numpy.uint16).reshape(count, 2, N)
+        return cls(thr, params, m, W, thr.to_device(data), variance, out, bits_out, single)
+
+    @classmethod
+    def loads(cls, s: bytes, thr):
+        return cls.load(io.BytesIO(s), thr)
+
+    def __eq__(self, other):
+        return (self.__class__ == other.__class__ and self.params == other.params and self.bits == other.bits
+                and self.columns == other.columns and self.single == other.single and self.out == other.out
+                and self.bits_out == other.bits_out and self.variance == other.variance
+                and numpy.array_equal(self.data.cpu().numpy(), other.data.cpu().numpy()))
+
+
+def _round16(x):
+    """int32 coefficients -> round(x / 2^16) mod 2^16 as uint16 (packing's rounding)."""
+    u = ((x.to(torch.int64) & 0xffffffff) + 0x8000) >> 16
+    return (u & 0xffff).to(torch.int32).to(torch.int16).view(torch.uint16)
+
+
+def encrypt_table(thr, rng, key, table, out='int', bits=None):
+    """An EncryptedIndexTable of `table` (shape (2^m,) or (W, 2^m), entries encoded and laid out as IndexTable does).
+    With a NuFHECompactPublicKey, whoever holds it encrypts: compact_encrypt of the flattened layout, its draws.  With
+    the owner's NuFHEIndexSecretKey: a GLWE encryption under S with tlwe_params.min_noise (draws the masks, then the
+    noises, as tlwe_encrypt_zero), rounded to the same 16-bit form.  TypeError for any other key."""
+    if isinstance(key, compact.NuFHECompactPublicKey):
+        params = key.params
+        single, W, m, plain = _plain_layout(params, table, out, bits)
+        data = compact.compact_encrypt(thr, rng, key, thr.to_device(plain)).data
+        fresh, mask_rnd, body_rnd, _ = compact.noise_terms(params)
+        variance = fresh + mask_rnd + body_rnd
+    elif isinstance(key, NuFHEIndexSecretKey):
+        params = key.params
+        single, W, m, plain = _plain_layout(params, table, out, bits)
+        tl = params.tgsw_params.tlwe_params
+        samples = TLweSampleArray.empty(thr, tl, (plain.shape[0],))
+        tlwe_encrypt_zero(thr, rng, samples, tl.min_noise, key._tgsw_key().tlwe_key)
+        x = samples.a.coeffs
+        x[:, 1] = _wrap32((x[:, 1].to(torch.int64) + thr.to_device(plain).to(torch.int64)) & 0xffffffff)
+        data = _round16(x)
+        variance = tl.min_noise**2 + rounding_variance(params)
+    else:
+        raise TypeError('encrypt_table needs a NuFHECompactPublicKey or the NuFHEIndexSecretKey, got %s'
+                        % type(key).__name__)
+    return EncryptedIndexTable(thr, params, m, W, data, variance, out, bits, single)
+
+
+def make_encrypted_table(thr, params, tree_key, columns, out='int', bits=None):
+    """The EncryptedIndexTable whose entries are the LWE samples `columns` (an LweSampleArray of shape (2^m,) or
+    (W, 2^m), or a list of W of shape (2^m,), under the cloud key's LWE key), packed under S with the tree key: the
+    packing pipeline of DESIGN.md section 12 (packing.pack with the tree key's spectra), one GLWE sample per 1024 entries
+    in the lookup layout.  The leaves carry the largest input variance, at least lut.bootstrap_variance, plus
+    packing_variance.  TypeError unless tree_key is a NuFHETreeKey; ValueError for other parameters or a shape that is
+    not a table's."""
+    from .tree_lut import NuFHETreeKey
+    if not isinstance(tree_key, NuFHETreeKey):
+        raise TypeError('make_encrypted_table needs a NuFHETreeKey (ctx.make_cloud_key(sk, tree_key=True)), got %s'
+                        % type(tree_key).__name__)
+    if tree_key.params != params:
+        raise ValueError('the tree key was made for other parameters than this virtual machine')
+    _check_params(params)
+    _check_out(out, bits)
+    if out == 'int':
+        lut._check_bits(bits)
+    single = isinstance(columns, LweSampleArray) and len(columns.shape) == 1
+    cols = [columns] if isinstance(columns, LweSampleArray) else list(columns)
+    if not cols or not all(isinstance(c, LweSampleArray) for c in cols):
+        raise TypeError('make_encrypted_table takes an LweSampleArray or a list of them')
+    if any(c.params != params.in_out_params for c in cols):
+        raise ValueError('the columns do not have the LWE parameters of this virtual machine')
+    if len(cols) == 1:
+        shape = tuple(cols[0].shape)
+    elif all(len(c.shape) == 1 and tuple(c.shape) == tuple(cols[0].shape) for c in cols):
+        shape = (len(cols),) + tuple(cols[0].shape)
+    else:
+        raise ValueError('a list of columns holds W arrays of one shape (2^m,)')
+    W, m = _table_shape(shape)
+    n = params.in_out_params.size
+    flat = LweSampleArray(params.in_out_params, torch.cat([c.a.reshape(-1, n) for c in cols]),
+                          torch.cat([c.b.reshape(-1) for c in cols]),
+                          torch.cat([c.current_variances.reshape(-1) for c in cols]))
+    data = packing.pack(thr, tree_key, flat).data         # W 2^m entries in C order: exactly the lookup layout
+    # bootstrap outputs record the key switch's variance only (the blind rotation's is not tracked), so a leaf counts
+    # at least a bootstrap output's estimate
+    variance = max(float(flat.current_variances.max()), lut.bootstrap_variance(params)) + packing_variance(params)
+    return EncryptedIndexTable(thr, params, m, W, data, variance, out, bits, single)
+
+
+def _table_nodes(table):
+    """The (P, 2, N) int32 leaves the first level reads, and the variance they carry."""
+    if isinstance(table, EncryptedIndexTable):
+        return table.nodes, table.variance
+    return table.polys, 0.0
+
+
+def queries_per_pass(m, columns, tables=0):
+    """Queries per pass of `lookup`: as many as keep the selector spectra, the tree nodes and `tables` concatenated
+    encrypted tables (mk.lookup with one table per tenant: 8 MB each at m = 20) within PASS_BYTES."""
     spectra = m * 16 * 512 * 16                                     # BK_FFT_U64 words of 8 bytes per bit
     nodes = (columns << max(m - ROTATE_BITS, 0)) * NODE_BYTES if m > ROTATE_BITS else 0
-    return max(1, PASS_BYTES // (spectra + nodes))
+    table_bytes = tables * table_polys_count(m, columns) * NODE_BYTES
+    return max(1, (PASS_BYTES - table_bytes) // (spectra + nodes))
 
 
-def lookup_extracted(thr, index, table: IndexTable):
+def lookup_extracted(thr, index, table):
     """The lookup before the key switch: LWE samples under the N-word key of S, a (W, B, N) and b (W, B) int32 for the
     B = prod(index.shape) queries, column w of query q at [w, q]."""
     m, W = table.bits, table.columns
@@ -381,7 +569,7 @@ def lookup_extracted(thr, index, table: IndexTable):
         q1 = min(B, q0 + step)
         Q = q1 - q0
         spec = thr.index_prepare(sel_all[q0:q1]).reshape(Q, m, -1)
-        cur = table.polys                       # shared by every query until the first CMux level
+        cur = _table_nodes(table)[0]            # shared by every query until the first CMux level
         for j in range(ROTATE_BITS, m):
             cur = thr.index_cmux_level(cur, spec, j, Q)
         a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
@@ -393,17 +581,19 @@ def lookup_extracted(thr, index, table: IndexTable):
     return out_a, out_b
 
 
-def lookup(thr, ks, index, table: IndexTable, dest=None):
+def lookup(thr, ks, index, table, dest=None):
     """table[idx] for every encrypted index of `index`: a list of W LweSampleArrays of the index's shape under the
     user's key (one array for a one-dimensional table).  TypeError unless `index` is an EncryptedIndexArray (a
-    compressed one must be decompressed first) and `table` an IndexTable; ValueError for other parameters or an index
-    bit count that is not the table's m."""
+    compressed one must be decompressed first) and `table` an IndexTable or EncryptedIndexTable; ValueError for other
+    parameters or an index bit count that is not the table's m.  The results' variances add an encrypted table's leaf
+    variance: a CMux passes the selected leaf's noise through unchanged."""
     if not isinstance(index, EncryptedIndexArray):
         raise TypeError('lookup needs an EncryptedIndexArray%s, got %s'
                         % (' (decompress() it first)' if isinstance(index, CompressedEncryptedIndexArray) else '',
                            type(index).__name__))
-    if not isinstance(table, IndexTable):
-        raise TypeError('lookup needs an IndexTable (vm.make_index_table), got %s' % type(table).__name__)
+    if not isinstance(table, (IndexTable, EncryptedIndexTable)):
+        raise TypeError('lookup needs an IndexTable (vm.make_index_table) or an EncryptedIndexTable, got %s'
+                        % type(table).__name__)
     if index.params != table.params:
         raise ValueError('the encrypted index was made for other parameters than this table')
     if index.bits != table.bits:
@@ -425,5 +615,5 @@ def lookup(thr, ks, index, table: IndexTable, dest=None):
     for w, r in enumerate(dest):
         r.a.copy_(ra[w].reshape(shape + (n,)))
         r.b.copy_(rb[w].reshape(shape))
-        r.current_variances.fill_(float(output_variance(params, table.bits)))
+        r.current_variances.fill_(float(_table_nodes(table)[1] + output_variance(params, table.bits)))
     return dest[0] if table.single else dest

@@ -28,7 +28,7 @@ from .tgsw import engine_format, fused_kernel_supported
 from .tree_lut import NuFHETreeKey, TreeLookupTable
 from .packing import NuFHEPackingKey, PackedLweSampleArray
 from .compact import CompactLweSampleArray
-from .index_lookup import EncryptedIndexArray, IndexTable
+from .index_lookup import EncryptedIndexArray, EncryptedIndexTable, IndexTable
 from . import compact, gates, index_lookup, packing, tree_lut
 
 # gates that need no key: run per tenant
@@ -684,32 +684,45 @@ class MultiKeyVirtualMachine:
             row += c
         return out
 
-    @_in_rounds(('indexes',), ('dest',))
+    @_in_rounds(('indexes',), ('table', 'dest'))
     def lookup(self, indexes, table, dest=None):
-        """table[idx] for every tenant's EncryptedIndexArray (VirtualMachine.lookup) with one IndexTable shared by all
-        tenants: the queries of all tenants go through one CMux tree and rotation per pass, then one multi-key key
-        switch.  Entry t of the result is one ciphertext array of the tenant's index shape, or a list of W for a table
-        of W columns."""
-        if not isinstance(table, IndexTable):
-            raise TypeError('lookup needs an IndexTable (vm.make_index_table), got %s' % type(table).__name__)
+        """table[idx] for every tenant's EncryptedIndexArray (VirtualMachine.lookup): `table` is one IndexTable shared by
+        all tenants, or a list with one EncryptedIndexTable per tenant (None for an idle tenant; DESIGN.md section 20)
+        that share m, W and out.  The queries of all tenants go through one CMux tree and rotation per pass, the level
+        that first reads a table taking each query's own table, then one multi-key key switch.  Entry t of the result is
+        one ciphertext array of the tenant's index shape, or a list of W for a table of W columns."""
+        per_tenant = isinstance(table, (list, tuple))
+        if not per_tenant and not isinstance(table, IndexTable):
+            raise TypeError('lookup needs an IndexTable (vm.make_index_table) or a list of EncryptedIndexTables, got %s'
+                            % type(table).__name__)
         if not isinstance(indexes, (list, tuple)) or len(indexes) != self.tenants:
             raise ValueError('indexes must be a list of %d entries, one per tenant' % self.tenants)
         active = [t for t in range(self.tenants) if indexes[t] is not None]
         indexes = self._tenant_objects(indexes, active, EncryptedIndexArray, 'encrypted index',
                                        ' (decompress() a compressed one first)')
-        if table.params != self.params:
-            raise ValueError('the table was made for other parameters than the cloud keys')
+        if per_tenant:
+            tables = self._tenant_objects(table, active, EncryptedIndexTable, 'encrypted table',
+                                          ' (ctx.encrypt_table or vm.make_encrypted_table)')
+            ref = tables[active[0]] if active else None
+            for t in active:
+                if (tables[t].bits, tables[t].columns, tables[t].single) != (ref.bits, ref.columns, ref.single):
+                    raise ValueError('tenant %d: the tables of one call share m = %d and W = %d, got m = %d, W = %d'
+                                     % (t, ref.bits, ref.columns, tables[t].bits, tables[t].columns))
+        else:
+            if table.params != self.params:
+                raise ValueError('the table was made for other parameters than the cloud keys')
+            tables, ref = None, table
+        out = [None] * self.tenants
+        if not active:
+            return out
         for t in active:
-            if indexes[t].bits != table.bits:
-                raise ValueError('tenant %d: the table takes %d-bit indices, got %d bits' % (t, table.bits, indexes[t].bits))
-        m, W = table.bits, table.columns
+            if indexes[t].bits != ref.bits:
+                raise ValueError('tenant %d: the table takes %d-bit indices, got %d bits' % (t, ref.bits, indexes[t].bits))
+        m, W = ref.bits, ref.columns
         dest_lists = self._per_tenant(dest, active, W, 'a table of %d columns' % W)
         for t in active:
             if dest_lists is not None and any(tuple(d.shape) != indexes[t].shape for d in dest_lists[t]):
                 raise ValueError('tenant %d: lookup writes %d results of shape %s' % (t, W, indexes[t].shape))
-        out = [None] * self.tenants
-        if not active:
-            return out
         thr = self.thread
         n = self.params.in_out_params.size
         counts = [int(numpy.prod(indexes[t].shape, dtype=numpy.int64)) for t in active]
@@ -717,20 +730,46 @@ class MultiKeyVirtualMachine:
         B = int(offsets[-1])
         sels = [indexes[t].samples.reshape(c, m, 2, 2, 2, index_lookup.N) for t, c in zip(active, counts)]
         kss = [self._ks[t] for t in active]
+        tabs = [tables[t] for t in active] if per_tenant else [None] * len(active)
         # column w of query q (of the concatenated batch) at row w B + q
         res_a, res_b = thr.empty((W * B, n), torch.int32), thr.empty((W * B,), torch.int32)
-        step = index_lookup.queries_per_pass(m, W)
-        for q0 in range(0, B, step):
+        q0 = 0
+        while q0 < B:
+            step = index_lookup.queries_per_pass(m, W)
+            if per_tenant:          # as many queries as leave room for the tables of the tenants they belong to
+                k = 1
+                while True:
+                    step = index_lookup.queries_per_pass(m, W, k)
+                    k2 = len(self._pass_counts(counts, q0, min(B, q0 + step))[0])
+                    if k2 <= k:
+                        break
+                    k = k2
             q1 = min(B, q0 + step)
             Q = q1 - q0
-            cnt, pkss, psels, plos = self._pass_counts(counts, q0, q1, kss, sels, offsets[:-1])
+            cnt, pkss, psels, plos, ptabs = self._pass_counts(counts, q0, q1, kss, sels, offsets[:-1], tabs)
             pieces = [s[max(q0, lo) - lo:][:c] for s, lo, c in zip(psels, plos, cnt)]
             spec = thr.index_prepare(torch.cat(pieces) if len(pieces) > 1 else pieces[0]).reshape(Q, m, -1)
-            cur = table.polys
-            for j in range(index_lookup.ROTATE_BITS, m):
-                cur = thr.index_cmux_level(cur, spec, j, Q)
-            a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
+            j0 = index_lookup.ROTATE_BITS
+            cur = table.polys if not per_tenant else None
+            if per_tenant:
+                # the pass's distinct tables, concatenated, and the table of every query
+                uniq = {}
+                slot = [uniq.setdefault(id(tb), (len(uniq), tb))[0] for tb in ptabs]
+                nodes = torch.cat([tb.nodes for _, tb in uniq.values()]) if len(uniq) > 1 else ptabs[0].nodes
+                nodes = nodes.reshape(len(uniq), -1, 2, index_lookup.N)
+                ids = numpy.repeat(numpy.asarray(slot, numpy.uint32), cnt)
+                if m > j0:
+                    cur = thr.index_cmux_level_indirect(nodes, ids, spec, j0, Q)
+                    j0 += 1
+            if cur is None:
+                a, b = thr.index_rotate_extract_indirect(nodes, ids, spec, m, W, Q)
+            else:
+                for j in range(j0, m):
+                    cur = thr.index_cmux_level(cur, spec, j, Q)
+                a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
             del spec, cur
+            if per_tenant:
+                del nodes
             # rows (w, q) are column-major; the key switch wants each tenant's W c rows together, in vm.lookup's order
             perm, lo = [], 0
             for c in cnt:
@@ -743,12 +782,15 @@ class MultiKeyVirtualMachine:
             dst = thr.to_device((perm // Q) * B + q0 + perm % Q)
             res_a.index_copy_(0, dst, ra)
             res_b.index_copy_(0, dst, rb)
+            q0 = q1
         res_cv = thr.empty((W * B,), torch.float32).fill_(float(index_lookup.output_variance(self.params, m)))
         for i, t in enumerate(active):
             shape, lo, c = indexes[t].shape, int(offsets[i]), counts[i]
             cols = []
             for w in range(W):
                 r = slice(w * B + lo, w * B + lo + c)
+                if per_tenant:
+                    res_cv[r] = float(tables[t].variance + index_lookup.output_variance(self.params, m))
                 x = LweSampleArray(self.params.in_out_params, res_a[r].reshape(shape + (n,)), res_b[r].reshape(shape),
                                    res_cv[r].reshape(shape))
                 if dest_lists is not None:
@@ -758,5 +800,5 @@ class MultiKeyVirtualMachine:
                     d.current_variances.copy_(x.current_variances)
                     x = d
                 cols.append(x)
-            out[t] = cols[0] if table.single else cols
+            out[t] = cols[0] if ref.single else cols
         return out

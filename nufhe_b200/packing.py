@@ -91,7 +91,9 @@ class NuFHEPackingSecretKey:
 class _GadgetKey:
     """n t seeded GLWE encryptions of the constants s_i g_j (s the LWE key, g_j = PACK_GADGET[j]) under a GLWE key:
     params, the 256-bit seed of the masks (ChaCha20 stream (seed, NONCE)), the bodies (n, t, N) int32 and the variance
-    of their noise.  The packing key and the tree key (nufhe_b200/tree_lut.py) are two distinct subclasses."""
+    of their noise.  The packing key and the tree key (nufhe_b200/tree_lut.py) are two distinct subclasses.
+    `spectra(thr)` -- the NTT of all n t (k+1) key polynomials, 16.4 MB for k = 1 -- is built once per engine and cached
+    on the object: with it, `pack` packs under the key's GLWE key (S_p for the packing key, S for the tree key)."""
     NONCE = None
     TAG = None
     NAME = None
@@ -101,6 +103,7 @@ class _GadgetKey:
         self.seed = numpy.asarray(seed, numpy.uint32).reshape(8)
         self.body = body
         self.variance = float(variance)
+        self._spectra = None
         tl, k, N = _glwe(params)
         want = (params.in_out_params.size, PACK_LEVELS, N)
         if tuple(body.shape) != want:
@@ -126,6 +129,15 @@ class _GadgetKey:
     def masks(self, thr):
         """The masks A (n, t, k, N), regenerated from the seed."""
         return _masks(thr, self.seed, self.params, self.NONCE)
+
+    def spectra(self, thr):
+        """NTT of the key polynomials K_iju as (n t, k + 1, N) field elements, row i t + j: what nb_ntt_mac reads."""
+        if self._spectra is None or self._spectra[0] is not thr:
+            tl, k, N = _glwe(self.params)
+            polys = torch.cat([self.masks(thr), self.body.to(thr.device)[:, :, None, :]], dim=2)   # (n, t, k+1, N)
+            spec = thr.ntt_forward_i32(polys.contiguous()).reshape(-1, k + 1, N)
+            self._spectra = (thr, spec)
+        return self._spectra[1]
 
     def dump(self, file_obj):
         pickle.dump(self.TAG, file_obj)
@@ -159,29 +171,15 @@ class _GadgetKey:
 
 class NuFHEPackingKey(_GadgetKey):
     """The server's half: params, the 256-bit seed of the masks, the bodies (n, t, N) int32 (4.1 MB for the default
-    parameters) and the variance of their noise.  `spectra(thr)` -- the NTT of all n t (k+1) key polynomials, 16.4 MB
-    for k = 1 -- is built once per engine and cached on the object."""
+    parameters) and the variance of their noise."""
     NONCE = NONCE_PACKING_KEY
     TAG = _PACKING_KEY_TAG
     NAME = 'packing key'
-
-    def __init__(self, params, seed, body, variance: float):
-        super().__init__(params, seed, body, variance)
-        self._spectra = None
 
     @classmethod
     def from_secret_key(cls, thr, rng, secret_key, packing_secret_key: NuFHEPackingSecretKey):
         """K_ij = GLWE_{S_p}(s_i g_j) with seeded masks: draws the seed, then the Gaussian body noises (n, t, N)."""
         return cls._encrypt(thr, rng, secret_key, packing_secret_key.key)
-
-    def spectra(self, thr):
-        """NTT of the key polynomials K_iju as (n t, k + 1, N) field elements, row i t + j: what nb_ntt_mac reads."""
-        if self._spectra is None or self._spectra[0] is not thr:
-            tl, k, N = _glwe(self.params)
-            polys = torch.cat([self.masks(thr), self.body.to(thr.device)[:, :, None, :]], dim=2)   # (n, t, k+1, N)
-            spec = thr.ntt_forward_i32(polys.contiguous()).reshape(-1, k + 1, N)
-            self._spectra = (thr, spec)
-        return self._spectra[1]
 
 
 def _masks(thr, seed, params, nonce=NONCE_PACKING_KEY):
@@ -246,8 +244,8 @@ def make_packing_keys(thr, rng, secret_key):
     return psk, NuFHEPackingKey.from_secret_key(thr, rng, secret_key, psk)
 
 
-def pack(thr, packing_key: NuFHEPackingKey, ciphertexts: LweSampleArray):
-    """Pack an LweSampleArray of any shape into a PackedLweSampleArray, a few groups per pass
+def pack(thr, packing_key: _GadgetKey, ciphertexts: LweSampleArray):
+    """Pack an LweSampleArray of any shape into a PackedLweSampleArray under the key's GLWE key, a few groups per pass
     (nb_pack_digits -> nb_ntt_forward_i32 -> nb_ntt_mac -> nb_ntt_inverse_i32 -> nb_pack_finish)."""
     params = packing_key.params
     if ciphertexts.params != params.in_out_params:
