@@ -26,6 +26,7 @@ from .lwe import LweSampleArray
 from .tlwe import TLweSampleArray, tlwe_encrypt_zero_with_masks
 from .compressed import draw_seed, _check_tag
 from .random_numbers import rand_gaussian_torus32
+from .batch_keys import OneKey, group_rows
 
 NONCE_COMPACT_KEY = 7
 NONCE_COMPACT_RANDOMNESS = 8
@@ -219,22 +220,38 @@ def expand(thr, params, ks, compact: CompactLweSampleArray):
     """The LweSampleArray (under the cloud key's LWE key s) of a CompactLweSampleArray, a few groups per pass
     (nb_compact_extract -> nb_keyswitch with `ks`, the cloud key's LweKeyswitchKey).  Its variances are the key
     switch's plus the fresh and rounding terms of noise_terms."""
-    tl, k, N = _glwe(params)
-    io_params = params.in_out_params
-    n = io_params.size
-    shape = compact.shape
-    batch = compact.size
-    out = LweSampleArray.empty(thr, io_params, shape)
-    a, b, cv = out.a.view(batch, n), out.b.view(batch), out.current_variances.view(batch)
-    fresh, mask_rnd, body_rnd, _ = noise_terms(params)
-    step = groups_per_pass(params) * N
-    data = compact.data.to(thr.device)
-    ks_arrays = ks.device_arrays()
-    for c0 in range(0, batch, step):
-        c1 = min(batch, c0 + step)
-        ext = thr.compact_extract(data[c0 // N:-(-c1 // N)], c1 - c0)
-        _, _, rcv = thr.keyswitch(ks_arrays, ext, out=(a[c0:c1], b[c0:c1]), want_cv=True)
-        del ext
-        cv[c0:c1] = rcv + (fresh + mask_rnd + body_rnd)
+    out = LweSampleArray.empty(thr, params.in_out_params, compact.shape)
+    expand_groups(thr, params, OneKey(thr, ks=ks), [compact], (out.a, out.b, out.current_variances))
     return out
 
+
+def expand_groups(thr, params, keys, compacts, out):
+    """Expand `compacts`, one CompactLweSampleArray per tenant of `keys` (batch_keys), into the concatenation of their
+    rows, out = (a, b, variances), a few groups per pass.  One tenant's rows are extracted and key-switched straight
+    into `out`; with several, whole groups are extracted and the slots that pad a tenant's last group are dropped."""
+    tl, k, N = _glwe(params)
+    a, b, cv = out[0].view(-1, out[0].shape[-1]), out[1].view(-1), out[2].view(-1)
+    fresh, mask_rnd, body_rnd, _ = noise_terms(params)
+    if len(compacts) == 1:
+        data, B = compacts[0].data.to(thr.device), compacts[0].size
+        G = -(-B // N)
+    else:
+        groups, rows = group_rows(keys.counts, N, -1)
+        data, G = torch.cat([c.data.to(thr.device) for c in compacts]), sum(groups)
+    step = groups_per_pass(params)
+    for p0 in range(0, G, step):
+        p1 = min(G, p0 + step)
+        if len(compacts) == 1:
+            r0, r1 = p0 * N, min(B, p1 * N)
+            ext = thr.compact_extract(data[p0:p1], r1 - r0)
+        else:
+            slots = rows[p0 * N:p1 * N]
+            real = numpy.nonzero(slots >= 0)[0]
+            r0, r1 = int(slots[real[0]]), int(slots[real[-1]]) + 1      # the rows of a pass are consecutive
+            ext = thr.compact_extract(data[p0:p1], (p1 - p0) * N)
+            if len(real) < len(slots):
+                sel = thr.to_device(real)
+                ext = ext[0].index_select(0, sel), ext[1].index_select(0, sel)
+        _, _, rcv = keys.split(r0, r1).keyswitch(ext, out=(a[r0:r1], b[r0:r1]), want_cv=True)
+        del ext
+        cv[r0:r1] = rcv + (fresh + mask_rnd + body_rnd)

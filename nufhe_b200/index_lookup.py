@@ -29,6 +29,7 @@ from .polynomials import IntPolynomialArray
 from .compressed import draw_seed, _check_tag, _variance, _wrap32, tgsw_add_message_seeded
 from .random_numbers import rand_gaussian_torus32
 from .gates import MU
+from .batch_keys import owners
 from . import compact, lut, packing
 
 NONCE_INDEX = 6
@@ -556,25 +557,61 @@ def queries_per_pass(m, columns, tables=0):
     return max(1, (PASS_BYTES - table_bytes) // (spectra + nodes))
 
 
+def lookup_passes(thr, m, W, sels, table=None, tables=None):
+    """The lookup_extracted samples of the queries of `sels` (selector arrays (c, m, 2, 2, 2, N), one per tenant, in
+    order) a pass at a time: yields q0, q1 and a (W, q1 - q0, N), b (W, q1 - q0) of queries [q0, q1).  Every query reads
+    `table`, or, with `tables` (one EncryptedIndexTable per tenant), its tenant's table from the first level on."""
+    counts = [s.shape[0] for s in sels]
+    starts = numpy.cumsum([0] + counts)
+    B = int(starts[-1])
+    q0 = 0
+    while q0 < B:
+        if tables is None:
+            step = queries_per_pass(m, W)
+        else:           # as many queries as leave room for the tables of the tenants they belong to
+            k = 1
+            while True:
+                step = queries_per_pass(m, W, k)
+                k2 = len(owners(counts, q0, min(B, q0 + step))[0])
+                if k2 <= k:
+                    break
+                k = k2
+        q1 = min(B, q0 + step)
+        Q = q1 - q0
+        idx, own = owners(counts, q0, q1) if len(sels) > 1 else ([0], [Q])
+        pieces = [sels[i][max(q0, starts[i]) - starts[i]:][:c] for i, c in zip(idx, own)]
+        spec = thr.index_prepare(torch.cat(pieces) if len(pieces) > 1 else pieces[0]).reshape(Q, m, -1)
+        j0 = ROTATE_BITS
+        cur = _table_nodes(table)[0] if tables is None else None    # shared by every query until the first CMux level
+        if tables is not None:
+            # the pass's distinct tables, concatenated, and the table of every query
+            uniq = {}
+            slot = [uniq.setdefault(id(tables[i]), (len(uniq), tables[i]))[0] for i in idx]
+            nodes = torch.cat([tb.nodes for _, tb in uniq.values()]) if len(uniq) > 1 else tables[idx[0]].nodes
+            nodes = nodes.reshape(len(uniq), -1, 2, N)
+            ids = numpy.repeat(numpy.asarray(slot, numpy.uint32), own)
+            if m > j0:
+                cur, j0 = thr.index_cmux_level_indirect(nodes, ids, spec, j0, Q), j0 + 1
+            else:
+                a, b = thr.index_rotate_extract_indirect(nodes, ids, spec, m, W, Q)
+            del nodes
+        if cur is not None:
+            for j in range(j0, m):
+                cur = thr.index_cmux_level(cur, spec, j, Q)
+            a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
+        del spec, cur
+        yield q0, q1, a, b
+        q0 = q1
+
+
 def lookup_extracted(thr, index, table):
     """The lookup before the key switch: LWE samples under the N-word key of S, a (W, B, N) and b (W, B) int32 for the
     B = prod(index.shape) queries, column w of query q at [w, q]."""
     m, W = table.bits, table.columns
     B = int(numpy.prod(index.shape, dtype=numpy.int64))
-    sel_all = index.samples.reshape(B, m, 2, 2, 2, N)
-    out_a = thr.empty((W, B, N), torch.int32)
-    out_b = thr.empty((W, B), torch.int32)
-    step = queries_per_pass(m, W)
-    for q0 in range(0, B, step):
-        q1 = min(B, q0 + step)
-        Q = q1 - q0
-        spec = thr.index_prepare(sel_all[q0:q1]).reshape(Q, m, -1)
-        cur = _table_nodes(table)[0]            # shared by every query until the first CMux level
-        for j in range(ROTATE_BITS, m):
-            cur = thr.index_cmux_level(cur, spec, j, Q)
-        a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
-        del spec, cur
-        if B == Q:
+    out_a, out_b = thr.empty((W, B, N), torch.int32), thr.empty((W, B), torch.int32)
+    for q0, q1, a, b in lookup_passes(thr, m, W, [index.samples.reshape(B, m, 2, 2, 2, N)], table):
+        if q1 - q0 == B:
             return a, b
         out_a[:, q0:q1] = a
         out_b[:, q0:q1] = b

@@ -22,9 +22,9 @@ from .numeric_functions import t32_to_phase
 from .lwe import LweSampleArray
 from .polynomials import TorusPolynomialArray, shift_tp_inverted_power
 from .tlwe import TLweSampleArray, tlwe_noiseless_trivial, tlwe_extract_lwe_samples
-from .tgsw import engine_format
-from .bootstrap import blind_rotate, _single_kernel
+from .bootstrap import blind_rotate
 from .gates import MU, check_shape
+from .batch_keys import OneKey
 
 MAX_BITS = 3
 MAX_LOG2_OUTPUTS = 2
@@ -268,16 +268,13 @@ def bootstrap_lut(thr, results, bk, ks, table: LookupTable, x: LweSampleArray, y
     _check_margin(_sigma(bk.in_out_params, bk.bk_params, ks.decomp_length, ks.log2_base, L,
                          None if y is None else shift, getattr(bk, 'multi_bit', 1)), table.bits, L,
                   None if y is None else shift)
-    B = int(numpy.prod(shape, dtype=numpy.int64))
     p1 = _expand(x, shape)
     p2 = _expand(y, shape) if y is not None else None
     s1 = 1 << shift if y is not None else 1
     tv = table.tv.reshape(-1, 1024) if table.batch_shape else table.tv
-    if _single_kernel(perf_params, bk):
-        ea, eb = thr.bootstrap_lut_extract(p1, p2, 0, s1, 1, tv, L, engine_format(thr, bk.tgsw))
-    else:
-        ea, eb = _lut_steps(thr, bk, p1, p2, s1, tv, L, B, perf_params)
-    ra, rb, rcv = thr.keyswitch(ks.device_arrays(), (ea, eb), want_cv=True)
+    keys = OneKey(thr, bk, ks, perf_params)
+    ea, eb = keys.bootstrap_lut_extract(p1, p2, s1, tv, L)
+    ra, rb, rcv = keys.keyswitch((ea, eb), want_cv=True)
     K = table.outputs
     ra, rb, rcv = ra.reshape(shape + (K, ra.shape[-1])), rb.reshape(shape + (K,)), rcv.reshape(shape + (K,))
     for j, r in enumerate(results):

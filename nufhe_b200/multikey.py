@@ -21,7 +21,7 @@ from .api_low_level import NuFHECloudKey, empty_ciphertext
 from .compressed import CompressedCloudKey
 from .gates import MU, _BINARY_GATES, check_shape, get_shape, result_shape
 from .lwe import LweSampleArray
-from .lut import LookupTable, _check_config, _check_margin, _sigma
+from .lut import LookupTable, _check_config, _check_margin, _expand, _sigma
 from .numeric_functions import phase_to_t32
 from .performance import PerformanceParameters
 from .tgsw import engine_format, fused_kernel_supported
@@ -29,6 +29,7 @@ from .tree_lut import NuFHETreeKey, TreeLookupTable
 from .packing import NuFHEPackingKey, PackedLweSampleArray
 from .compact import CompactLweSampleArray
 from .index_lookup import EncryptedIndexArray, EncryptedIndexTable, IndexTable
+from .batch_keys import TenantKeys
 from . import compact, gates, index_lookup, packing, tree_lut
 
 # gates that need no key: run per tenant
@@ -259,17 +260,8 @@ class MultiKeyVirtualMachine:
             shapes[t] = shape
         return active, shapes
 
-    @staticmethod
-    def _expand(x, shape):
-        a, b = x.a, x.b
-        if tuple(b.shape) != shape:
-            while b.dim() < len(shape):
-                a, b = a.unsqueeze(0), b.unsqueeze(0)
-            a, b = a.expand(shape + (a.shape[-1],)), b.expand(shape)
-        return a.contiguous().reshape(-1, a.shape[-1]), b.contiguous().reshape(-1)
-
     def _concat(self, ops, active, shapes):
-        parts = [self._expand(ops[t], shapes[t]) for t in active]
+        parts = [_expand(ops[t], shapes[t]) for t in active]
         return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
 
     def _counts(self, active, shapes):
@@ -298,6 +290,16 @@ class MultiKeyVirtualMachine:
                 dest[t].b.copy_(b)
                 dest[t].current_variances.copy_(cv)
                 out[t] = dest[t]
+        return out
+
+    def _columns(self, cols, active, shapes, counts, dest_lists, single):
+        """Per tenant, its views of several results (a, b, cv) of the whole batch (the outputs of a table, the columns
+        of a lookup), or copies into its list of `dest_lists`: one array when `single`, else a list."""
+        res = [self._results(c, active, shapes, counts, None if dest_lists is None else
+                             [None if d is None else d[j] for d in dest_lists]) for j, c in enumerate(cols)]
+        out = [None] * self.tenants
+        for t in active:
+            out[t] = res[0][t] if single else [r[t] for r in res]
         return out
 
     # --- gates ---------------------------------------------------------------------------------
@@ -430,19 +432,15 @@ class MultiKeyVirtualMachine:
         tv = table.tv
         if tables is not None:      # one test vector per ciphertext: its tenant's
             tv = torch.cat([tables[t].tv.reshape(1, -1).expand(counts[t], -1) for t in active])
-        ea, eb = self.thread.mk_bootstrap_lut_extract(p1, p2, 0, s1, 1, tv, L, self._bk_ints, counts)
-        ra, rb, rcv = self._keyswitch([c * K for c in counts], (ea, eb))
+        keys = TenantKeys(self.thread, counts, self._bk_ints, self._ks)
+        ea, eb = keys.bootstrap_lut_extract(p1, p2, s1, tv, L)
+        ra, rb, rcv = keys.keyswitch((ea, eb), per=K, want_cv=True)
         # sample j of ciphertext c is row c * K + j: one contiguous block per output
         total = rb.numel() // K
         ra = ra.reshape(total, K, -1).transpose(0, 1).contiguous()
         rb = rb.reshape(total, K).t().contiguous()
         rcv = rcv.reshape(total, K).t().contiguous()
-        per_output = [self._results((ra[j], rb[j], rcv[j]), active, shapes, counts,
-                                    None if dest_lists is None else [None if d is None else d[j] for d in dest_lists])
-                      for j in range(K)]
-        for t in active:
-            out[t] = per_output[0][t] if K == 1 else [per_output[j][t] for j in range(K)]
-        return out
+        return self._columns([(ra[j], rb[j], rcv[j]) for j in range(K)], active, shapes, counts, dest_lists, K == 1)
 
     # --- per-tenant extras (DESIGN.md section 18) --------------------------------------------------
     def _tenant_objects(self, objs, active, cls, what, hint=''):
@@ -456,15 +454,6 @@ class MultiKeyVirtualMachine:
             if objs[t].params != self.params:
                 raise ValueError('tenant %d: the %s was made for other parameters than the cloud keys' % (t, what))
         return list(objs)
-
-    @staticmethod
-    def _pass_counts(counts, c0, c1, *per_tenant):
-        """The rows of [c0, c1) of the concatenated batch that each tenant owns (counts: rows per tenant, in order), for
-        the tenants that own some, and their entries of each list in `per_tenant`."""
-        hi = numpy.cumsum(counts, dtype=numpy.int64)
-        own = numpy.clip(numpy.minimum(hi, c1) - numpy.maximum(hi - counts, c0), 0, None)
-        idx = numpy.nonzero(own)[0]
-        return ([int(own[i]) for i in idx],) + tuple([lst[i] for i in idx] for lst in per_tenant)
 
     def _per_tenant(self, dest, active, K, what):
         """dest as a list of lists of K results (None for idle tenants)."""
@@ -512,76 +501,17 @@ class MultiKeyVirtualMachine:
         if not active:
             return out
         thr = self.thread
-        all_counts = self._counts(active, shapes)
-        counts = [all_counts[t] for t in active]
-        bks = [self._bk_ints[t] for t in active]
-        kss = [self._ks[t] for t in active]
-        planes = [tree_keys[t].planes(thr) for t in active]
+        counts = self._counts(active, shapes)
+        keys = TenantKeys(thr, [counts[t] for t in active], [self._bk_ints[t] for t in active],
+                          [self._ks[t] for t in active], planes=[tree_keys[t].planes(thr) for t in active])
         flat = [self._concat(d, active, shapes) for d in reversed(digits)]        # d_0 first
-        B = sum(counts)
-        n = self.params.in_out_params.size
-        out_a = thr.empty((B, F, n), torch.int32)
-        out_b = thr.empty((B, F), torch.int32)
-        step = max(1, tree_lut.ROWS_PER_PASS // table.groups)
-        for c0 in range(0, B, step):
-            c1 = min(B, c0 + step)
-            cnt, pbks, pkss, pplanes = self._pass_counts(counts, c0, c1, bks, kss, planes)
-            part = [(a[c0:c1], b[c0:c1]) for a, b in flat]
-            cur = self._tree_level1(table, part[0], pbks, pkss, cnt)
-            for level in range(1, table.digits):
-                cur = self._tree_level(table, pplanes, cur, part[level], pbks, pkss, cnt)
-            out_a[c0:c1].copy_(cur[0])
-            out_b[c0:c1].copy_(cur[1])
+        out_a, out_b = tree_lut.evaluate(keys, table, flat)
         # function f of every tenant: views of one (F, B) allocation
         out_a, out_b = out_a.transpose(0, 1).contiguous(), out_b.t().contiguous()
-        out_cv = thr.empty((F, B), torch.float32).fill_(float(tree_lut.output_variance(table.params, table.bits,
-                                                                                        table.digits)))
-        row = 0
-        for t, rows in zip(active, counts):
-            shape, r = shapes[t], slice(row, row + rows)
-            res = [LweSampleArray(self.params.in_out_params, out_a[f, r].reshape(shape + (n,)),
-                                  out_b[f, r].reshape(shape), out_cv[f, r].reshape(shape)) for f in range(F)]
-            row += rows
-            if dest_lists is not None:
-                for d, x in zip(dest_lists[t], res):
-                    d.a.copy_(x.a)
-                    d.b.copy_(x.b)
-                    d.current_variances.copy_(x.current_variances)
-                res = dest_lists[t]
-            out[t] = res[0] if table.single else res
-        return out
-
-    def _tree_level1(self, table, d0, bks, kss, cnt):
-        """tree_lut._level1 over the concatenated batch: cnt[i] ciphertexts of the i-th active tenant."""
-        a, b = d0
-        B, n = a.shape
-        Q, L = table.groups, table.log2_outputs
-        K = 1 << L
-        ea_ = a[:, None, :].expand(B, Q, n).reshape(B * Q, n)
-        eb_ = b[:, None].expand(B, Q).reshape(B * Q)
-        tv = table.tv.reshape(Q, -1)[None].expand(B, Q, table.tv.shape[-1]).reshape(B * Q, -1)
-        ea, eb = self.thread.mk_bootstrap_lut_extract((ea_, eb_), None, 0, 1, 1, tv, L, bks, [c * Q for c in cnt])
-        ra, rb, _ = self.thread.mk_keyswitch(kss, [c * Q * K for c in cnt], (ea, eb))
-        return ra.reshape(B, Q * K, n)[:, :table.columns], rb.reshape(B, Q * K)[:, :table.columns]
-
-    def _tree_level(self, table, planes, cur, digit, bks, kss, cnt):
-        """tree_lut._level over the concatenated batch: the tree key switch with each tenant's planes, one assembly,
-        the GLWE-test-vector bootstrap and the key switch with each tenant's keys."""
-        thr = self.thread
-        ca, cb = cur
-        B, W, n = ca.shape
-        M = 1 << table.bits
-        k = self.params.tgsw_params.tlwe_params.mask_size
-        T = B * (W // M)
-        v = thr.mk_tree_keyswitch(ca.reshape(B * W, n), planes, [c * W for c in cnt], k)
-        tv = thr.tree_assemble(v.reshape(T, M, k + 1, -1), cb.reshape(T, M), table.bits)
-        da, db = digit
-        xa = da[:, None, :].expand(B, W // M, n).reshape(T, n)
-        xb = db[:, None].expand(B, W // M).reshape(T)
-        per = [c * (W // M) for c in cnt]
-        ea, eb = thr.mk_bootstrap_glwe_lut_extract((xa, xb), tv, bks, per)
-        ra, rb, _ = thr.mk_keyswitch(kss, per, (ea, eb))
-        return ra.reshape(B, W // M, n), rb.reshape(B, W // M)
+        variance = tree_lut.output_variance(table.params, table.bits, table.digits)
+        out_cv = thr.empty((F, sum(counts)), torch.float32).fill_(float(variance))
+        return self._columns([(out_a[f], out_b[f], out_cv[f]) for f in range(F)], active, shapes, counts, dest_lists,
+                             table.single)
 
     def pack(self, packing_keys, results_list):
         """Pack every tenant's results (VirtualMachine.pack) with its NuFHEPackingKey: a list of PackedLweSampleArrays
@@ -597,33 +527,11 @@ class MultiKeyVirtualMachine:
         if not active:
             return out
         thr = self.thread
-        tl = self.params.tgsw_params.tlwe_params
-        k, N = tl.mask_size, tl.polynomial_degree
-        n = self.params.in_out_params.size
-        counts = [int(numpy.prod(shapes[t], dtype=numpy.int64)) for t in active]
-        groups = [-(-c // N) for c in counts]
-        G = sum(groups)
-        # padded row r of group g holds row src[g N + slot] of the concatenated batch, or the zero row B
-        B = sum(counts)
-        src = numpy.full(G * N, B, numpy.int64)
-        g0 = c0 = 0
-        for c, g in zip(counts, groups):
-            src[g0 * N:g0 * N + c] = numpy.arange(c0, c0 + c)
-            g0, c0 = g0 + g, c0 + c
-        a_all = torch.cat([results_list[t].a.reshape(-1, n) for t in active] + [thr.empty((1, n), torch.int32).zero_()])
-        b_all = torch.cat([results_list[t].b.reshape(-1) for t in active] + [thr.empty((1,), torch.int32).zero_()])
-        src = thr.to_device(src)
-        keys = [packing_keys[t].spectra(thr) for t in active]
-        data = thr.empty((G, k + 1, N), torch.uint16)
-        step = packing.groups_per_pass(self.params)
-        for p0 in range(0, G, step):
-            p1 = min(G, p0 + step)
-            idx = src[p0 * N:p1 * N]
-            spec = thr.ntt_forward_i32(thr.pack_digits(a_all.index_select(0, idx)))
-            cnt, pkeys = self._pass_counts(groups, p0, p1, keys)
-            part = thr.pack_finish(thr.ntt_inverse_i32(thr.mk_ntt_mac(spec, pkeys, cnt)), b_all.index_select(0, idx))
-            del spec
-            data.view(torch.int16)[p0:p1].copy_(part.view(torch.int16))
+        n, N = self.params.in_out_params.size, self.params.tgsw_params.tlwe_params.polynomial_degree
+        parts = [(results_list[t].a.reshape(-1, n), results_list[t].b.reshape(-1)) for t in active]
+        groups = [-(-b.shape[0] // N) for a, b in parts]
+        keys = TenantKeys(thr, groups, spectra=[packing_keys[t].spectra(thr) for t in active])
+        data = packing.pack_groups(thr, self.params, keys, parts)
         g0 = 0
         for t, g in zip(active, groups):
             out[t] = PackedLweSampleArray(self.params, shapes[t], data[g0:g0 + g])
@@ -643,46 +551,14 @@ class MultiKeyVirtualMachine:
         if not active:
             return out
         thr = self.thread
-        tl = self.params.tgsw_params.tlwe_params
-        N = tl.polynomial_degree
-        io_params = self.params.in_out_params
-        n = io_params.size
-        counts = [compacts[t].size for t in active]
-        groups = [-(-c // N) for c in counts]
-        B, G = sum(counts), sum(groups)
-        res_a, res_b = thr.empty((B, n), torch.int32), thr.empty((B,), torch.int32)
-        res_cv = thr.empty((B,), torch.float32)
-        # slot s of the concatenated groups is row keep[s] of the batch, or padding (-1)
-        keep = numpy.full(G * N, -1, numpy.int64)
-        g0 = c0 = 0
-        for c, g in zip(counts, groups):
-            keep[g0 * N:g0 * N + c] = numpy.arange(c0, c0 + c)
-            g0, c0 = g0 + g, c0 + c
-        data = torch.cat([compacts[t].data.to(thr.device) for t in active]) if G else None
-        kss = [self._ks[t] for t in active]
-        fresh, mask_rnd, body_rnd, _ = compact.noise_terms(self.params)
-        step = compact.groups_per_pass(self.params)
-        for p0 in range(0, G, step):
-            p1 = min(G, p0 + step)
-            slots = keep[p0 * N:p1 * N]
-            rows = numpy.nonzero(slots >= 0)[0]
-            r0, r1 = int(slots[rows[0]]), int(slots[rows[-1]]) + 1      # the rows of a pass are consecutive
-            ea, eb = thr.compact_extract(data[p0:p1], (p1 - p0) * N)
-            if len(rows) < (p1 - p0) * N:
-                sel = thr.to_device(rows)
-                ea, eb = ea.index_select(0, sel), eb.index_select(0, sel)
-            cnt, pkss = self._pass_counts(counts, r0, r1, kss)
-            ra, rb, rcv = thr.mk_keyswitch(pkss, cnt, (ea, eb), want_cv=True)
-            del ea, eb
-            res_a[r0:r1], res_b[r0:r1] = ra, rb
-            res_cv[r0:r1] = rcv + (fresh + mask_rnd + body_rnd)
-        row = 0
-        for t, c in zip(active, counts):
-            shape = compacts[t].shape
-            out[t] = LweSampleArray(io_params, res_a[row:row + c].reshape(shape + (n,)), res_b[row:row + c].reshape(shape),
-                                    res_cv[row:row + c].reshape(shape))
-            row += c
-        return out
+        shapes = {t: compacts[t].shape for t in active}
+        counts = self._counts(active, shapes)
+        B = sum(counts)
+        res = (thr.empty((B, self.params.in_out_params.size), torch.int32), thr.empty((B,), torch.int32),
+               thr.empty((B,), torch.float32))
+        keys = TenantKeys(thr, [counts[t] for t in active], kss=[self._ks[t] for t in active])
+        compact.expand_groups(thr, self.params, keys, [compacts[t] for t in active], res)
+        return self._results(res, active, shapes, counts, None)
 
     @_in_rounds(('indexes',), ('table', 'dest'))
     def lookup(self, indexes, table, dest=None):
@@ -725,80 +601,31 @@ class MultiKeyVirtualMachine:
                 raise ValueError('tenant %d: lookup writes %d results of shape %s' % (t, W, indexes[t].shape))
         thr = self.thread
         n = self.params.in_out_params.size
-        counts = [int(numpy.prod(indexes[t].shape, dtype=numpy.int64)) for t in active]
-        offsets = numpy.concatenate([[0], numpy.cumsum(counts)]).astype(numpy.int64)
-        B = int(offsets[-1])
+        shapes = {t: indexes[t].shape for t in active}
+        all_counts = self._counts(active, shapes)
+        counts = [all_counts[t] for t in active]
+        B = sum(counts)
         sels = [indexes[t].samples.reshape(c, m, 2, 2, 2, index_lookup.N) for t, c in zip(active, counts)]
-        kss = [self._ks[t] for t in active]
-        tabs = [tables[t] for t in active] if per_tenant else [None] * len(active)
+        keys = TenantKeys(thr, counts, kss=[self._ks[t] for t in active])
         # column w of query q (of the concatenated batch) at row w B + q
         res_a, res_b = thr.empty((W * B, n), torch.int32), thr.empty((W * B,), torch.int32)
-        q0 = 0
-        while q0 < B:
-            step = index_lookup.queries_per_pass(m, W)
-            if per_tenant:          # as many queries as leave room for the tables of the tenants they belong to
-                k = 1
-                while True:
-                    step = index_lookup.queries_per_pass(m, W, k)
-                    k2 = len(self._pass_counts(counts, q0, min(B, q0 + step))[0])
-                    if k2 <= k:
-                        break
-                    k = k2
-            q1 = min(B, q0 + step)
+        for q0, q1, a, b in index_lookup.lookup_passes(thr, m, W, sels, None if per_tenant else table,
+                                                       [tables[t] for t in active] if per_tenant else None):
             Q = q1 - q0
-            cnt, pkss, psels, plos, ptabs = self._pass_counts(counts, q0, q1, kss, sels, offsets[:-1], tabs)
-            pieces = [s[max(q0, lo) - lo:][:c] for s, lo, c in zip(psels, plos, cnt)]
-            spec = thr.index_prepare(torch.cat(pieces) if len(pieces) > 1 else pieces[0]).reshape(Q, m, -1)
-            j0 = index_lookup.ROTATE_BITS
-            cur = table.polys if not per_tenant else None
-            if per_tenant:
-                # the pass's distinct tables, concatenated, and the table of every query
-                uniq = {}
-                slot = [uniq.setdefault(id(tb), (len(uniq), tb))[0] for tb in ptabs]
-                nodes = torch.cat([tb.nodes for _, tb in uniq.values()]) if len(uniq) > 1 else ptabs[0].nodes
-                nodes = nodes.reshape(len(uniq), -1, 2, index_lookup.N)
-                ids = numpy.repeat(numpy.asarray(slot, numpy.uint32), cnt)
-                if m > j0:
-                    cur = thr.index_cmux_level_indirect(nodes, ids, spec, j0, Q)
-                    j0 += 1
-            if cur is None:
-                a, b = thr.index_rotate_extract_indirect(nodes, ids, spec, m, W, Q)
-            else:
-                for j in range(j0, m):
-                    cur = thr.index_cmux_level(cur, spec, j, Q)
-                a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
-            del spec, cur
-            if per_tenant:
-                del nodes
+            pass_keys = keys.split(q0, q1)
             # rows (w, q) are column-major; the key switch wants each tenant's W c rows together, in vm.lookup's order
-            perm, lo = [], 0
-            for c in cnt:
-                perm.append((numpy.arange(W)[:, None] * Q + numpy.arange(lo, lo + c)[None, :]).reshape(-1))
-                lo += c
-            perm = numpy.concatenate(perm)
+            lo = numpy.cumsum([0] + pass_keys.counts)
+            perm = numpy.concatenate([(numpy.arange(W)[:, None] * Q + numpy.arange(lo[i], lo[i + 1])).reshape(-1)
+                                      for i in range(len(pass_keys.counts))])
             sel = thr.to_device(perm)
-            ra, rb, _ = thr.mk_keyswitch(pkss, [W * c for c in cnt], (a.reshape(W * Q, -1).index_select(0, sel),
-                                                                      b.reshape(W * Q).index_select(0, sel)))
+            ra, rb, _ = pass_keys.keyswitch((a.reshape(W * Q, -1).index_select(0, sel),
+                                             b.reshape(W * Q).index_select(0, sel)), per=W)
             dst = thr.to_device((perm // Q) * B + q0 + perm % Q)
             res_a.index_copy_(0, dst, ra)
             res_b.index_copy_(0, dst, rb)
-            q0 = q1
-        res_cv = thr.empty((W * B,), torch.float32).fill_(float(index_lookup.output_variance(self.params, m)))
-        for i, t in enumerate(active):
-            shape, lo, c = indexes[t].shape, int(offsets[i]), counts[i]
-            cols = []
-            for w in range(W):
-                r = slice(w * B + lo, w * B + lo + c)
-                if per_tenant:
-                    res_cv[r] = float(tables[t].variance + index_lookup.output_variance(self.params, m))
-                x = LweSampleArray(self.params.in_out_params, res_a[r].reshape(shape + (n,)), res_b[r].reshape(shape),
-                                   res_cv[r].reshape(shape))
-                if dest_lists is not None:
-                    d = dest_lists[t][w]
-                    d.a.copy_(x.a)
-                    d.b.copy_(x.b)
-                    d.current_variances.copy_(x.current_variances)
-                    x = d
-                cols.append(x)
-            out[t] = cols[0] if ref.single else cols
-        return out
+        res_cv = thr.empty((W, B), torch.float32).fill_(float(index_lookup.output_variance(self.params, m)))
+        if per_tenant:
+            for t, lo, c in zip(active, numpy.cumsum([0] + counts), counts):
+                res_cv[:, lo:lo + c] = float(tables[t].variance + index_lookup.output_variance(self.params, m))
+        return self._columns([(res_a[w * B:(w + 1) * B], res_b[w * B:(w + 1) * B], res_cv[w]) for w in range(W)],
+                             active, shapes, all_counts, dest_lists, ref.single)

@@ -21,6 +21,7 @@ from .tlwe import TLweKey, TLweSampleArray, tlwe_encrypt_zero_with_masks
 from .polynomials import IntPolynomialArray
 from .compressed import draw_seed, _check_tag, _variance, _wrap32
 from .random_numbers import rand_gaussian_torus32
+from .batch_keys import OneKey, group_rows
 
 NONCE_PACKING_KEY = 4
 PACK_LEVELS = 2                         # t
@@ -254,24 +255,45 @@ def pack(thr, packing_key: _GadgetKey, ciphertexts: LweSampleArray):
     n = params.in_out_params.size
     shape = tuple(ciphertexts.shape)
     batch = int(numpy.prod(shape, dtype=numpy.int64))
-    a = ciphertexts.a.reshape(batch, n)
-    b = ciphertexts.b.reshape(batch)
-    groups = -(-batch // N)
-    step = groups_per_pass(params)
-    if groups == 0:
+    if batch == 0:
         return PackedLweSampleArray(params, shape, thr.empty((0, k + 1, N), torch.uint16))
-    key = packing_key.spectra(thr)
-    out = thr.empty((groups, k + 1, N), torch.uint16) if groups > step else None
-    for g0 in range(0, groups, step):
-        c0, c1 = g0 * N, min(batch, (g0 + step) * N)
-        spec = thr.ntt_forward_i32(thr.pack_digits(a[c0:c1].contiguous()))
-        part = thr.pack_finish(thr.ntt_inverse_i32(thr.ntt_mac(spec, key)), b[c0:c1].contiguous())
+    keys = OneKey(thr, spectra=packing_key.spectra(thr))
+    return PackedLweSampleArray(params, shape, pack_groups(thr, params, keys, [(ciphertexts.a.reshape(batch, n),
+                                                                                 ciphertexts.b.reshape(batch))]))
+
+
+def pack_groups(thr, params, keys, parts):
+    """The packed groups (G, k + 1, N) uint16 of `parts`, one (a (c, n), b (c,)) per tenant of `keys` (batch_keys),
+    each starting at a group boundary, so a group never mixes tenants.  One part is packed in slices of itself; several
+    are gathered with a zero row in the slots that pad a tenant's last group, which packs exactly as an empty slot."""
+    tl, k, N = _glwe(params)
+    if len(parts) == 1:
+        (a, b), = parts
+        G = -(-b.shape[0] // N)
+    else:
+        counts = [b.shape[0] for a, b in parts]
+        groups, src = group_rows(counts, N, sum(counts))          # padding: the zero row after the last part
+        G, n = sum(groups), parts[0][0].shape[1]
+        a_all = torch.cat([a for a, b in parts] + [thr.empty((1, n), torch.int32).zero_()])
+        b_all = torch.cat([b for a, b in parts] + [thr.empty((1,), torch.int32).zero_()])
+        src = thr.to_device(src)
+    step = groups_per_pass(params)
+    out = None if len(parts) == 1 and 0 < G <= step else thr.empty((G, k + 1, N), torch.uint16)
+    for g0 in range(0, G, step):
+        g1 = min(G, g0 + step)
+        if len(parts) == 1:
+            xa, xb = a[g0 * N:g1 * N].contiguous(), b[g0 * N:g1 * N].contiguous()
+        else:
+            idx = src[g0 * N:g1 * N]
+            xa, xb = a_all.index_select(0, idx), b_all.index_select(0, idx)
+        spec = thr.ntt_forward_i32(thr.pack_digits(xa))
+        part = thr.pack_finish(thr.ntt_inverse_i32(keys.split(g0, g1).ntt_mac(spec)), xb)
         del spec
         if out is None:
             out = part
         else:       # (uint16 tensors are copied through their int16 view)
-            out.view(torch.int16)[g0:g0 + part.shape[0]].copy_(part.view(torch.int16))
-    return PackedLweSampleArray(params, shape, out)
+            out.view(torch.int16)[g0:g1].copy_(part.view(torch.int16))
+    return out
 
 
 def _check_pair(secret_key, packed):

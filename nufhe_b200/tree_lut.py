@@ -14,10 +14,10 @@ import torch
 from .lwe import LweSampleArray
 from .tlwe import TLweSampleArray, tlwe_extract_lwe_samples
 from .numeric_functions import t32_to_phase
-from .tgsw import engine_format
-from .bootstrap import blind_rotate, _single_kernel
+from .bootstrap import blind_rotate
 from .gates import check_shape
 from .packing import _GadgetKey, PACK_LEVELS, PACK_LOG2_BASE
+from .batch_keys import OneKey
 from . import lut
 
 NONCE_TREE_KEY = 5
@@ -179,7 +179,7 @@ class TreeLookupTable:
         return min(batch, max(1, ROWS_PER_PASS // self.groups)) * per
 
 
-def _level1(thr, bk, ks, table, d0, perf_params):
+def _level1(keys, table, d0):
     """(B, n) masks and (B,) bodies of one digit -> LWE (B, columns) of f(v, d_0) for every column v."""
     a, b = d0
     B, n = a.shape
@@ -188,11 +188,8 @@ def _level1(thr, bk, ks, table, d0, perf_params):
     ea_ = a[:, None, :].expand(B, Q, n).reshape(B * Q, n)
     eb_ = b[:, None].expand(B, Q).reshape(B * Q)
     tv = table.tv.reshape(Q, -1)[None].expand(B, Q, table.tv.shape[-1]).reshape(B * Q, -1)
-    if _single_kernel(perf_params, bk):
-        ea, eb = thr.bootstrap_lut_extract((ea_, eb_), None, 0, 1, 1, tv, L, engine_format(thr, bk.tgsw))
-    else:
-        ea, eb = lut._lut_steps(thr, bk, (ea_, eb_), None, 1, tv, L, B * Q, perf_params)
-    ra, rb, _ = thr.keyswitch(ks.device_arrays(), (ea, eb))
+    ea, eb = keys.bootstrap_lut_extract((ea_, eb_), None, 1, tv, L, per=Q)
+    ra, rb, _ = keys.keyswitch((ea, eb), per=Q * K)
     return ra.reshape(B, Q * K, n)[:, :table.columns], rb.reshape(B, Q * K)[:, :table.columns]
 
 
@@ -215,25 +212,41 @@ def _glwe_steps(thr, bk, x, tv, perf_params):
     return ext.a, ext.b
 
 
-def _level(thr, bk, ks, tree_key, bits, cur, digit, perf_params):
+def _level(keys, table, cur, digit):
     """One level >= 2: cur (B, W, n) / (B, W) LWE outputs whose last 2^bits entries differ in this level's digit ->
     (B, W / 2^bits, n) / (B, W / 2^bits)."""
     ca, cb = cur
     B, W, n = ca.shape
-    M = 1 << bits
-    k = bk.bk_params.tlwe_params.mask_size
+    M = 1 << table.bits
+    k = table.params.tgsw_params.tlwe_params.mask_size
     T = B * (W // M)
-    v = thr.tree_keyswitch(ca.reshape(B * W, n), tree_key.planes(thr), k)
-    tv = thr.tree_assemble(v.reshape(T, M, k + 1, -1), cb.reshape(T, M), bits)
+    v = keys.tree_keyswitch(ca.reshape(B * W, n), k, per=W)
+    tv = keys.thr.tree_assemble(v.reshape(T, M, k + 1, -1), cb.reshape(T, M), table.bits)
     da, db = digit
     xa = da[:, None, :].expand(B, W // M, n).reshape(T, n)
     xb = db[:, None].expand(B, W // M).reshape(T)
-    if _single_kernel(perf_params, bk):
-        ea, eb = thr.bootstrap_glwe_lut_extract((xa, xb), tv, engine_format(thr, bk.tgsw))
-    else:
-        ea, eb = _glwe_steps(thr, bk, (xa, xb), tv, perf_params)
-    ra, rb, _ = thr.keyswitch(ks.device_arrays(), (ea, eb))
+    ea, eb = keys.bootstrap_glwe_lut_extract((xa, xb), tv, per=W // M)
+    ra, rb, _ = keys.keyswitch((ea, eb), per=W // M)
     return ra.reshape(B, W // M, n), rb.reshape(B, W // M)
+
+
+def evaluate(keys, table, flat):
+    """The tree LUT on the batch `flat` (the D digits as (a (B, n), b (B,)), d_0 first) with `keys` (batch_keys):
+    out_a (B, F, n) and out_b (B, F), at most ROWS_PER_PASS level-1 bootstraps per pass."""
+    thr = keys.thr
+    B, n = flat[0][0].shape
+    out_a, out_b = thr.empty((B, table.functions, n), torch.int32), thr.empty((B, table.functions), torch.int32)
+    step = max(1, ROWS_PER_PASS // table.groups)
+    for c0 in range(0, B, step):
+        c1 = min(B, c0 + step)
+        part = [(a[c0:c1], b[c0:c1]) for a, b in flat]
+        pass_keys = keys.split(c0, c1)
+        cur = _level1(pass_keys, table, part[0])
+        for level in range(1, table.digits):
+            cur = _level(pass_keys, table, cur, part[level])
+        out_a[c0:c1].copy_(cur[0])
+        out_b[c0:c1].copy_(cur[1])
+    return out_a, out_b
 
 
 def lut_tree(thr, results, bk, ks, tree_key, table: TreeLookupTable, digits, perf_params=None):
@@ -263,23 +276,9 @@ def lut_tree(thr, results, bk, ks, tree_key, table: TreeLookupTable, digits, per
     for d in digits:
         if tuple(d.shape) != tuple(digits[0].shape):
             raise ValueError('all digits must have one shape, got %s and %s' % (tuple(digits[0].shape), tuple(d.shape)))
-    B = int(numpy.prod(shape, dtype=numpy.int64))
     flat = [lut._expand(d, shape) for d in reversed(digits)]    # d_0 first
-    F = table.functions
-    n = bk.in_out_params.size
-    out_a = thr.empty((B, F, n), torch.int32)
-    out_b = thr.empty((B, F), torch.int32)
-    step = max(1, ROWS_PER_PASS // table.groups)
-    for c0 in range(0, B, step):
-        c1 = min(B, c0 + step)
-        part = [(a[c0:c1], b[c0:c1]) for a, b in flat]
-        cur = _level1(thr, bk, ks, table, part[0], perf_params)
-        for level in range(1, table.digits):
-            cur = _level(thr, bk, ks, tree_key, table.bits, cur, part[level], perf_params)
-        out_a[c0:c1].copy_(cur[0])
-        out_b[c0:c1].copy_(cur[1])
-    out_a = out_a.reshape(shape + (F, n))
-    out_b = out_b.reshape(shape + (F,))
+    out_a, out_b = evaluate(OneKey(thr, bk, ks, perf_params, tree_key=tree_key), table, flat)
+    out_a, out_b = out_a.reshape(shape + out_a.shape[1:]), out_b.reshape(shape + out_b.shape[1:])
     for f, r in enumerate(results):
         r.a.copy_(out_a[..., f, :])
         r.b.copy_(out_b[..., f])
