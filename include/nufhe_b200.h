@@ -377,6 +377,30 @@ int nb_index_rotate_extract_indirect(nb_ctx *ctx, const int32_t *tables, size_t 
                                      const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
                                      int bits, size_t columns, int32_t *out_a, int32_t *out_b, size_t queries);
 
+/* ---- oblivious writes into encrypted tables (DESIGN.md section 21; no reference counterpart): the transpose of a
+ * lookup, on the same FP64 CMux step and selector spectra.
+ * nb_index_write_assemble: the delta of every query, (0, b) - V: v (queries, columns, 2, N) (the nb_tree_keyswitch
+ *     output of the values' masks; NULL for trivial values, V = 0) and b (queries, columns) -> out (queries, A, 2, N),
+ *     A = columns for bits >= 10 (one sample per column), A = 1 below (column w times X^(w 2^bits)).
+ * nb_index_write_rotate: for j < min(bits, 10), ACC <- ACC + sel_j[q] (x) ((X^(+2^j) - 1) ACC) on each of the A deltas
+ *     of query q (sel_j[q] as for nb_index_rotate_extract).  bits > 10: the samples go to out (queries, A, 2, N) and acc
+ *     must be NULL.  bits <= 10: sample c of query q is added (mod 2^32) into sample c of table table_ids_host[q] of
+ *     acc (acc_count tables of int32 GLWE samples, acc_stride words apart; table_ids_host NULL: one table), out unused.
+ * nb_index_demux_level: node y of in (queries, nodes, 2, N) becomes (y - sel[q] (x) y, sel[q] (x) y) at nodes 2i, 2i+1
+ *     of out (queries, 2 nodes, 2, N), or, with acc, is added into samples 2i, 2i+1 of the query's table (the last
+ *     level, bit 10).
+ * Adds are atomic, and sums mod 2^32 do not depend on their order.  NB_EINVAL for a NULL pointer, bits outside 1..20,
+ * columns 2^bits > N below 10 bits, acc given or missing against the rule above, a stride shorter than a table, an id
+ * >= acc_count or several tables without ids; queries = 0 is a no-op. */
+int nb_index_write_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, size_t columns, int32_t *out,
+                            size_t queries);
+int nb_index_write_rotate(nb_ctx *ctx, const int32_t *delta, const uint64_t *sel, size_t sel_query_stride, int bits,
+                          size_t columns, int32_t *out, int32_t *acc, size_t acc_stride, size_t acc_count,
+                          const uint32_t *table_ids_host, size_t queries);
+int nb_index_demux_level(nb_ctx *ctx, const int32_t *in, const uint64_t *sel, size_t sel_query_stride, int32_t *out,
+                         int32_t *acc, size_t acc_stride, size_t acc_count, const uint32_t *table_ids_host,
+                         size_t nodes, size_t queries);
+
 /* ---- compact public-key encryption (DESIGN.md section 16; no reference counterpart).  B messages go into
  * G = ceil(B / 1024) GLWE samples under the bootstrap key's GLWE key S (k + 1 polynomials of N = 1024 coefficients),
  * message c in group c / 1024, slot c % 1024, every coefficient rounded to 16 bits.  Encryption: nb_ntt_forward_i32 of

@@ -19,7 +19,7 @@ from .performance import PerformanceParameters
 from .computation_cache import clear_computation_cache
 from .gates import result_shape, get_shape
 from .engine import Engine
-from . import gates
+from . import gates, index_write
 
 
 def _check_api(api):
@@ -378,6 +378,30 @@ class VirtualMachine:
         (DESIGN.md sections 15 and 20).  TypeError for anything but an EncryptedIndexArray (decompress a compressed one
         first), ValueError for other parameters or a bit count other than the table's."""
         return lookup(self.thread, self.cloud_key.keyswitch_key, index, table, dest=dest)
+
+    def scatter_add(self, tree_key, table, index, values):
+        """T[w, idx_q] += v_q[w] for every index of the EncryptedIndexArray `index`, without learning which entries
+        change (DESIGN.md section 21); repeated indexes add up.  `table` is an out='int' EncryptedIndexTable, or an
+        IndexTable, which starts as the noiseless encryption of its entries.  `values` is an LweSampleArray (or a list
+        of W) of the index's shape under the cloud key, with `tree_key` the NuFHETreeKey of this machine, or plain
+        integers broadcast to the index's shape (tree_key=None), for counting.  Keeping sums below 2^bits is the
+        caller's job, as with int_add.  Returns a new EncryptedIndexTable.  TypeError as lookup, or for anything but a
+        NuFHETreeKey with LWE values; ValueError for a 'bool' table, other parameters or shapes, and for a result whose
+        lookups would keep less than lut.MARGIN_SIGMAS (refresh_table it first)."""
+        return index_write.scatter_add(self.thread, self.params, tree_key, table, index, values)
+
+    def write(self, tree_key, table, index, values):
+        """T[idx_q] <- v_q for every index (DESIGN.md section 21), on 'int' and 'bool' tables: scatter_add of
+        v_q - lookup(idx_q).  `values` as for scatter_add (plain values are 'bool' bits for a 'bool' table); the tree
+        key is needed either way.  Defined for distinct indexes: an entry that several queries name receives
+        old + sum_q (v_q - old).  Errors as scatter_add."""
+        return index_write.write(self.thread, self.params, self.cloud_key.keyswitch_key, tree_key, table, index, values)
+
+    def refresh_table(self, tree_key, table):
+        """The same entries with fresh noise: every entry extracted, key-switched and bootstrapped through an identity
+        vm.lut (W 2^m bootstraps), then packed again with make_encrypted_table.  Every write adds noise to every entry;
+        this is the way out when a write raises for lack of margin."""
+        return index_write.refresh_table(self, tree_key, table)
 
     def int_add(self, x, y, dest=None):
         """x + y of two integer ciphertexts without a bootstrap (the caller keeps the sum below 2^bits)."""

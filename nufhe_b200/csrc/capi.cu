@@ -203,6 +203,9 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
                         index_lookup_kernel<true, true>})
         NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<BrFft>()),
                      "cudaFuncSetAttribute(index_lookup)"));
+    for (auto kernel : {index_write_kernel<false>, index_write_kernel<true>})
+        NB_TRY(check(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)br_smem_bytes<BrFft>()),
+                     "cudaFuncSetAttribute(index_write)"));
     {   // batches that fit one wave of wide CTAs (one ciphertext on 256 threads) take the low-latency shape
         const char *e = getenv("NUFHE_B200_WIDE_MAX");
         // up to one wave the wide shape has the shortest step; between one and ~1.7 waves it still wins, time-sliced
@@ -1257,6 +1260,86 @@ int nb_index_rotate_extract_indirect(nb_ctx *ctx, const int32_t *tables, size_t 
     p.steps = bits < 10 ? bits : 10;
     p.log2_stride = bits;
     return index_launch(ctx, p, true, what, table_ids_host, table_count);
+}
+
+// ---- oblivious writes (index_lookup.cuh, DESIGN.md section 21) ----
+
+int nb_index_write_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int bits, size_t columns, int32_t *out,
+                            size_t queries)
+{
+    const char *what = "nb_index_write_assemble";
+    if (!ctx) return NB_EINVAL;
+    if (!b || !out) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
+    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    if (queries == 0) return NB_OK;
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:index_write_assemble");
+    const u64 total = (u64)queries * (bits >= 10 ? columns : 1) * 2 * NTT_N;
+    index_write_assemble_kernel<<<ew_grid(ctx, total), 256, 0, ctx->stream>>>(v, b, bits, (u32)columns, out, total);
+    return launch_check(ctx, "index_write_assemble_kernel");
+}
+
+// out or (acc, acc_stride, acc_count, table_ids_host): the last level adds into the tables instead of storing
+static int index_write_launch(nb_ctx *ctx, IndexWriteArgs &p, bool rotate, size_t out_nodes, size_t acc_count,
+                              const uint32_t *table_ids_host, const char *what)
+{
+    if (!p.in || !p.sel || (!p.out && !p.acc)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (p.acc && (acc_count == 0 || p.acc_stride < out_nodes * 2 * NTT_N || (!table_ids_host && acc_count != 1)))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": the tables overlap or are not named per query");
+    if (p.nodes == 0 || p.queries == 0) return NB_OK;
+    p.items = p.queries * p.nodes;
+    const size_t ctas = (p.items + BrFft::CT - 1) / BrFft::CT;
+    if (p.nodes > ((size_t)1 << 40) / p.queries || ctas > 0x7fffffffu)
+        return fail(ctx, NB_EINVAL, std::string(what) + ": too many items");
+    if (p.acc && table_ids_host)
+        for (size_t q = 0; q < p.queries; q++)
+            if (table_ids_host[q] >= acc_count)
+                return fail(ctx, NB_EINVAL, std::string(what) + ": query " + std::to_string(q) + " names table " +
+                                                std::to_string(table_ids_host[q]) + " of " + std::to_string(acc_count));
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range(rotate ? "nufhe_b200:index_write_rotate" : "nufhe_b200:index_demux_level");
+    p.fft_tab = ctx->d_fft_tab;
+    p.table_id = nullptr;
+    if (p.acc && table_ids_host) {
+        NB_TRY(mk_upload(ctx, table_ids_host, p.queries * sizeof(u32)));
+        p.table_id = reinterpret_cast<const u32 *>(ctx->d_mk);
+    }
+    const size_t smem = br_smem_bytes<BrFft>();
+    if (rotate) index_write_kernel<true><<<(unsigned)ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+    else index_write_kernel<false><<<(unsigned)ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+    return launch_check(ctx, what);
+}
+
+int nb_index_write_rotate(nb_ctx *ctx, const int32_t *delta, const uint64_t *sel, size_t sel_query_stride, int bits,
+                          size_t columns, int32_t *out, int32_t *acc, size_t acc_stride, size_t acc_count,
+                          const uint32_t *table_ids_host, size_t queries)
+{
+    const char *what = "nb_index_write_rotate";
+    if (!ctx) return NB_EINVAL;
+    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
+    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    if ((acc != nullptr) != (bits <= 10))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": the rotation adds into the tables exactly when bits <= 10");
+    IndexWriteArgs p{};
+    p.in = delta; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out = out; p.acc = acc; p.acc_stride = acc_stride; p.queries = queries;
+    p.nodes = bits >= 10 ? columns : 1;
+    p.steps = bits < 10 ? bits : 10;
+    return index_write_launch(ctx, p, true, p.nodes, acc_count, table_ids_host, what);
+}
+
+int nb_index_demux_level(nb_ctx *ctx, const int32_t *in, const uint64_t *sel, size_t sel_query_stride, int32_t *out,
+                         int32_t *acc, size_t acc_stride, size_t acc_count, const uint32_t *table_ids_host,
+                         size_t nodes, size_t queries)
+{
+    if (!ctx) return NB_EINVAL;
+    IndexWriteArgs p{};
+    p.in = in; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
+    p.out = acc ? nullptr : out; p.acc = acc; p.acc_stride = acc_stride; p.nodes = nodes; p.queries = queries;
+    return index_write_launch(ctx, p, false, 2 * nodes, acc_count, table_ids_host, "nb_index_demux_level");
 }
 
 // ---- compact public-key encryption (compact.cuh) ----

@@ -783,6 +783,74 @@ class Engine:
                        queries)
         return out_a, out_b
 
+    # --- oblivious writes (nufhe_b200/index_write.py) ---------------------------------------------
+    def index_write_assemble(self, v, b, bits):
+        """The delta of every query (nb_index_write_assemble): v (Q, W, 2, N) tree_keyswitch output or None for trivial
+        values, bodies b (Q, W) int32.  Returns (Q, A, 2, N), A = W for bits >= 10, else 1."""
+        b = self._dense(b, torch.int32)
+        if b.dim() != 2:
+            raise ValueError('index_write_assemble: bodies %s are not (queries, columns)' % (tuple(b.shape),))
+        Q, W = b.shape
+        if v is not None:
+            v = self._dense(v, torch.int32)
+            if tuple(v.shape) != (Q, W, 2, N):
+                raise ValueError('index_write_assemble: v %s for bodies %s' % (tuple(v.shape), tuple(b.shape)))
+        out = self.empty((Q, W if bits >= 10 else 1, 2, N), torch.int32)
+        if Q:
+            self._call('nb_index_write_assemble', _ptr(v), _ptr(b), int(bits), W, _ptr(out), Q)
+        return out
+
+    @staticmethod
+    def _write_tables(acc, table_ids, queries, what):
+        """(acc, stride, count, ids) of the accumulators acc (T, P, 2, N) int32 and the host ids (queries,) < T (None:
+        one table)."""
+        if acc is None:
+            return None, 0, 0, None
+        if acc.dim() != 4 or acc.shape[-2:] != (2, N) or not acc.is_contiguous() or acc.dtype != torch.int32:
+            raise ValueError('%s: accumulators %s %s are not contiguous int32 (T, P, 2, N)' % (what, acc.dtype, tuple(acc.shape)))
+        ids = None
+        if table_ids is not None:
+            ids = numpy.ascontiguousarray(table_ids, numpy.uint32).reshape(-1)
+            if ids.size != queries:
+                raise ValueError('%s: %d table ids for %d queries' % (what, ids.size, queries))
+        return acc, acc.shape[1] * 2 * N, acc.shape[0], ids
+
+    def index_write_rotate(self, delta, sel, bits, acc=None, table_ids=None):
+        """The rotation by X^(+idx mod 1024) of every delta (nb_index_write_rotate): delta (Q, A, 2, N), sel (Q, bits, R).
+        bits > 10: returns the rotated (Q, A, 2, N); bits <= 10: adds them into the accumulators acc (T, P, 2, N) in
+        place, query q into acc[table_ids[q]] (None: T = 1), and returns None."""
+        delta = self._dense(delta, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        Q, A = delta.shape[0], delta.shape[1]
+        if delta.dim() != 4 or delta.shape[-2:] != (2, N) or sel.dim() != 3 or sel.shape[1] != bits:
+            raise ValueError('index_write_rotate: deltas %s and selector spectra %s for %d bits'
+                             % (tuple(delta.shape), tuple(sel.shape), bits))
+        columns = A if bits >= 10 else 1
+        sp, sstride = self._index_sel(sel, 0, Q, 'index_write_rotate')
+        acc, astride, count, ids = self._write_tables(acc, table_ids, Q, 'index_write_rotate')
+        out = self.empty((Q, A, 2, N), torch.int32) if acc is None else None
+        if Q:
+            self._call('nb_index_write_rotate', _ptr(delta), sp, sstride, int(bits), columns, _ptr(out), _ptr(acc),
+                       astride, count, None if ids is None else ids.ctypes.data_as(ctypes.c_void_p), Q)
+        return out
+
+    def index_demux_level(self, x, sel, bit, acc=None, table_ids=None):
+        """One demultiplexer level (nb_index_demux_level): node y of x (Q, K, 2, N) becomes (y - C [x] y, C [x] y), C
+        the selector `bit` of sel (Q, m, R).  Returns (Q, 2 K, 2, N), or with acc (the last level) adds them into
+        acc[table_ids[q]] in place and returns None."""
+        x = self._dense(x, torch.int32)
+        sel = self._dense(sel, torch.int64)
+        if x.dim() != 4 or x.shape[-2:] != (2, N):
+            raise ValueError('index_demux_level: %s GLWE samples' % (tuple(x.shape),))
+        Q, K = x.shape[0], x.shape[1]
+        sp, sstride = self._index_sel(sel, bit, Q, 'index_demux_level')
+        acc, astride, count, ids = self._write_tables(acc, table_ids, Q, 'index_demux_level')
+        out = self.empty((Q, 2 * K, 2, N), torch.int32) if acc is None else None
+        if Q and K:
+            self._call('nb_index_demux_level', _ptr(x), sp, sstride, _ptr(out), _ptr(acc), astride, count,
+                       None if ids is None else ids.ctypes.data_as(ctypes.c_void_p), K, Q)
+        return out
+
     def lwe_affine(self, res, x1, x2, c, s1, s2):
         res_a, res_b = res
         B = res_b.numel()

@@ -118,6 +118,75 @@ def packing_variance(params):
     return key + n / 2 * 2.0**-32 / 12 + rounding_variance(params)
 
 
+def write_variance(params, m, lwe_values=True):
+    """What one query of a write adds to every entry of the table (DESIGN.md section 21): the m external products of its
+    rotation and demultiplexer, extracted_variance(m), and with LWE values the tree key's noise on every coefficient of
+    the delta, n t E[d^2] sigma^2 (the key term of test_vector_variance without the box sum)."""
+    tl = params.tgsw_params.tlwe_params
+    e_d2 = (2**(2 * packing.PACK_LOG2_BASE) - 1) / 12 + 0.25
+    key = params.in_out_params.size * packing.PACK_LEVELS * e_d2 * tl.min_noise**2 if lwe_values else 0.0
+    return extracted_variance(params, m) + key
+
+
+def value_variance(params, variance):
+    """What an LWE value of `variance` brings to the entry it is written to: its own noise and the truncation of its
+    mask to the tree key's 16 bits, (n / 2) 2^-32 / 12."""
+    return variance + params.in_out_params.size / 2 * 2.0**-32 / 12
+
+
+def table_sigma(params, leaf_variance, m, out):
+    """Standard deviation of the rounded phase of what a lookup result of the table feeds: a one-input vm.lut for an
+    'int' table, a two-input gate (the weight of lut's x + y inputs) for a 'bool' table."""
+    return lut_input_sigma(params, leaf_variance, m) if out == 'int' else lut_input_sigma(params, leaf_variance, m, 0, 0)
+
+
+def _box(out, bits_out):
+    return 2.0**-((bits_out if out == 'int' else 1) + 2)
+
+
+def check_table_variance(params, leaf_variance, m, out, bits_out):
+    """ValueError unless lookups into a table whose leaves carry `leaf_variance` keep lut.MARGIN_SIGMAS."""
+    margin = _box(out, bits_out) / table_sigma(params, leaf_variance, m, out)
+    if margin < lut.MARGIN_SIGMAS:
+        raise ValueError('the written table would keep %.1f sigma of noise margin on its lookups, below %d: '
+                         'refresh_table it first' % (margin, lut.MARGIN_SIGMAS))
+
+
+def max_table_variance(params, m, out, bits_out):
+    """The largest leaf variance check_table_variance accepts (negative when even a noiseless table falls short)."""
+    shift = None if out == 'int' else 0
+    weight = 1 if shift is None else 2
+    extra = ((_box(out, bits_out) / lut.MARGIN_SIGMAS)**2 - lut.lut_sigma(params, 0, shift)**2) / weight
+    return extra + lut.bootstrap_variance(params) - output_variance(params, m)
+
+
+def written_table_variance(params, leaf_variance, m, queries, value_variances=None, write=False):
+    """The leaf variance of a table after one call of `queries` queries: every entry gains queries * write_variance and
+    the 16-bit rounding.  scatter_add of LWE values (value_variances, one per query) adds them all, as repeated indexes
+    add up; `write` replaces its entries by values that carry their own noise and the lookup's, not the old leaf's."""
+    lwe = value_variances is not None
+    common = queries * write_variance(params, m, lwe) + rounding_variance(params)
+    if not lwe:
+        return leaf_variance + common
+    vv = [value_variance(params, v) for v in value_variances]
+    if write:
+        return max(leaf_variance, max(vv, default=0.0) + output_variance(params, m)) + common
+    return leaf_variance + sum(vv) + common
+
+
+def writes_before_refresh(params, m, out, bits_out, lwe_values=False):
+    """How many one-query calls a refreshed table (leaves of a bootstrap output plus packing_variance) takes before the
+    next would be refused: scatter_adds of plain counts, or (lwe_values) writes of bootstrap outputs."""
+    limit = max_table_variance(params, m, out, bits_out)
+    v = lut.bootstrap_variance(params) + packing_variance(params)
+    count = 0
+    while True:
+        v = written_table_variance(params, v, m, 1, [lut.bootstrap_variance(params)] if lwe_values else None, lwe_values)
+        if v > limit:
+            return count
+        count += 1
+
+
 def lut_input_sigma(params, leaf_variance, m, log2_outputs=0, shift=None):
     """Standard deviation of the rounded phase of a vm.lut input made of results of an m-bit lookup whose leaves carry
     `leaf_variance`: lut.lut_sigma (measured where larger) plus whatever such a result carries beyond a LUT output,
@@ -557,16 +626,16 @@ def queries_per_pass(m, columns, tables=0):
     return max(1, (PASS_BYTES - table_bytes) // (spectra + nodes))
 
 
-def lookup_passes(thr, m, W, sels, table=None, tables=None):
-    """The lookup_extracted samples of the queries of `sels` (selector arrays (c, m, 2, 2, 2, N), one per tenant, in
-    order) a pass at a time: yields q0, q1 and a (W, q1 - q0, N), b (W, q1 - q0) of queries [q0, q1).  Every query reads
-    `table`, or, with `tables` (one EncryptedIndexTable per tenant), its tenant's table from the first level on."""
+def selector_passes(thr, m, W, sels, per_tenant=False):
+    """The passes of a batch of queries (selector arrays (c, m, 2, 2, 2, N), one per tenant, in order) that lookups and
+    writes share: yields q0, q1, the tenants owning queries [q0, q1) and how many each owns, and the selector spectra
+    (q1 - q0, m, R) of those queries.  With `per_tenant` a pass leaves room for one table per tenant it serves."""
     counts = [s.shape[0] for s in sels]
     starts = numpy.cumsum([0] + counts)
     B = int(starts[-1])
     q0 = 0
     while q0 < B:
-        if tables is None:
+        if not per_tenant:
             step = queries_per_pass(m, W)
         else:           # as many queries as leave room for the tables of the tenants they belong to
             k = 1
@@ -581,6 +650,17 @@ def lookup_passes(thr, m, W, sels, table=None, tables=None):
         idx, own = owners(counts, q0, q1) if len(sels) > 1 else ([0], [Q])
         pieces = [sels[i][max(q0, starts[i]) - starts[i]:][:c] for i, c in zip(idx, own)]
         spec = thr.index_prepare(torch.cat(pieces) if len(pieces) > 1 else pieces[0]).reshape(Q, m, -1)
+        yield q0, q1, idx, own, spec
+        del spec, pieces            # one pass's spectra on the device at a time
+        q0 = q1
+
+
+def lookup_passes(thr, m, W, sels, table=None, tables=None):
+    """The lookup_extracted samples of the queries of `sels` (selector arrays (c, m, 2, 2, 2, N), one per tenant, in
+    order) a pass at a time: yields q0, q1 and a (W, q1 - q0, N), b (W, q1 - q0) of queries [q0, q1).  Every query reads
+    `table`, or, with `tables` (one EncryptedIndexTable per tenant), its tenant's table from the first level on."""
+    for q0, q1, idx, own, spec in selector_passes(thr, m, W, sels, tables is not None):
+        Q = q1 - q0
         j0 = ROTATE_BITS
         cur = _table_nodes(table)[0] if tables is None else None    # shared by every query until the first CMux level
         if tables is not None:
@@ -601,7 +681,6 @@ def lookup_passes(thr, m, W, sels, table=None, tables=None):
             a, b = thr.index_rotate_extract(cur, spec, m, W, Q)
         del spec, cur
         yield q0, q1, a, b
-        q0 = q1
 
 
 def lookup_extracted(thr, index, table):

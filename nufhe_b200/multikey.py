@@ -30,7 +30,7 @@ from .packing import NuFHEPackingKey, PackedLweSampleArray
 from .compact import CompactLweSampleArray
 from .index_lookup import EncryptedIndexArray, EncryptedIndexTable, IndexTable
 from .batch_keys import TenantKeys
-from . import compact, gates, index_lookup, packing, tree_lut
+from . import compact, gates, index_lookup, index_write, packing, tree_lut
 
 # gates that need no key: run per tenant
 _KEYLESS = {'not': 1, 'copy': 1, 'constant': 1}
@@ -629,3 +629,94 @@ class MultiKeyVirtualMachine:
                 res_cv[:, lo:lo + c] = float(tables[t].variance + index_lookup.output_variance(self.params, m))
         return self._columns([(res_a[w * B:(w + 1) * B], res_b[w * B:(w + 1) * B], res_cv[w]) for w in range(W)],
                              active, shapes, all_counts, dest_lists, ref.single)
+
+    def _write_operands(self, what, tree_keys, tables, indexes, values):
+        """Validate per-tenant writes: the active tenants (those with an index) and whether their values are LWE
+        samples.  Errors name the tenant."""
+        for name, lst in (('tree_keys', tree_keys), ('tables', tables), ('indexes', indexes), ('values', values)):
+            if not isinstance(lst, (list, tuple)) or len(lst) != self.tenants:
+                raise ValueError('%s must be a list of %d entries, one per tenant' % (name, self.tenants))
+        active = [t for t in range(self.tenants) if indexes[t] is not None]
+        kinds = set()
+        for t in active:
+            try:
+                kinds.add(index_write.check_arguments(what, self.params, indexes[t], tables[t], tree_keys[t], values[t]))
+            except (TypeError, ValueError) as e:
+                raise type(e)('tenant %d: %s' % (t, e)) from None
+            ref = tables[active[0]]
+            if (tables[t].bits, tables[t].columns) != (ref.bits, ref.columns):
+                raise ValueError('tenant %d: the tables of one call share m = %d and W = %d, got m = %d, W = %d'
+                                 % (t, ref.bits, ref.columns, tables[t].bits, tables[t].columns))
+        if len(kinds) > 1:
+            raise ValueError('the values of one call are all ciphertexts or all plain integers')
+        return active, bool(kinds) and kinds.pop()
+
+    def _scatter(self, what, tree_keys, tables, indexes, values, write_variances=None):
+        active, lwe = self._write_operands(what, tree_keys, tables, indexes, values)
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        ref = tables[active[0]]
+        m, W = ref.bits, ref.columns
+        counts, a, b, variances = [], [], [], []
+        for t in active:
+            if tables[t].out != 'int' and write_variances is None:
+                raise ValueError("tenant %d: scatter_add adds integers: it takes out='int' tables only (write overwrites "
+                                 "'bool' entries)" % t)
+            shape = indexes[t].shape
+            B = int(numpy.prod(shape, dtype=numpy.int64))
+            if lwe:
+                at, bt, var = index_write.lwe_values(self.params, shape, W, values[t])
+                a.append(at)
+            else:
+                bt, var = index_write.plain_values(thr, tables[t], shape, W, values[t]), None
+            if write_variances is not None:
+                var = write_variances[t]
+            v = index_lookup.written_table_variance(self.params, index_write.leaf_variance(tables[t]), m, B, var,
+                                                    write_variances is not None)
+            try:
+                index_lookup.check_table_variance(self.params, v, m, tables[t].out, tables[t].bits_out)
+            except ValueError as e:
+                raise ValueError('tenant %d: %s' % (t, e)) from None
+            counts.append(B)
+            b.append(bt)
+            variances.append(v)
+        accs = torch.stack([index_write.table_nodes(tables[t]) for t in active])
+        keys = TenantKeys(thr, counts, planes=[tree_keys[t].planes(thr) for t in active]) if lwe else None
+        sels = [indexes[t].samples.reshape(c, m, 2, 2, 2, index_lookup.N) for t, c in zip(active, counts)]
+        ids = numpy.repeat(numpy.arange(len(active), dtype=numpy.uint32), counts)
+        if sum(counts):
+            index_write.scatter_passes(thr, self.params, keys, m, W, sels, torch.cat(a) if lwe else None, torch.cat(b),
+                                       accs, ids)
+        for i, t in enumerate(active):
+            out[t] = index_write.finish(thr, self.params, tables[t], accs[i], variances[i])
+        return out
+
+    def scatter_add(self, tree_keys, tables, indexes, values):
+        """VirtualMachine.scatter_add for every tenant with an index (None: idle), one table per tenant (the tables of a
+        call share m and W): the queries of all tenants go through one tree key switch, rotation and demultiplexer per
+        pass, each adding into its tenant's table.  A list of EncryptedIndexTables aligned with the tenants, each
+        bit-identical to the tenant's own vm.scatter_add."""
+        return self._scatter('scatter_add', tree_keys, tables, indexes, values)
+
+    def write(self, tree_keys, tables, indexes, values):
+        """VirtualMachine.write for every tenant with an index: mk.lookup of the old entries, then one scatter of
+        v_q - old_q.  Each result is bit-identical to the tenant's own vm.write."""
+        active, _ = self._write_operands('write', tree_keys, tables, indexes, values)
+        for t in active:
+            if not isinstance(tree_keys[t], NuFHETreeKey):
+                raise TypeError('tenant %d: write needs a NuFHETreeKey (ctx.make_cloud_key(sk, tree_key=True)), got %s'
+                                % (t, type(tree_keys[t]).__name__))
+        if not active:
+            return [None] * self.tenants
+        if all(isinstance(tables[t], EncryptedIndexTable) for t in active):
+            old = self.lookup(indexes, [tables[t] if indexes[t] is not None else None for t in range(self.tenants)])
+        elif len({id(tables[t]) for t in active}) == 1:
+            old = self.lookup(indexes, tables[active[0]])
+        else:
+            raise ValueError('write takes one EncryptedIndexTable per tenant, or one IndexTable shared by all')
+        diffs, variances = [None] * self.tenants, [None] * self.tenants
+        for t in active:
+            diffs[t], variances[t] = index_write.differences(self.thread, tables[t], indexes[t].shape, old[t], values[t])
+        return self._scatter('write', tree_keys, tables, indexes, diffs, variances)
