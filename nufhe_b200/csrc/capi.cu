@@ -577,6 +577,8 @@ int nb_external_product(nb_ctx *ctx, int32_t *accum, const uint64_t *bk_int, siz
     return launch_check(ctx, "blind_rotate_kernel(plain external product)");
 }
 
+}  // extern "C"
+
 static int launch_blind_rotate(nb_ctx *ctx, BlindRotateArgs &p)
 {
     if (p.n <= 0 || p.n > LWE_N_MAX) return fail(ctx, NB_EUNSUPPORTED, "LWE dimension out of range");
@@ -589,12 +591,189 @@ static int launch_blind_rotate(nb_ctx *ctx, BlindRotateArgs &p)
     return launch_check(ctx, "blind_rotate_kernel");
 }
 
+// copy `bytes` of host data into the context's multi-key scratch (stream-ordered after every earlier launch that reads it)
+static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
+{
+    NB_TRY(reserve_words(ctx, &ctx->d_mk, &ctx->mk_bytes, bytes, 1));
+    return check(ctx, cudaMemcpyAsync(ctx->d_mk, host, bytes, cudaMemcpyHostToDevice, ctx->stream), "cudaMemcpyAsync(multi-key tables)");
+}
+
+// the two parts `names` of an optional operand are both given or both null
+static int check_pair(nb_ctx *ctx, const char *what, const void *a, const void *b, const char *names)
+{
+    if ((a == nullptr) != (b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": " + names + " must come together");
+    return NB_OK;
+}
+
+// entry t of each of the host tables `tables` is non-null for every tenant t
+template <class... T> static int mk_check_tenants(nb_ctx *ctx, const char *what, const char *kind, size_t tenants, T... tables)
+{
+    for (size_t t = 0; t < tenants; t++)
+        if (((tables[t] == nullptr) || ...))
+            return fail(ctx, NB_EINVAL, std::string(what) + ": null " + kind + " of tenant " + std::to_string(t));
+    return NB_OK;
+}
+
+// The first checks of a multi-key call over `batch` rows, tenant t owning counts[t] of them: the host tables (counts
+// and `tables`) are given while there are tenants, the counts add up to the batch, the operands are given unless the
+// batch is empty (`operands`), and so is every tenant's entry of `tables`.  All of it holds for an empty batch too.
+template <class... T>
+static int mk_preamble(nb_ctx *ctx, const char *what, const size_t *counts, size_t tenants, size_t batch, bool operands,
+                       const char *kind, T... tables)
+{
+    if (!ctx) return NB_EINVAL;
+    if (tenants && (!counts || ((tables == nullptr) || ...))) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    size_t sum = 0;
+    for (size_t t = 0; t < tenants; t++) sum += counts[t];
+    if (sum != batch)
+        return fail(ctx, NB_EINVAL, std::string(what) + ": the counts add up to " + std::to_string(sum) + ", not the batch " +
+                                        std::to_string(batch));
+    if (batch && !operands) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    return mk_check_tenants(ctx, what, kind, tenants, tables...);
+}
+
+// The common part of the multi-key bootstraps: p carries everything but the keys, for a batch of jobs x sum(counts)
+// ciphertexts whose job j covers rows [j B, (j + 1) B), split into tenants by the same counts.  Every tenant's key must lie
+// inside an engine key with FP64 spectra prepared on this context, or inside a slot nb_mk_bk_expand filled, since the
+// multi-key kernel runs the FP64 step.  The keys are checked before an empty batch returns.
+static int mk_blind_rotate(nb_ctx *ctx, const char *what, BlindRotateArgs &p, const uint64_t *const *bk,
+                           const size_t *counts, size_t tenants, size_t job_batch, int jobs)
+{
+    if (p.n <= 0 || p.n > LWE_N_MAX) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": LWE dimension out of range");
+    if (!ctx->fft) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": multi-key launches run the FP64 step, which NUFHE_B200_FFT=0 disables");
+    for (size_t t = 0; t < tenants; t++) {
+        const u64 *key = (const u64 *)bk[t];
+        for (const auto &k : ctx->multibit_keys)
+            if (k.first <= key && key < k.second)
+                return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": tenant " + std::to_string(t) + " has a multi-bit key");
+        bool spectral = false;
+        for (auto *keys : {&ctx->spectral_keys, &ctx->mk_slots})
+            for (const auto &k : *keys) spectral |= k.first <= key && key + (size_t)p.n * BK_ROW_U64 <= k.second;
+        if (!spectral)
+            return fail(ctx, NB_EINVAL, std::string(what) + ": the key of tenant " + std::to_string(t) +
+                                            " is not inside an engine key with FP64 spectra prepared on this context "
+                                            "or a slot filled by nb_mk_bk_expand");
+    }
+    if (p.batch == 0) return NB_OK;
+    // [tenant key pointers][tenant of each ciphertext]
+    std::vector<unsigned char> host(tenants * sizeof(const u64 *) + p.batch * sizeof(unsigned));
+    memcpy(host.data(), bk, tenants * sizeof(const u64 *));
+    unsigned *tenant_of = reinterpret_cast<unsigned *>(host.data() + tenants * sizeof(const u64 *));
+    for (int j = 0; j < jobs; j++) {
+        size_t c = (size_t)j * job_batch;
+        for (size_t t = 0; t < tenants; t++)
+            for (size_t i = 0; i < counts[t]; i++) tenant_of[c++] = (unsigned)t;
+    }
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:multikey_blind_rotate");
+    NB_TRY(mk_upload(ctx, host.data(), host.size()));
+    p.bk = nullptr;
+    p.mk_bk = reinterpret_cast<const u64 *const *>(ctx->d_mk);
+    p.mk_tenant = reinterpret_cast<const unsigned *>(reinterpret_cast<unsigned char *>(ctx->d_mk) + tenants * sizeof(const u64 *));
+    NB_TRY(launch_br_cfg<BrFftMk>(ctx, p));
+    return launch_check(ctx, "blind_rotate_kernel(multi-key)");
+}
+
+// The keys of a bootstrap: one engine key, or per-tenant keys (bk_host[t] serves counts[t] ciphertexts of every job)
+struct BrKeys {
+    bool multi = false;
+    const uint64_t *bk = nullptr;
+    const uint64_t *const *bk_host = nullptr;
+    const size_t *counts = nullptr;
+    size_t tenants = 0;
+
+    explicit BrKeys(const uint64_t *bk) : bk(bk) {}
+    BrKeys(const uint64_t *const *bk_host, const size_t *counts, size_t tenants) : multi(true), bk_host(bk_host), counts(counts), tenants(tenants) {}
+    // One key: an empty batch needs no check (empty arrays have no storage to check).  Per-tenant keys are checked
+    // even then, so that an empty launch validates them (MultiKeyVirtualMachine does).
+    bool nothing_to_do(const nb_ctx *ctx, size_t batch) const { return ctx && !multi && batch == 0; }
+    // the key tables and counts, and the operands, which `operands` says are all given
+    int check(nb_ctx *ctx, const char *what, bool operands, size_t batch) const
+    {
+        if (multi) return mk_preamble(ctx, what, counts, tenants, batch, operands, "key", bk_host);
+        if (!ctx || !operands || !bk) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+        return NB_OK;
+    }
+    // p's `jobs` jobs of `batch` ciphertexts each, extracted into out_a, out_b
+    int run(nb_ctx *ctx, const char *what, BlindRotateArgs &p, size_t n, int32_t *out_a, int32_t *out_b, size_t batch, int jobs) const
+    {
+        p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = jobs * batch;
+        if (multi) return mk_blind_rotate(ctx, what, p, bk_host, counts, tenants, batch, jobs);
+        p.bk = (const u64 *)bk;
+        return launch_blind_rotate(ctx, p);
+    }
+};
+
+// the operands of a gate-style job: x = (0, c) + s1 * in1 + s2 * in2, in2 optional
+struct GateJob { const int32_t *in1_a, *in1_b, *in2_a, *in2_b; int32_t c, s1, s2; };
+
+static void set_job(BlindRotateArgs &p, const GateJob &x)
+{
+    p.in1_a = x.in1_a; p.in1_b = x.in1_b; p.in2_a = x.in2_a; p.in2_b = x.in2_b; p.c = x.c; p.s1 = x.s1; p.s2 = x.s2;
+}
+
+static int bootstrap_extract(nb_ctx *ctx, const char *what, const BrKeys &keys, const GateJob &x, int32_t mu, size_t n,
+                             int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    if (keys.nothing_to_do(ctx, batch)) return NB_OK;
+    NB_TRY(keys.check(ctx, what, x.in1_a && x.in1_b && out_a && out_b, batch));
+    NB_TRY(check_pair(ctx, what, x.in2_a, x.in2_b, "in2_a/in2_b"));
+    BlindRotateArgs p{};
+    set_job(p, x);
+    p.mu = mu;
+    return keys.run(ctx, what, p, n, out_a, out_b, batch, 1);
+}
+
+// tv_stride 0: one test vector for the batch, 1024: one per ciphertext; 2^log2_outputs extracted samples per ciphertext
+static int bootstrap_lut_extract(nb_ctx *ctx, const char *what, const BrKeys &keys, const GateJob &x, const int32_t *tv,
+                                 size_t tv_stride, int log2_outputs, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    if (keys.nothing_to_do(ctx, batch)) return NB_OK;
+    NB_TRY(keys.check(ctx, what, x.in1_a && x.in1_b && tv && out_a && out_b, batch));
+    NB_TRY(check_pair(ctx, what, x.in2_a, x.in2_b, "in2_a/in2_b"));
+    if (tv_stride != 0 && tv_stride != (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tv_stride must be 0 or 1024");
+    if (log2_outputs < 0 || log2_outputs > 2) return fail(ctx, NB_EINVAL, std::string(what) + ": log2_outputs must be 0, 1 or 2");
+    BlindRotateArgs p{};
+    set_job(p, x);
+    p.tv = tv; p.tv_stride = tv_stride; p.log2_outputs = log2_outputs;
+    return keys.run(ctx, what, p, n, out_a, out_b, batch, 1);
+}
+
+static int bootstrap_glwe_lut_extract(nb_ctx *ctx, const char *what, const BrKeys &keys, const int32_t *in_a,
+                                      const int32_t *in_b, const int32_t *tv, size_t n, int32_t *out_a, int32_t *out_b,
+                                      size_t batch)
+{
+    if (keys.nothing_to_do(ctx, batch)) return NB_OK;
+    NB_TRY(keys.check(ctx, what, in_a && in_b && tv && out_a && out_b, batch));
+    BlindRotateArgs p{};
+    set_job(p, {in_a, in_b, nullptr, nullptr, 0, 1, 0});
+    p.tv = tv; p.tv_stride = 2 * (size_t)NTT_N; p.log2_outputs = 0;
+    return keys.run(ctx, what, p, n, out_a, out_b, batch, 1);
+}
+
+// two gate bootstraps in one launch: rows [0, batch) of the outputs are job a's, rows [batch, 2 batch) job b's
+static int bootstrap_extract2(nb_ctx *ctx, const char *what, const BrKeys &keys, const GateJob &a, const GateJob &b,
+                              int32_t mu, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    if (keys.nothing_to_do(ctx, batch)) return NB_OK;
+    NB_TRY(keys.check(ctx, what, a.in1_a && a.in1_b && b.in1_a && b.in1_b && out_a && out_b, batch));
+    NB_TRY(check_pair(ctx, what, a.in2_a, a.in2_b, "a/b parts"));
+    NB_TRY(check_pair(ctx, what, b.in2_a, b.in2_b, "a/b parts"));
+    BlindRotateArgs p{};
+    set_job(p, a);
+    p.j2_in1_a = b.in1_a; p.j2_in1_b = b.in1_b; p.j2_in2_a = b.in2_a; p.j2_in2_b = b.in2_b; p.j2_c = b.c; p.j2_s1 = b.s1; p.j2_s2 = b.s2;
+    p.mu = mu; p.job_batch = batch;
+    return keys.run(ctx, what, p, n, out_a, out_b, batch, 2);
+}
+
+extern "C" {
+
 int nb_blind_rotate(nb_ctx *ctx, const int32_t *accum, const int32_t *bara, const uint64_t *bk_int, size_t n,
                     int32_t *out_a, int32_t *out_b, int32_t *accum_out, size_t batch)
 {
     if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
     if (!ctx || !accum || !bara || !bk_int) return fail(ctx, NB_EINVAL, "nb_blind_rotate: null argument");
-    if ((out_a == nullptr) != (out_b == nullptr)) return fail(ctx, NB_EINVAL, "nb_blind_rotate: out_a/out_b must come together");
+    NB_TRY(check_pair(ctx, "nb_blind_rotate", out_a, out_b, "out_a/out_b"));
     BlindRotateArgs p{};
     p.accum = accum; p.bara = bara; p.bk = (const u64 *)bk_int; p.n = (int)n;
     p.out_a = out_a; p.out_b = out_b; p.accum_out = accum_out; p.extract = out_a != nullptr; p.batch = batch;
@@ -605,15 +784,8 @@ int nb_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b
                          const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
                          const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
 {
-    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
-    if (!ctx || !in1_a || !in1_b || !bk_int || !out_a || !out_b)
-        return fail(ctx, NB_EINVAL, "nb_bootstrap_extract: null argument");
-    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, "nb_bootstrap_extract: in2_a/in2_b must come together");
-    BlindRotateArgs p{};
-    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
-    p.c = c; p.s1 = s1; p.s2 = s2; p.mu = mu;
-    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return launch_blind_rotate(ctx, p);
+    return bootstrap_extract(ctx, "nb_bootstrap_extract", BrKeys(bk_int), {in1_a, in1_b, in2_a, in2_b, c, s1, s2}, mu,
+                             n, out_a, out_b, batch);
 }
 
 int nb_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
@@ -621,31 +793,14 @@ int nb_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *i
                              int log2_outputs, const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b,
                              size_t batch)
 {
-    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
-    if (!ctx || !in1_a || !in1_b || !tv || !bk_int || !out_a || !out_b)
-        return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: null argument");
-    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: in2_a/in2_b must come together");
-    if (tv_stride != 0 && tv_stride != (size_t)NTT_N) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: tv_stride must be 0 or 1024");
-    if (log2_outputs < 0 || log2_outputs > 2) return fail(ctx, NB_EINVAL, "nb_bootstrap_lut_extract: log2_outputs must be 0, 1 or 2");
-    BlindRotateArgs p{};
-    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
-    p.c = c; p.s1 = s1; p.s2 = s2;
-    p.tv = tv; p.tv_stride = tv_stride; p.log2_outputs = log2_outputs;
-    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return launch_blind_rotate(ctx, p);
+    return bootstrap_lut_extract(ctx, "nb_bootstrap_lut_extract", BrKeys(bk_int), {in1_a, in1_b, in2_a, in2_b, c, s1, s2},
+                                 tv, tv_stride, log2_outputs, n, out_a, out_b, batch);
 }
 
 int nb_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
                                   const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
 {
-    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
-    if (!ctx || !in_a || !in_b || !tv || !bk_int || !out_a || !out_b)
-        return fail(ctx, NB_EINVAL, "nb_bootstrap_glwe_lut_extract: null argument");
-    BlindRotateArgs p{};
-    p.in1_a = in_a; p.in1_b = in_b; p.c = 0; p.s1 = 1; p.s2 = 0;
-    p.tv = tv; p.tv_stride = 2 * (size_t)NTT_N; p.log2_outputs = 0;
-    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return launch_blind_rotate(ctx, p);
+    return bootstrap_glwe_lut_extract(ctx, "nb_bootstrap_glwe_lut_extract", BrKeys(bk_int), in_a, in_b, tv, n, out_a, out_b, batch);
 }
 
 int nb_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
@@ -654,39 +809,109 @@ int nb_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b,
                           int32_t b_s2, int32_t mu, const uint64_t *bk_int, size_t n, int32_t *out_a, int32_t *out_b,
                           size_t batch)
 {
-    if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
-    if (!ctx || !a1_a || !a1_b || !b1_a || !b1_b || !bk_int || !out_a || !out_b)
-        return fail(ctx, NB_EINVAL, "nb_bootstrap_extract2: null argument");
-    if ((a2_a == nullptr) != (a2_b == nullptr) || (b2_a == nullptr) != (b2_b == nullptr))
-        return fail(ctx, NB_EINVAL, "nb_bootstrap_extract2: a/b parts must come together");
-    BlindRotateArgs p{};
-    p.in1_a = a1_a; p.in1_b = a1_b; p.in2_a = a2_a; p.in2_b = a2_b; p.c = a_c; p.s1 = a_s1; p.s2 = a_s2;
-    p.j2_in1_a = b1_a; p.j2_in1_b = b1_b; p.j2_in2_a = b2_a; p.j2_in2_b = b2_b; p.j2_c = b_c; p.j2_s1 = b_s1; p.j2_s2 = b_s2;
-    p.mu = mu; p.job_batch = batch;
-    p.bk = (const u64 *)bk_int; p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = 2 * batch;
-    return launch_blind_rotate(ctx, p);
+    return bootstrap_extract2(ctx, "nb_bootstrap_extract2", BrKeys(bk_int), {a1_a, a1_b, a2_a, a2_b, a_c, a_s1, a_s2},
+                              {b1_a, b1_b, b2_a, b2_b, b_c, b_s1, b_s2}, mu, n, out_a, out_b, batch);
+}
+
+// ---- multi-key bootstraps (DESIGN.md section 17) ----
+
+int nb_mk_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                            const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
+                            const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants, size_t n,
+                            int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    return bootstrap_extract(ctx, "nb_mk_bootstrap_extract", BrKeys(bk_int_host, counts_host, tenants),
+                             {in1_a, in1_b, in2_a, in2_b, c, s1, s2}, mu, n, out_a, out_b, batch);
+}
+
+int nb_mk_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
+                             const int32_t *a2_b, int32_t a_c, int32_t a_s1, int32_t a_s2, const int32_t *b1_a,
+                             const int32_t *b1_b, const int32_t *b2_a, const int32_t *b2_b, int32_t b_c, int32_t b_s1,
+                             int32_t b_s2, int32_t mu, const uint64_t *const *bk_int_host, const size_t *counts_host,
+                             size_t tenants, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    return bootstrap_extract2(ctx, "nb_mk_bootstrap_extract2", BrKeys(bk_int_host, counts_host, tenants),
+                              {a1_a, a1_b, a2_a, a2_b, a_c, a_s1, a_s2}, {b1_a, b1_b, b2_a, b2_b, b_c, b_s1, b_s2}, mu, n, out_a, out_b, batch);
+}
+
+int nb_mk_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
+                                const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv,
+                                size_t tv_stride, int log2_outputs, const uint64_t *const *bk_int_host,
+                                const size_t *counts_host, size_t tenants, size_t n, int32_t *out_a, int32_t *out_b,
+                                size_t batch)
+{
+    return bootstrap_lut_extract(ctx, "nb_mk_bootstrap_lut_extract", BrKeys(bk_int_host, counts_host, tenants),
+                                 {in1_a, in1_b, in2_a, in2_b, c, s1, s2}, tv, tv_stride, log2_outputs, n, out_a, out_b, batch);
+}
+
+int nb_mk_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
+                                     const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants,
+                                     size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
+{
+    return bootstrap_glwe_lut_extract(ctx, "nb_mk_bootstrap_glwe_lut_extract", BrKeys(bk_int_host, counts_host, tenants),
+                                      in_a, in_b, tv, n, out_a, out_b, batch);
 }
 
 }  // extern "C"
 
-// The prepared planes of (ks_a, ks_b) when a fast-path key switch of `batch` ciphertexts runs as the tensor-core GEMM
-// (registered key, batch from ks_mma_min, rows aligned for its loads and stores), else null
-static const uint8_t *ks_gemm_planes(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src2_a, const int32_t *ks_a,
-                                     const int32_t *ks_b, const int32_t *res_a, size_t batch)
+// The prepared planes of the fast-shape key switch p when it runs as the tensor-core GEMM (registered key, batch from
+// ks_mma_min, rows aligned for its loads and stores), else null
+static const uint8_t *ks_gemm_planes(nb_ctx *ctx, const KeyswitchArgs &p)
 {
     const uint8_t *planes = nullptr;
-    if (batch >= ctx->ks_mma_min &&
-        (((uintptr_t)src1_a | (uintptr_t)(src2_a ? src2_a : src1_a)) & 15) == 0 && ((uintptr_t)res_a & 7) == 0)
+    if (p.batch >= ctx->ks_mma_min &&
+        (((uintptr_t)p.src1_a | (uintptr_t)(p.src2_a ? p.src2_a : p.src1_a)) & 15) == 0 && ((uintptr_t)p.res_a & 7) == 0)
         for (const auto &k : ctx->ks_keys)
-            if (k.ks_a == ks_a && k.ks_b == ks_b) planes = k.planes;
+            if (k.ks_a == p.ks_a && k.ks_b == p.ks_b) planes = k.planes;
     return planes;
 }
 
-// copy `bytes` of host data into the context's multi-key scratch (stream-ordered after every earlier launch that reads it)
-static int mk_upload(nb_ctx *ctx, const void *host, size_t bytes)
+// The key switch p as the tensor-core GEMM: tiles of 256 ciphertexts x 32 output columns; K is split over blockIdx.z
+// (partial sums meet in integer atomics) while a launch would leave half of the SMs idle
+static int ks_gemm(nb_ctx *ctx, const KeyswitchArgs &p, const uint8_t *planes)
 {
-    NB_TRY(reserve_words(ctx, &ctx->d_mk, &ctx->mk_bytes, bytes, 1));
-    return check(ctx, cudaMemcpyAsync(ctx->d_mk, host, bytes, cudaMemcpyHostToDevice, ctx->stream), "cudaMemcpyAsync(multi-key tables)");
+    KeyswitchMmaArgs m{};
+    m.src1_a = p.src1_a; m.src1_b = p.src1_b; m.src2_a = p.src2_a; m.src2_b = p.src2_b; m.c = p.c;
+    m.planes = planes; m.res_a = p.res_a; m.res_b = p.res_b; m.batch = p.batch;
+    const size_t tiles = (p.batch + KM_M - 1) / KM_M * KM_NTILES;
+    int splits = 1;
+    while (splits < 16 && tiles * (size_t)splits * 2 <= (size_t)ctx->sm_count) splits *= 2;
+    m.splits = splits;
+    if (splits > 1) {
+        NB_TRY(check(ctx, cudaMemsetAsync(p.res_a, 0, p.batch * p.n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+        NB_TRY(check(ctx, cudaMemsetAsync(p.res_b, 0, p.batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+    }
+    keyswitch_mma_kernel<<<dim3((unsigned)((p.batch + KM_M - 1) / KM_M), KM_NTILES, splits), KM_THREADS, KM_SMEM_BYTES,
+                           ctx->stream>>>(m);
+    if (p.res_cv) {
+        NB_TRY(launch_check(ctx, "keyswitch_mma_kernel"));
+        ks_cv_kernel<<<(unsigned)((p.batch + 31) / 32), 256, 0, ctx->stream>>>(p.src1_a, p.src2_a, p.ks_cv, p.res_cv, p.batch);
+    }
+    return launch_check(ctx, "keyswitch_mma_kernel");
+}
+
+// The key switch p on the gather kernel over `ctas` tiles: launch(grid) enqueues the kernel `what`.  The consumer loop
+// always walks KS_TILE ciphertext slots, so a CTA costs the same whatever its tile: the 1024 input coefficients are
+// split over blockIdx.y until the SMs are covered (partial sums meet in integer atomics).  One ciphertext: 128 CTAs x 8
+// coefficients.  Every output row is exact integer arithmetic and its variance the fixed-shape sum, so the split
+// changes no bit.
+template <class Launch> static int ks_gather(nb_ctx *ctx, KeyswitchArgs &p, size_t ctas, const char *what, Launch launch)
+{
+    const int splits = (int)std::min<size_t>(128, std::max<size_t>(1, (size_t)ctx->sm_count / ctas));
+    p.splits = splits;
+    if (splits > 1) {
+        NB_TRY(check(ctx, cudaMemsetAsync(p.res_a, 0, p.batch * p.n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+        NB_TRY(check(ctx, cudaMemsetAsync(p.res_b, 0, p.batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
+        if (p.res_cv) {
+            NB_TRY(reserve_words(ctx, (void **)&ctx->d_cv_blocks, &ctx->cv_words, p.batch * KS_CV_BLOCKS, sizeof(float)));
+            p.cv_blocks = ctx->d_cv_blocks;
+        }
+    }
+    NB_TRY(launch(dim3((unsigned)ctas, splits)));
+    NB_TRY(launch_check(ctx, what));
+    if (!p.cv_blocks) return NB_OK;
+    ks_cv_finalize_kernel<<<(int)((p.batch + 127) / 128), 128, 0, ctx->stream>>>(p.res_cv, p.cv_blocks, p.batch);
+    return launch_check(ctx, "ks_cv_finalize_kernel");
 }
 
 extern "C" {
@@ -699,68 +924,26 @@ int nb_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, cons
     if (ctx && batch == 0) return NB_OK;     // nothing to do: empty arrays have no storage to check
     if (!ctx || !src1_a || !src1_b || !ks_a || !ks_b || !ks_cv || !res_a || !res_b)
         return fail(ctx, NB_EINVAL, "nb_keyswitch: null argument");
-    if ((src2_a == nullptr) != (src2_b == nullptr)) return fail(ctx, NB_EINVAL, "nb_keyswitch: src2_a/src2_b must come together");
+    NB_TRY(check_pair(ctx, "nb_keyswitch", src2_a, src2_b, "src2_a/src2_b"));
     if (n + 1 > 512) return fail(ctx, NB_EUNSUPPORTED, "nb_keyswitch: output LWE dimension above 511");
     if (t < 1 || log2_base < 1 || t * log2_base > 31) return fail(ctx, NB_EINVAL, "nb_keyswitch: bad decomposition");
-    if (batch == 0) return NB_OK;
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:keyswitch");
     KeyswitchArgs p{};
     p.src1_a = src1_a; p.src1_b = src1_b; p.src2_a = src2_a; p.src2_b = src2_b; p.c = c;
     p.ks_a = ks_a; p.ks_b = ks_b; p.ks_cv = ks_cv; p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
     p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch;
-    const bool fast = t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N;
-    const uint8_t *planes = fast ? ks_gemm_planes(ctx, src1_a, src2_a, ks_a, ks_b, res_a, batch) : nullptr;
-    if (planes) {
-        // the GEMM: tiles of 256 ciphertexts x 32 output columns; K is split over blockIdx.z (partial sums meet in
-        // integer atomics) while a launch would leave half of the SMs idle
-        KeyswitchMmaArgs m{};
-        m.src1_a = src1_a; m.src1_b = src1_b; m.src2_a = src2_a; m.src2_b = src2_b; m.c = c;
-        m.planes = planes; m.res_a = res_a; m.res_b = res_b; m.batch = batch;
-        const size_t tiles = (batch + KM_M - 1) / KM_M * KM_NTILES;
-        int splits = 1;
-        while (splits < 16 && tiles * (size_t)splits * 2 <= (size_t)ctx->sm_count) splits *= 2;
-        m.splits = splits;
-        if (splits > 1) {
-            NB_TRY(check(ctx, cudaMemsetAsync(res_a, 0, batch * n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-            NB_TRY(check(ctx, cudaMemsetAsync(res_b, 0, batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-        }
-        keyswitch_mma_kernel<<<dim3((unsigned)((batch + KM_M - 1) / KM_M), KM_NTILES, splits), KM_THREADS, KM_SMEM_BYTES,
-                               ctx->stream>>>(m);
-        if (res_cv) {
-            NB_TRY(launch_check(ctx, "keyswitch_mma_kernel"));
-            ks_cv_kernel<<<(unsigned)((batch + 31) / 32), 256, 0, ctx->stream>>>(src1_a, src2_a, ks_cv, res_cv, batch);
-        }
-        return launch_check(ctx, "keyswitch_mma_kernel");
-    }
-    if (fast) {
-        // The consumer loop always walks KS_TILE ciphertext slots, so a CTA costs the same whatever its tile:
-        // fill the tiles, then split the 1024 input coefficients over blockIdx.y until the SMs are covered
-        // (partial sums meet in integer atomics).  One ciphertext: 128 CTAs x 8 coefficients.
-        size_t tile = batch < (size_t)KS_TILE ? batch : (size_t)KS_TILE;
-        p.tile = (int)tile;
-        int grid = (int)((batch + tile - 1) / tile);
-        int splits = ctx->sm_count / grid;
-        if (splits > 128) splits = 128;
-        if (splits < 1) splits = 1;
-        p.splits = splits;
-        if (splits > 1) {
-            NB_TRY(check(ctx, cudaMemsetAsync(res_a, 0, batch * n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-            NB_TRY(check(ctx, cudaMemsetAsync(res_b, 0, batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-        }
-        if (splits > 1 && res_cv) {
-            NB_TRY(reserve_words(ctx, (void **)&ctx->d_cv_blocks, &ctx->cv_words, batch * KS_CV_BLOCKS, sizeof(float)));
-            p.cv_blocks = ctx->d_cv_blocks;
-        }
-        keyswitch_kernel<<<dim3(grid, splits), KS_THREADS, KS_SMEM_BYTES, ctx->stream>>>(p);
-        if (p.cv_blocks) {
-            NB_TRY(launch_check(ctx, "keyswitch_kernel"));
-            ks_cv_finalize_kernel<<<(int)((batch + 127) / 128), 128, 0, ctx->stream>>>(res_cv, p.cv_blocks, batch);
-        }
-    } else {
+    if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N)) {
         keyswitch_generic_kernel<<<(int)batch, 512, 0, ctx->stream>>>(p);
+        return launch_check(ctx, "keyswitch_kernel");
     }
-    return launch_check(ctx, "keyswitch_kernel");
+    if (const uint8_t *planes = ks_gemm_planes(ctx, p)) return ks_gemm(ctx, p, planes);
+    const size_t tile = batch < (size_t)KS_TILE ? batch : (size_t)KS_TILE;
+    p.tile = (int)tile;
+    return ks_gather(ctx, p, (batch + tile - 1) / tile, "keyswitch_kernel", [&](dim3 grid) {
+        keyswitch_kernel<<<grid, KS_THREADS, KS_SMEM_BYTES, ctx->stream>>>(p);
+        return NB_OK;
+    });
 }
 
 size_t nb_ks_prepared_bytes(void) { return KM_PLANES_BYTES; }
@@ -1162,8 +1345,21 @@ int nb_index_prepare(nb_ctx *ctx, const int32_t *ggsw, size_t rows, uint64_t *sp
     return NB_OK;
 }
 
-static int index_launch(nb_ctx *ctx, IndexArgs &p, bool rotate, const char *what, const uint32_t *table_ids_host = nullptr,
-                        size_t tables = 0)
+}  // extern "C"
+
+// the bits of an index and the columns of a table: columns * 2^bits fit one polynomial below 10 bits
+static int index_check_bits(nb_ctx *ctx, const char *what, int bits, size_t columns)
+{
+    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
+    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
+        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    return NB_OK;
+}
+
+// One launch of the index kernel of the entry point `what` over p.queries x p.nodes items, BrFft::CT per CTA, enqueued by
+// launch(ctas, smem).  With table_ids_host, query q works on table table_ids_host[q]: each id is checked, then uploaded.
+template <class Args, class Launch>
+static int index_run(nb_ctx *ctx, const char *what, Args &p, const uint32_t *table_ids_host, size_t tables, Launch launch)
 {
     p.items = p.queries * p.nodes;
     const size_t ctas = (p.items + BrFft::CT - 1) / BrFft::CT;
@@ -1175,91 +1371,85 @@ static int index_launch(nb_ctx *ctx, IndexArgs &p, bool rotate, const char *what
                 return fail(ctx, NB_EINVAL, std::string(what) + ": query " + std::to_string(q) + " names table " +
                                                 std::to_string(table_ids_host[q]) + " of " + std::to_string(tables));
     NB_ON_DEVICE(ctx);
-    NvtxRange nvtx_range(rotate ? (table_ids_host ? "nufhe_b200:index_rotate_extract_indirect" : "nufhe_b200:index_rotate_extract")
-                                : (table_ids_host ? "nufhe_b200:index_cmux_level_indirect" : "nufhe_b200:index_cmux_level"));
+    NvtxRange nvtx_range(("nufhe_b200:" + std::string(what + 3)).c_str());     // named after the entry point
     p.fft_tab = ctx->d_fft_tab;
-    const dim3 grid((unsigned)ctas);
-    const size_t smem = br_smem_bytes<BrFft>();
     if (table_ids_host) {
         NB_TRY(mk_upload(ctx, table_ids_host, p.queries * sizeof(u32)));
         p.table_id = reinterpret_cast<const u32 *>(ctx->d_mk);
-        if (rotate) index_lookup_kernel<true, true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
-        else index_lookup_kernel<false, true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
-    } else if (rotate) {
-        index_lookup_kernel<true><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
-    } else {
-        index_lookup_kernel<false><<<grid, BrFft::THREADS, smem, ctx->stream>>>(p);
     }
+    launch((unsigned)ctas, br_smem_bytes<BrFft>());
     return launch_check(ctx, what);
 }
+
+// nb_index_cmux_level, and with `indirect` nb_index_cmux_level_indirect: query q reads table table_ids_host[q] < tables
+static int index_cmux_level(nb_ctx *ctx, const char *what, bool indirect, const int32_t *in, size_t in_stride,
+                            size_t tables, const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_stride,
+                            int32_t *out, size_t nodes, size_t queries)
+{
+    if (!ctx || !in || !sel || !out || (indirect && !table_ids_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    if (indirect && in_stride < 4 * nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
+    if (nodes == 0 || queries == 0) return NB_OK;
+    IndexArgs p{};
+    p.in = in; p.in_stride = in_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_stride;
+    p.out = out; p.nodes = nodes; p.queries = queries;
+    return index_run(ctx, what, p, table_ids_host, tables, [&](unsigned ctas, size_t smem) {
+        if (indirect) index_lookup_kernel<false, true><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+        else index_lookup_kernel<false><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+    });
+}
+
+// nb_index_rotate_extract, and with `indirect` nb_index_rotate_extract_indirect (tables as for index_cmux_level)
+static int index_rotate_extract(nb_ctx *ctx, const char *what, bool indirect, const int32_t *in, size_t in_stride,
+                                size_t tables, const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_stride,
+                                int bits, size_t columns, int32_t *out_a, int32_t *out_b, size_t queries)
+{
+    if (!ctx || !in || !sel || !out_a || !out_b || (indirect && !table_ids_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
+    NB_TRY(index_check_bits(ctx, what, bits, columns));
+    IndexArgs p{};
+    p.nodes = bits >= 10 ? columns : 1;
+    if (indirect && in_stride < 2 * p.nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
+    if (queries == 0) return NB_OK;
+    p.in = in; p.in_stride = in_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_stride;
+    p.out_a = out_a; p.out_b = out_b; p.queries = queries;
+    p.samples = bits >= 10 ? 1 : (int)columns;
+    p.steps = bits < 10 ? bits : 10;
+    p.log2_stride = bits;
+    return index_run(ctx, what, p, table_ids_host, tables, [&](unsigned ctas, size_t smem) {
+        if (indirect) index_lookup_kernel<true, true><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+        else index_lookup_kernel<true><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+    });
+}
+
+extern "C" {
 
 int nb_index_cmux_level(nb_ctx *ctx, const int32_t *in, size_t in_query_stride, const uint64_t *sel,
                         size_t sel_query_stride, int32_t *out, size_t nodes, size_t queries)
 {
-    if (!ctx) return NB_EINVAL;
-    if (!in || !sel || !out) return fail(ctx, NB_EINVAL, "nb_index_cmux_level: null argument");
-    if (nodes == 0 || queries == 0) return NB_OK;
-    IndexArgs p{};
-    p.in = in; p.in_stride = in_query_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
-    p.out = out; p.nodes = nodes; p.queries = queries;
-    return index_launch(ctx, p, false, "nb_index_cmux_level");
+    return index_cmux_level(ctx, "nb_index_cmux_level", false, in, in_query_stride, 0, nullptr, sel, sel_query_stride, out, nodes, queries);
 }
 
 int nb_index_rotate_extract(nb_ctx *ctx, const int32_t *acc, size_t acc_query_stride, const uint64_t *sel,
                             size_t sel_query_stride, int bits, size_t columns, int32_t *out_a, int32_t *out_b,
                             size_t queries)
 {
-    if (!ctx) return NB_EINVAL;
-    if (!acc || !sel || !out_a || !out_b) return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: null argument");
-    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: bits must be 1 to 20");
-    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
-        return fail(ctx, NB_EINVAL, "nb_index_rotate_extract: columns * 2^bits must be at most N below 10 bits");
-    if (queries == 0) return NB_OK;
-    IndexArgs p{};
-    p.in = acc; p.in_stride = acc_query_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
-    p.out_a = out_a; p.out_b = out_b; p.queries = queries;
-    p.nodes = bits >= 10 ? columns : 1;
-    p.samples = bits >= 10 ? 1 : (int)columns;
-    p.steps = bits < 10 ? bits : 10;
-    p.log2_stride = bits;
-    return index_launch(ctx, p, true, "nb_index_rotate_extract");
+    return index_rotate_extract(ctx, "nb_index_rotate_extract", false, acc, acc_query_stride, 0, nullptr, sel,
+                                sel_query_stride, bits, columns, out_a, out_b, queries);
 }
 
 int nb_index_cmux_level_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
                                  const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
                                  int32_t *out, size_t nodes, size_t queries)
 {
-    const char *what = "nb_index_cmux_level_indirect";
-    if (!ctx) return NB_EINVAL;
-    if (!tables || !table_ids_host || !sel || !out) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if (table_stride < 4 * nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
-    if (nodes == 0 || queries == 0) return NB_OK;
-    IndexArgs p{};
-    p.in = tables; p.in_stride = table_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
-    p.out = out; p.nodes = nodes; p.queries = queries;
-    return index_launch(ctx, p, false, what, table_ids_host, table_count);
+    return index_cmux_level(ctx, "nb_index_cmux_level_indirect", true, tables, table_stride, table_count, table_ids_host,
+                            sel, sel_query_stride, out, nodes, queries);
 }
 
 int nb_index_rotate_extract_indirect(nb_ctx *ctx, const int32_t *tables, size_t table_stride, size_t table_count,
                                      const uint32_t *table_ids_host, const uint64_t *sel, size_t sel_query_stride,
                                      int bits, size_t columns, int32_t *out_a, int32_t *out_b, size_t queries)
 {
-    const char *what = "nb_index_rotate_extract_indirect";
-    if (!ctx) return NB_EINVAL;
-    if (!tables || !table_ids_host || !sel || !out_a || !out_b) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
-    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
-    IndexArgs p{};
-    p.nodes = bits >= 10 ? columns : 1;
-    if (table_stride < 2 * p.nodes * (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tables overlap");
-    if (queries == 0) return NB_OK;
-    p.in = tables; p.in_stride = table_stride; p.sel = (const u64 *)sel; p.sel_stride = sel_query_stride;
-    p.out_a = out_a; p.out_b = out_b; p.queries = queries;
-    p.samples = bits >= 10 ? 1 : (int)columns;
-    p.steps = bits < 10 ? bits : 10;
-    p.log2_stride = bits;
-    return index_launch(ctx, p, true, what, table_ids_host, table_count);
+    return index_rotate_extract(ctx, "nb_index_rotate_extract_indirect", true, tables, table_stride, table_count,
+                                table_ids_host, sel, sel_query_stride, bits, columns, out_a, out_b, queries);
 }
 
 // ---- oblivious writes (index_lookup.cuh, DESIGN.md section 21) ----
@@ -1270,9 +1460,7 @@ int nb_index_write_assemble(nb_ctx *ctx, const int32_t *v, const int32_t *b, int
     const char *what = "nb_index_write_assemble";
     if (!ctx) return NB_EINVAL;
     if (!b || !out) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
-    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    NB_TRY(index_check_bits(ctx, what, bits, columns));
     if (queries == 0) return NB_OK;
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:index_write_assemble");
@@ -1289,27 +1477,10 @@ static int index_write_launch(nb_ctx *ctx, IndexWriteArgs &p, bool rotate, size_
     if (p.acc && (acc_count == 0 || p.acc_stride < out_nodes * 2 * NTT_N || (!table_ids_host && acc_count != 1)))
         return fail(ctx, NB_EINVAL, std::string(what) + ": the tables overlap or are not named per query");
     if (p.nodes == 0 || p.queries == 0) return NB_OK;
-    p.items = p.queries * p.nodes;
-    const size_t ctas = (p.items + BrFft::CT - 1) / BrFft::CT;
-    if (p.nodes > ((size_t)1 << 40) / p.queries || ctas > 0x7fffffffu)
-        return fail(ctx, NB_EINVAL, std::string(what) + ": too many items");
-    if (p.acc && table_ids_host)
-        for (size_t q = 0; q < p.queries; q++)
-            if (table_ids_host[q] >= acc_count)
-                return fail(ctx, NB_EINVAL, std::string(what) + ": query " + std::to_string(q) + " names table " +
-                                                std::to_string(table_ids_host[q]) + " of " + std::to_string(acc_count));
-    NB_ON_DEVICE(ctx);
-    NvtxRange nvtx_range(rotate ? "nufhe_b200:index_write_rotate" : "nufhe_b200:index_demux_level");
-    p.fft_tab = ctx->d_fft_tab;
-    p.table_id = nullptr;
-    if (p.acc && table_ids_host) {
-        NB_TRY(mk_upload(ctx, table_ids_host, p.queries * sizeof(u32)));
-        p.table_id = reinterpret_cast<const u32 *>(ctx->d_mk);
-    }
-    const size_t smem = br_smem_bytes<BrFft>();
-    if (rotate) index_write_kernel<true><<<(unsigned)ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
-    else index_write_kernel<false><<<(unsigned)ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
-    return launch_check(ctx, what);
+    return index_run(ctx, what, p, p.acc ? table_ids_host : nullptr, acc_count, [&](unsigned ctas, size_t smem) {
+        if (rotate) index_write_kernel<true><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+        else index_write_kernel<false><<<ctas, BrFft::THREADS, smem, ctx->stream>>>(p);
+    });
 }
 
 int nb_index_write_rotate(nb_ctx *ctx, const int32_t *delta, const uint64_t *sel, size_t sel_query_stride, int bits,
@@ -1318,9 +1489,7 @@ int nb_index_write_rotate(nb_ctx *ctx, const int32_t *delta, const uint64_t *sel
 {
     const char *what = "nb_index_write_rotate";
     if (!ctx) return NB_EINVAL;
-    if (bits < 1 || bits > 20) return fail(ctx, NB_EINVAL, std::string(what) + ": bits must be 1 to 20");
-    if (columns == 0 || (bits < 10 && (columns << bits) > (size_t)NTT_N))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": columns * 2^bits must be at most N below 10 bits");
+    NB_TRY(index_check_bits(ctx, what, bits, columns));
     if ((acc != nullptr) != (bits <= 10))
         return fail(ctx, NB_EINVAL, std::string(what) + ": the rotation adds into the tables exactly when bits <= 10");
     IndexWriteArgs p{};
@@ -1380,123 +1549,7 @@ int nb_compact_extract(nb_ctx *ctx, const uint16_t *data, int mask_size, int32_t
 
 // ---- multi-key calls (DESIGN.md section 17) --------------------------------------------------------------------
 
-// counts[0 .. tenants) must add up to `batch`
-static int mk_check_counts(nb_ctx *ctx, const char *what, const size_t *counts, size_t tenants, size_t batch)
-{
-    size_t sum = 0;
-    for (size_t t = 0; t < tenants; t++) sum += counts[t];
-    if (sum != batch)
-        return fail(ctx, NB_EINVAL, std::string(what) + ": the counts add up to " + std::to_string(sum) + ", not the batch " +
-                                        std::to_string(batch));
-    return NB_OK;
-}
-
-// The common part of the multi-key bootstraps: p carries everything but the keys, for a batch of jobs x sum(counts)
-// ciphertexts whose job j covers rows [j B, (j + 1) B), split into tenants by the same counts.  Every tenant's key must lie
-// inside an engine key with FP64 spectra prepared on this context, or inside a slot nb_mk_bk_expand filled, since the
-// multi-key kernel runs the FP64 step.  The keys are checked before an empty batch returns.
-static int mk_blind_rotate(nb_ctx *ctx, const char *what, BlindRotateArgs &p, const uint64_t *const *bk,
-                           const size_t *counts, size_t tenants, size_t job_batch, int jobs)
-{
-    if (p.n <= 0 || p.n > LWE_N_MAX) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": LWE dimension out of range");
-    if (!ctx->fft) return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": multi-key launches run the FP64 step, which NUFHE_B200_FFT=0 disables");
-    for (size_t t = 0; t < tenants; t++) {
-        const u64 *key = (const u64 *)bk[t];
-        if (!key) return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(t));
-        for (const auto &k : ctx->multibit_keys)
-            if (k.first <= key && key < k.second)
-                return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": tenant " + std::to_string(t) + " has a multi-bit key");
-        bool spectral = false;
-        for (auto *keys : {&ctx->spectral_keys, &ctx->mk_slots})
-            for (const auto &k : *keys) spectral |= k.first <= key && key + (size_t)p.n * BK_ROW_U64 <= k.second;
-        if (!spectral)
-            return fail(ctx, NB_EINVAL, std::string(what) + ": the key of tenant " + std::to_string(t) +
-                                            " is not inside an engine key with FP64 spectra prepared on this context "
-                                            "or a slot filled by nb_mk_bk_expand");
-    }
-    if (p.batch == 0) return NB_OK;
-    // [tenant key pointers][tenant of each ciphertext]
-    std::vector<unsigned char> host(tenants * sizeof(const u64 *) + p.batch * sizeof(unsigned));
-    memcpy(host.data(), bk, tenants * sizeof(const u64 *));
-    unsigned *tenant_of = reinterpret_cast<unsigned *>(host.data() + tenants * sizeof(const u64 *));
-    for (int j = 0; j < jobs; j++) {
-        size_t c = (size_t)j * job_batch;
-        for (size_t t = 0; t < tenants; t++)
-            for (size_t i = 0; i < counts[t]; i++) tenant_of[c++] = (unsigned)t;
-    }
-    NB_ON_DEVICE(ctx);
-    NvtxRange nvtx_range("nufhe_b200:multikey_blind_rotate");
-    NB_TRY(mk_upload(ctx, host.data(), host.size()));
-    p.bk = nullptr;
-    p.mk_bk = reinterpret_cast<const u64 *const *>(ctx->d_mk);
-    p.mk_tenant = reinterpret_cast<const unsigned *>(reinterpret_cast<unsigned char *>(ctx->d_mk) + tenants * sizeof(const u64 *));
-    NB_TRY(launch_br_cfg<BrFftMk>(ctx, p));
-    return launch_check(ctx, "blind_rotate_kernel(multi-key)");
-}
-
 extern "C" {
-
-int nb_mk_bootstrap_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
-                            const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, int32_t mu,
-                            const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants, size_t n,
-                            int32_t *out_a, int32_t *out_b, size_t batch)
-{
-    const char *what = "nb_mk_bootstrap_extract";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
-    if (batch && (!in1_a || !in1_b || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": in2_a/in2_b must come together");
-    BlindRotateArgs p{};
-    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
-    p.c = c; p.s1 = s1; p.s2 = s2; p.mu = mu;
-    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
-}
-
-int nb_mk_bootstrap_extract2(nb_ctx *ctx, const int32_t *a1_a, const int32_t *a1_b, const int32_t *a2_a,
-                             const int32_t *a2_b, int32_t a_c, int32_t a_s1, int32_t a_s2, const int32_t *b1_a,
-                             const int32_t *b1_b, const int32_t *b2_a, const int32_t *b2_b, int32_t b_c, int32_t b_s1,
-                             int32_t b_s2, int32_t mu, const uint64_t *const *bk_int_host, const size_t *counts_host,
-                             size_t tenants, size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
-{
-    const char *what = "nb_mk_bootstrap_extract2";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
-    if (batch && (!a1_a || !a1_b || !b1_a || !b1_b || !out_a || !out_b))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if ((a2_a == nullptr) != (a2_b == nullptr) || (b2_a == nullptr) != (b2_b == nullptr))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": a/b parts must come together");
-    BlindRotateArgs p{};
-    p.in1_a = a1_a; p.in1_b = a1_b; p.in2_a = a2_a; p.in2_b = a2_b; p.c = a_c; p.s1 = a_s1; p.s2 = a_s2;
-    p.j2_in1_a = b1_a; p.j2_in1_b = b1_b; p.j2_in2_a = b2_a; p.j2_in2_b = b2_b; p.j2_c = b_c; p.j2_s1 = b_s1; p.j2_s2 = b_s2;
-    p.mu = mu; p.job_batch = batch;
-    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = 2 * batch;
-    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 2);
-}
-
-int nb_mk_bootstrap_lut_extract(nb_ctx *ctx, const int32_t *in1_a, const int32_t *in1_b, const int32_t *in2_a,
-                                const int32_t *in2_b, int32_t c, int32_t s1, int32_t s2, const int32_t *tv,
-                                size_t tv_stride, int log2_outputs, const uint64_t *const *bk_int_host,
-                                const size_t *counts_host, size_t tenants, size_t n, int32_t *out_a, int32_t *out_b,
-                                size_t batch)
-{
-    const char *what = "nb_mk_bootstrap_lut_extract";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
-    if (batch && (!in1_a || !in1_b || !tv || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if ((in2_a == nullptr) != (in2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": in2_a/in2_b must come together");
-    if (tv_stride != 0 && tv_stride != (size_t)NTT_N) return fail(ctx, NB_EINVAL, std::string(what) + ": tv_stride must be 0 or 1024");
-    if (log2_outputs < 0 || log2_outputs > 2) return fail(ctx, NB_EINVAL, std::string(what) + ": log2_outputs must be 0, 1 or 2");
-    BlindRotateArgs p{};
-    p.in1_a = in1_a; p.in1_b = in1_b; p.in2_a = in2_a; p.in2_b = in2_b;
-    p.c = c; p.s1 = s1; p.s2 = s2;
-    p.tv = tv; p.tv_stride = tv_stride; p.log2_outputs = log2_outputs;
-    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
-}
 
 int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, const int32_t *src2_a,
                     const int32_t *src2_b, int32_t c, const int32_t *const *ks_a_host, const int32_t *const *ks_b_host,
@@ -1504,98 +1557,51 @@ int nb_mk_keyswitch(nb_ctx *ctx, const int32_t *src1_a, const int32_t *src1_b, c
                     int t, int log2_base, int32_t *res_a, int32_t *res_b, float *res_cv, size_t batch)
 {
     const char *what = "nb_mk_keyswitch";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!ks_a_host || !ks_b_host || !ks_cv_host || !counts_host))
-        return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
-    if (batch && (!src1_a || !src1_b || !res_a || !res_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    if ((src2_a == nullptr) != (src2_b == nullptr)) return fail(ctx, NB_EINVAL, std::string(what) + ": src2_a/src2_b must come together");
-    for (size_t k = 0; k < tenants; k++)
-        if (!ks_a_host[k] || !ks_b_host[k] || !ks_cv_host[k])
-            return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(k));
+    NB_TRY(mk_preamble(ctx, what, counts_host, tenants, batch, src1_a && src1_b && res_a && res_b, "key", ks_a_host,
+                       ks_b_host, ks_cv_host));
+    NB_TRY(check_pair(ctx, what, src2_a, src2_b, "src2_a/src2_b"));
     if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N))
         return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the grouped key switch is for in = 1024, n = 500, t = 8, base 4 only");
     if (batch == 0) return NB_OK;
     NB_ON_DEVICE(ctx);
     NvtxRange nvtx_range("nufhe_b200:multikey_keyswitch");
-    // tenants whose segment nb_keyswitch would run as the GEMM go there; the others become tiles of the gather kernel
+    KeyswitchArgs p{};
+    p.src1_a = src1_a; p.src1_b = src1_b; p.src2_a = src2_a; p.src2_b = src2_b; p.c = c;
+    p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
+    p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch; p.tile = KS_TILE;
+    // segments that nb_keyswitch would run as the GEMM run so on their own; the others become tiles of the gather kernel
     std::vector<KsTile> tiles;
-    std::vector<std::pair<size_t, size_t>> gemm;      // (tenant, first row)
+    std::vector<std::pair<KeyswitchArgs, const uint8_t *>> gemm;      // (segment, planes)
     size_t row = 0;
     for (size_t k = 0; k < tenants; row += counts_host[k], k++) {
         const size_t cnt = counts_host[k];
-        if (cnt && ks_gemm_planes(ctx, src1_a + row * KS_IN, src2_a ? src2_a + row * KS_IN : nullptr, ks_a_host[k],
-                                  ks_b_host[k], res_a + row * KS_N, cnt)) {
-            gemm.emplace_back(k, row);
+        KeyswitchArgs s = p;      // rows [row, row + cnt)
+        s.src1_a += row * KS_IN; s.src1_b += row; s.src2_a = src2_a ? src2_a + row * KS_IN : nullptr;
+        s.src2_b = src2_b ? src2_b + row : nullptr; s.res_a += row * KS_N; s.res_b += row; s.res_cv = res_cv ? res_cv + row : nullptr;
+        s.ks_a = ks_a_host[k]; s.ks_b = ks_b_host[k]; s.ks_cv = ks_cv_host[k]; s.batch = cnt;
+        if (const uint8_t *planes = cnt ? ks_gemm_planes(ctx, s) : nullptr) {
+            gemm.emplace_back(s, planes);
             continue;
         }
         for (size_t q = 0; q < cnt; q += KS_TILE)
             tiles.push_back({ks_a_host[k], ks_b_host[k], ks_cv_host[k], row + q, (int)std::min<size_t>(KS_TILE, cnt - q)});
     }
-    if (!tiles.empty()) {
-        // the split rule of nb_keyswitch over the tile count; every output row is exact integer arithmetic and its
-        // variance the fixed-shape sum, so the split changes no bit
-        KeyswitchArgs p{};
-        p.src1_a = src1_a; p.src1_b = src1_b; p.src2_a = src2_a; p.src2_b = src2_b; p.c = c;
-        p.res_a = res_a; p.res_b = res_b; p.res_cv = res_cv;
-        p.in_size = (int)in_size; p.n = (int)n; p.t = t; p.log2_base = log2_base; p.batch = batch; p.tile = KS_TILE;
-        int splits = (int)std::min<size_t>(128, (size_t)ctx->sm_count / tiles.size());
-        if (splits < 1) splits = 1;
-        p.splits = splits;
-        if (splits > 1) {
-            // (the GEMM segments are written after this, by their own launches)
-            NB_TRY(check(ctx, cudaMemsetAsync(res_a, 0, batch * n * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-            NB_TRY(check(ctx, cudaMemsetAsync(res_b, 0, batch * sizeof(int32_t), ctx->stream), "cudaMemsetAsync"));
-            if (res_cv) {
-                NB_TRY(reserve_words(ctx, (void **)&ctx->d_cv_blocks, &ctx->cv_words, batch * KS_CV_BLOCKS, sizeof(float)));
-                p.cv_blocks = ctx->d_cv_blocks;
-            }
-        }
-        NB_TRY(mk_upload(ctx, tiles.data(), tiles.size() * sizeof(KsTile)));
-        keyswitch_grouped_kernel<<<dim3((unsigned)tiles.size(), splits), KS_THREADS, KS_SMEM_BYTES, ctx->stream>>>(
-            p, reinterpret_cast<const KsTile *>(ctx->d_mk));
-        NB_TRY(launch_check(ctx, "keyswitch_grouped_kernel"));
-        if (p.cv_blocks) {
-            // over the whole batch: the rows of GEMM segments get their variances from ks_cv_kernel after this
-            ks_cv_finalize_kernel<<<(int)((batch + 127) / 128), 128, 0, ctx->stream>>>(res_cv, p.cv_blocks, batch);
-            NB_TRY(launch_check(ctx, "ks_cv_finalize_kernel"));
-        }
-    }
-    for (const auto &g : gemm) {
-        const size_t k = g.first, r = g.second;
-        NB_TRY(nb_keyswitch(ctx, src1_a + r * KS_IN, src1_b + r, src2_a ? src2_a + r * KS_IN : nullptr,
-                            src2_b ? src2_b + r : nullptr, c, ks_a_host[k], ks_b_host[k], ks_cv_host[k], in_size, n, t,
-                            log2_base, res_a + r * KS_N, res_b + r, res_cv ? res_cv + r : nullptr, counts_host[k]));
-    }
+    // the gather launch zeroes and finalizes the variances of the whole batch: the GEMM segments are written after it
+    if (!tiles.empty())
+        NB_TRY(ks_gather(ctx, p, tiles.size(), "keyswitch_grouped_kernel", [&](dim3 grid) {
+            NB_TRY(mk_upload(ctx, tiles.data(), tiles.size() * sizeof(KsTile)));
+            keyswitch_grouped_kernel<<<grid, KS_THREADS, KS_SMEM_BYTES, ctx->stream>>>(p, reinterpret_cast<const KsTile *>(ctx->d_mk));
+            return NB_OK;
+        }));
+    for (const auto &g : gemm) NB_TRY(ks_gemm(ctx, g.first, g.second));
     return NB_OK;
-}
-
-int nb_mk_bootstrap_glwe_lut_extract(nb_ctx *ctx, const int32_t *in_a, const int32_t *in_b, const int32_t *tv,
-                                     const uint64_t *const *bk_int_host, const size_t *counts_host, size_t tenants,
-                                     size_t n, int32_t *out_a, int32_t *out_b, size_t batch)
-{
-    const char *what = "nb_mk_bootstrap_glwe_lut_extract";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!bk_int_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, batch));
-    if (batch && (!in_a || !in_b || !tv || !out_a || !out_b)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    BlindRotateArgs p{};
-    p.in1_a = in_a; p.in1_b = in_b; p.c = 0; p.s1 = 1; p.s2 = 0;
-    p.tv = tv; p.tv_stride = 2 * (size_t)NTT_N; p.log2_outputs = 0;
-    p.n = (int)n; p.out_a = out_a; p.out_b = out_b; p.extract = 1; p.batch = batch;
-    return mk_blind_rotate(ctx, what, p, bk_int_host, counts_host, tenants, batch, 1);
 }
 
 int nb_mk_tree_keyswitch(nb_ctx *ctx, const int32_t *a, const uint8_t *const *planes_host, const size_t *counts_host,
                          size_t tenants, size_t n, int mask_size, int32_t *out, size_t rows)
 {
     const char *what = "nb_mk_tree_keyswitch";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!planes_host || !counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, counts_host, tenants, rows));
-    if (rows && (!a || !out)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    for (size_t t = 0; t < tenants; t++)
-        if (!planes_host[t]) return fail(ctx, NB_EINVAL, std::string(what) + ": null planes of tenant " + std::to_string(t));
+    NB_TRY(mk_preamble(ctx, what, counts_host, tenants, rows, a && out, "planes", planes_host));
     NB_TRY(tree_check_shape(ctx, n, mask_size, what));
     if (rows == 0) return NB_OK;
     std::vector<TreeTile> tiles(mk_tree_tiles(counts_host, tenants, planes_host, nullptr));
@@ -1615,12 +1621,7 @@ int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_hos
                   size_t tenants, uint64_t *out, size_t rows, size_t outs, size_t groups)
 {
     const char *what = "nb_mk_ntt_mac";
-    if (!ctx) return NB_EINVAL;
-    if (tenants && (!key_host || !group_counts_host)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    NB_TRY(mk_check_counts(ctx, what, group_counts_host, tenants, groups));
-    if (groups && (!x || !out)) return fail(ctx, NB_EINVAL, std::string(what) + ": null argument");
-    for (size_t t = 0; t < tenants; t++)
-        if (!key_host[t]) return fail(ctx, NB_EINVAL, std::string(what) + ": null key of tenant " + std::to_string(t));
+    NB_TRY(mk_preamble(ctx, what, group_counts_host, tenants, groups, x && out, "key", key_host));
     if (rows == 0 || outs == 0 || rows > (1u << 24) || outs > (1u << 16))
         return fail(ctx, NB_EINVAL, std::string(what) + ": rows must be in [1, 2^24] and outputs in [1, 2^16]");
     if (groups == 0) return NB_OK;
@@ -1649,9 +1650,7 @@ int nb_mk_bk_expand(nb_ctx *ctx, const uint32_t *seeds_host, const int32_t *cons
     if (mask_size != 1 || decomp_length != 2 || poly_degree != (size_t)NTT_N || n == 0 || n > (size_t)LWE_N_MAX)
         return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the expansion is for k = 1, l = 2, N = 1024 and 1 <= n <= " +
                                               std::to_string(LWE_N_MAX) + " only");
-    for (size_t t = 0; t < tenants; t++)
-        if (!bodies_host[t] || !slots_host[t])
-            return fail(ctx, NB_EINVAL, std::string(what) + ": null bodies or slot of tenant " + std::to_string(t));
+    NB_TRY(mk_check_tenants(ctx, what, "bodies or slot", tenants, bodies_host, slots_host));
     if (tenants == 0) return NB_OK;
     if (tenants * n * 8 > 0x7fffffffu) return fail(ctx, NB_EINVAL, std::string(what) + ": too many rows in one call");
     std::vector<MkBkTenant> table(tenants);
@@ -1684,8 +1683,7 @@ int nb_mk_ks_expand(nb_ctx *ctx, const uint32_t *seeds_host, int32_t *const *ks_
     if (!(t == 8 && log2_base == 2 && in_size == (size_t)KS_IN && n == (size_t)KS_N))
         return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": the expansion is for the multi-key key switch, in = 1024, "
                                                              "n = 500, t = 8, base 4 only");
-    for (size_t k = 0; k < tenants; k++)
-        if (!ks_a_host[k]) return fail(ctx, NB_EINVAL, std::string(what) + ": null ks_a of tenant " + std::to_string(k));
+    NB_TRY(mk_check_tenants(ctx, what, "ks_a", tenants, ks_a_host));
     if (tenants == 0) return NB_OK;
     if (tenants > 65535) return fail(ctx, NB_EINVAL, std::string(what) + ": more than 65535 tenants in one call");
     std::vector<MkKsTenant> table(tenants);

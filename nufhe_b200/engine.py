@@ -88,6 +88,14 @@ class Engine:
         assert t.is_cuda and t.dtype == dtype, (t.device, t.dtype, dtype)
         return t if t.is_contiguous() else t.contiguous()
 
+    def _lwe(self, *samples):
+        """[a1, b1, a2, b2, ...]: the parts of the LWE samples (a, b) as dense int32 tensors, None for both parts of an
+        absent sample (the C calls take null pointers).  The tensors must outlive the call they are passed to."""
+        parts = []
+        for x in samples:
+            parts += [None, None] if x is None else [self._dense(x[0], torch.int32), self._dense(x[1], torch.int32)]
+        return parts
+
     # --- transforms -----------------------------------------------------------------------
     def ntt_forward_i32(self, x):
         x = self._dense(x, torch.int32)
@@ -164,67 +172,67 @@ class Engine:
 
     def bootstrap_extract(self, x1, x2, c, s1, s2, mu, bk_int, out=None):
         """x = (0,c) + s1*x1 + s2*x2 (x2 may be None); returns the extracted sample (a (B,1024), b (B,))."""
-        a1, b1 = x1
-        a1 = self._dense(a1, torch.int32)
-        b1 = self._dense(b1, torch.int32)
-        a2 = b2 = None
-        if x2 is not None:
-            a2 = self._dense(x2[0], torch.int32)
-            b2 = self._dense(x2[1], torch.int32)
-        B = b1.numel()
-        n = a1.shape[-1]
-        out_a, out_b = out if out is not None else (self.empty((B, N), torch.int32), self.empty((B,), torch.int32))
-        self._call('nb_bootstrap_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
-                   int(mu), _ptr(bk_int), n, _ptr(out_a), _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_extract('nb_bootstrap_extract', x1, x2, c, s1, s2, mu, (_ptr(bk_int),), out)
 
     def bootstrap_lut_extract(self, x1, x2, c, s1, s2, tv, log2_outputs, bk_int):
         """The programmable bootstrap of x = (0,c) + s1*x1 + s2*x2 (x2 may be None) with test vector `tv`: (1024,) int32
         for the whole batch or (B, 1024) for one per ciphertext.  Returns the 2^L extracted samples of every ciphertext,
         a (B * 2^L, 1024) and b (B * 2^L,), sample j of ciphertext c in row c * 2^L + j (nb_bootstrap_lut_extract)."""
-        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-        a2 = b2 = None
-        if x2 is not None:
-            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-        tv = self._dense(tv, torch.int32)
-        B = b1.numel()
-        n = a1.shape[-1]
-        stride = 0 if tv.dim() == 1 else N
-        assert tv.shape[-1] == N and (stride == 0 or tv.numel() == B * N), (tuple(tv.shape), B)
-        rows = B << int(log2_outputs)
-        out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
-        self._call('nb_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
-                   _ptr(tv), stride, int(log2_outputs), _ptr(bk_int), n, _ptr(out_a), _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_lut_extract('nb_bootstrap_lut_extract', x1, x2, c, s1, s2, tv, log2_outputs,
+                                           (_ptr(bk_int),))
 
     def bootstrap_extract2(self, job_a, job_b, mu, bk_int):
         """Two bootstraps in one launch.  job = (x1, x2, c, s1, s2) as for bootstrap_extract.
         Returns two extracted samples (views of one (2B, 1024) / (2B,) allocation)."""
-        def parts(job):
-            x1, x2, c, s1, s2 = job
-            a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-            a2 = b2 = None
-            if x2 is not None:
-                a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-            return a1, b1, a2, b2, int(c), int(s1), int(s2)
-        pa, pb = parts(job_a), parts(job_b)
+        return self._bootstrap_extract2('nb_bootstrap_extract2', job_a, job_b, mu, (_ptr(bk_int),))
+
+    # the bootstraps of one engine key (keys = (bk_int pointer,)) or of several tenants (keys = _mk_keys(...))
+    def _bootstrap_extract(self, name, x1, x2, c, s1, s2, mu, keys, out=None):
+        parts = self._lwe(x1, x2)
+        a1, b1 = parts[:2]
+        B = b1.numel()
+        out_a, out_b = out if out is not None else (self.empty((B, N), torch.int32), self.empty((B,), torch.int32))
+        self._call(name, *map(_ptr, parts), int(c), int(s1), int(s2), int(mu), *keys, a1.shape[-1], _ptr(out_a),
+                   _ptr(out_b), B)
+        return out_a, out_b
+
+    def _bootstrap_lut_extract(self, name, x1, x2, c, s1, s2, tv, log2_outputs, keys):
+        parts = self._lwe(x1, x2)
+        a1, b1 = parts[:2]
+        tv = self._dense(tv, torch.int32)
+        B = b1.numel()
+        stride = 0 if tv.dim() == 1 else N
+        assert tuple(tv.shape) == ((N,) if stride == 0 else (B, N)), (tuple(tv.shape), B)
+        rows = B << int(log2_outputs)
+        out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
+        self._call(name, *map(_ptr, parts), int(c), int(s1), int(s2), _ptr(tv), stride, int(log2_outputs), *keys,
+                   a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
+        return out_a, out_b
+
+    def _bootstrap_glwe_lut_extract(self, name, x, tv, keys):
+        a, b = self._lwe(x)
+        tv = self._dense(tv, torch.int32)
+        B = b.numel()
+        n = a.shape[-1]
+        if tuple(tv.shape) != (B, 2, N) or a.numel() != B * n:
+            raise ValueError('%s: tv %s for %d ciphertexts' % (name[3:], tuple(tv.shape), B))
+        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
+        self._call(name, _ptr(a), _ptr(b), _ptr(tv), *keys, n, _ptr(out_a), _ptr(out_b), B)
+        return out_a, out_b
+
+    def _bootstrap_extract2(self, name, job_a, job_b, mu, keys):
+        (x1, x2, c, s1, s2), (y1, y2, d, t1, t2) = job_a, job_b
+        pa, pb = self._lwe(x1, x2), self._lwe(y1, y2)
         B = pa[1].numel()
-        n = pa[0].shape[-1]
         out_a, out_b = self.empty((2 * B, N), torch.int32), self.empty((2 * B,), torch.int32)
-        self._call('nb_bootstrap_extract2', _ptr(pa[0]), _ptr(pa[1]), _ptr(pa[2]), _ptr(pa[3]), pa[4], pa[5], pa[6],
-                   _ptr(pb[0]), _ptr(pb[1]), _ptr(pb[2]), _ptr(pb[3]), pb[4], pb[5], pb[6], int(mu), _ptr(bk_int), n,
-                   _ptr(out_a), _ptr(out_b), B)
+        self._call(name, *map(_ptr, pa), int(c), int(s1), int(s2), *map(_ptr, pb), int(d), int(t1), int(t2), int(mu),
+                   *keys, pa[0].shape[-1], _ptr(out_a), _ptr(out_b), B)
         return (out_a[:B], out_b[:B]), (out_a[B:], out_b[B:])
 
     def keyswitch(self, ks, src1, src2=None, c=0, out=None, want_cv=False):
         ks_a, ks_b, ks_cv = ks
         in_size, t, base, n = ks_a.shape
-        a1 = self._dense(src1[0], torch.int32)
-        b1 = self._dense(src1[1], torch.int32)
-        a2 = b2 = None
-        if src2 is not None:
-            a2 = self._dense(src2[0], torch.int32)
-            b2 = self._dense(src2[1], torch.int32)
+        a1, b1, a2, b2 = self._lwe(src1, src2)
         B = b1.numel()
         if out is None:
             res_a = self.empty(tuple(b1.shape) + (n,), torch.int32)
@@ -249,49 +257,18 @@ class Engine:
     def mk_bootstrap_extract(self, x1, x2, c, s1, s2, mu, bk_ints, counts):
         """bootstrap_extract over the ciphertexts of several keys: bk_ints[t] (bk_prepare) serves the counts[t]
         ciphertexts of tenant t, which follow those of tenant t - 1 (nb_mk_bootstrap_extract)."""
-        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-        a2 = b2 = None
-        if x2 is not None:
-            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-        B = b1.numel()
-        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
-        keys, cnt, T = self._mk_keys(bk_ints, counts)
-        self._call('nb_mk_bootstrap_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
-                   int(mu), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_extract('nb_mk_bootstrap_extract', x1, x2, c, s1, s2, mu, self._mk_keys(bk_ints, counts))
 
     def mk_bootstrap_lut_extract(self, x1, x2, c, s1, s2, tv, log2_outputs, bk_ints, counts):
         """bootstrap_lut_extract over the ciphertexts of several keys, split as for mk_bootstrap_extract
         (nb_mk_bootstrap_lut_extract); tv (1024,) serves the whole batch, tv (B, 1024) holds one per ciphertext."""
-        a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-        a2 = b2 = None
-        if x2 is not None:
-            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-        tv = self._dense(tv, torch.int32)
-        B = b1.numel()
-        stride = 0 if tv.dim() == 1 else N
-        assert tuple(tv.shape) == ((N,) if stride == 0 else (B, N)), (tuple(tv.shape), B)
-        rows = B << int(log2_outputs)
-        out_a, out_b = self.empty((rows, N), torch.int32), self.empty((rows,), torch.int32)
-        keys, cnt, T = self._mk_keys(bk_ints, counts)
-        self._call('nb_mk_bootstrap_lut_extract', _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2), int(c), int(s1), int(s2),
-                   _ptr(tv), stride, int(log2_outputs), keys, cnt, T, a1.shape[-1], _ptr(out_a), _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_lut_extract('nb_mk_bootstrap_lut_extract', x1, x2, c, s1, s2, tv, log2_outputs,
+                                           self._mk_keys(bk_ints, counts))
 
     def mk_bootstrap_glwe_lut_extract(self, x, tv, bk_ints, counts):
         """bootstrap_glwe_lut_extract over the ciphertexts of several keys, split as for mk_bootstrap_extract
         (nb_mk_bootstrap_glwe_lut_extract)."""
-        a, b = self._dense(x[0], torch.int32), self._dense(x[1], torch.int32)
-        tv = self._dense(tv, torch.int32)
-        B = b.numel()
-        n = a.shape[-1]
-        if tuple(tv.shape) != (B, 2, N) or a.numel() != B * n:
-            raise ValueError('mk_bootstrap_glwe_lut_extract: tv %s for %d ciphertexts' % (tuple(tv.shape), B))
-        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
-        keys, cnt, T = self._mk_keys(bk_ints, counts)
-        self._call('nb_mk_bootstrap_glwe_lut_extract', _ptr(a), _ptr(b), _ptr(tv), keys, cnt, T, n, _ptr(out_a),
-                   _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_glwe_lut_extract('nb_mk_bootstrap_glwe_lut_extract', x, tv, self._mk_keys(bk_ints, counts))
 
     def mk_tree_keyswitch(self, a, planes, counts, mask_size):
         """tree_keyswitch over the rows of several tenants: planes[t] (tree_prepare) serves the counts[t] rows of tenant
@@ -329,30 +306,13 @@ class Engine:
     def mk_bootstrap_extract2(self, job_a, job_b, mu, bk_ints, counts):
         """bootstrap_extract2 over the ciphertexts of several keys: both jobs are split by the same counts
         (nb_mk_bootstrap_extract2).  Returns the two samples as views of one allocation."""
-        def parts(job):
-            x1, x2, c, s1, s2 = job
-            a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-            a2 = b2 = None
-            if x2 is not None:
-                a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-            return a1, b1, a2, b2, int(c), int(s1), int(s2)
-        pa, pb = parts(job_a), parts(job_b)
-        B = pa[1].numel()
-        out_a, out_b = self.empty((2 * B, N), torch.int32), self.empty((2 * B,), torch.int32)
-        keys, cnt, T = self._mk_keys(bk_ints, counts)
-        self._call('nb_mk_bootstrap_extract2', _ptr(pa[0]), _ptr(pa[1]), _ptr(pa[2]), _ptr(pa[3]), pa[4], pa[5], pa[6],
-                   _ptr(pb[0]), _ptr(pb[1]), _ptr(pb[2]), _ptr(pb[3]), pb[4], pb[5], pb[6], int(mu), keys, cnt, T,
-                   pa[0].shape[-1], _ptr(out_a), _ptr(out_b), B)
-        return (out_a[:B], out_b[:B]), (out_a[B:], out_b[B:])
+        return self._bootstrap_extract2('nb_mk_bootstrap_extract2', job_a, job_b, mu, self._mk_keys(bk_ints, counts))
 
     def mk_keyswitch(self, keys, counts, src1, src2=None, c=0, want_cv=False):
         """keyswitch over the ciphertexts of several keys: keys[t] = (ks_a, ks_b, ks_cv) of tenant t serves its counts[t]
         rows (nb_mk_keyswitch).  Returns res_a (B, n), res_b (B,) and the variances (B,) or None."""
         in_size, t, base, n = keys[0][0].shape if keys else (0, 0, 0, 0)
-        a1, b1 = self._dense(src1[0], torch.int32), self._dense(src1[1], torch.int32)
-        a2 = b2 = None
-        if src2 is not None:
-            a2, b2 = self._dense(src2[0], torch.int32), self._dense(src2[1], torch.int32)
+        a1, b1, a2, b2 = self._lwe(src1, src2)
         B = b1.numel()
         res_a, res_b = self.empty((B, n), torch.int32), self.empty((B,), torch.int32)
         res_cv = self.empty((B,), torch.float32) if want_cv else None
@@ -677,16 +637,7 @@ class Engine:
     def bootstrap_glwe_lut_extract(self, x, tv, bk_int):
         """The programmable bootstrap of x = (a (B, n), b (B,)) with per-ciphertext GLWE test vectors tv (B, 2, N):
         returns the extracted samples a (B, N), b (B,) (nb_bootstrap_glwe_lut_extract)."""
-        a, b = self._dense(x[0], torch.int32), self._dense(x[1], torch.int32)
-        tv = self._dense(tv, torch.int32)
-        B = b.numel()
-        n = a.shape[-1]
-        if tuple(tv.shape) != (B, 2, N) or a.numel() != B * n:
-            raise ValueError('bootstrap_glwe_lut_extract: tv %s for %d ciphertexts' % (tuple(tv.shape), B))
-        out_a, out_b = self.empty((B, N), torch.int32), self.empty((B,), torch.int32)
-        self._call('nb_bootstrap_glwe_lut_extract', _ptr(a), _ptr(b), _ptr(tv), _ptr(bk_int), n, _ptr(out_a),
-                   _ptr(out_b), B)
-        return out_a, out_b
+        return self._bootstrap_glwe_lut_extract('nb_bootstrap_glwe_lut_extract', x, tv, (_ptr(bk_int),))
 
     # --- encrypted-index lookups (nufhe_b200/index_lookup.py) -----------------------------------
     def index_prepare(self, ggsw):
@@ -718,13 +669,7 @@ class Engine:
         x = self._dense(x, torch.int32)
         sel = self._dense(sel, torch.int64)
         pairs, stride = self._index_nodes(x, queries, 'index_cmux_level')
-        if pairs % 2:
-            raise ValueError('index_cmux_level: an odd node count %d' % pairs)
-        sp, sstride = self._index_sel(sel, bit, queries, 'index_cmux_level')
-        out = self.empty((queries, pairs // 2, 2, N), torch.int32)
-        if queries and pairs:
-            self._call('nb_index_cmux_level', _ptr(x), stride, sp, sstride, _ptr(out), pairs // 2, queries)
-        return out
+        return self._index_cmux('nb_index_cmux_level', (_ptr(x), stride), pairs, sel, bit, queries)
 
     def index_rotate_extract(self, acc, sel, bits, columns, queries):
         """Rotation by the low index bits and extraction (nb_index_rotate_extract): acc (queries, A, 2, N) or (A, 2, N)
@@ -733,15 +678,7 @@ class Engine:
         acc = self._dense(acc, torch.int32)
         sel = self._dense(sel, torch.int64)
         accs, stride = self._index_nodes(acc, queries, 'index_rotate_extract')
-        if accs != (columns if bits >= 10 else 1) or sel.dim() != 3 or sel.shape[1] != bits:
-            raise ValueError('index_rotate_extract: %d accumulators and %s selector spectra for %d columns of %d bits'
-                             % (accs, tuple(sel.shape), columns, bits))
-        sp, sstride = self._index_sel(sel, 0, queries, 'index_rotate_extract')
-        out_a, out_b = self.empty((columns, queries, N), torch.int32), self.empty((columns, queries), torch.int32)
-        if queries:
-            self._call('nb_index_rotate_extract', _ptr(acc), stride, sp, sstride, int(bits), columns, _ptr(out_a),
-                       _ptr(out_b), queries)
-        return out_a, out_b
+        return self._index_rotate('nb_index_rotate_extract', (_ptr(acc), stride), accs, sel, bits, columns, queries)
 
     @staticmethod
     def _index_tables(tables, table_ids, queries, what):
@@ -757,14 +694,8 @@ class Engine:
         tables = self._dense(tables, torch.int32)
         sel = self._dense(sel, torch.int64)
         count, pairs, stride, ids = self._index_tables(tables, table_ids, queries, 'index_cmux_level_indirect')
-        if pairs % 2:
-            raise ValueError('index_cmux_level_indirect: an odd node count %d' % pairs)
-        sp, sstride = self._index_sel(sel, bit, queries, 'index_cmux_level_indirect')
-        out = self.empty((queries, pairs // 2, 2, N), torch.int32)
-        if queries and pairs:
-            self._call('nb_index_cmux_level_indirect', _ptr(tables), stride, count, ids.ctypes.data_as(ctypes.c_void_p),
-                       sp, sstride, _ptr(out), pairs // 2, queries)
-        return out
+        return self._index_cmux('nb_index_cmux_level_indirect',
+                                (_ptr(tables), stride, count, ids.ctypes.data_as(ctypes.c_void_p)), pairs, sel, bit, queries)
 
     def index_rotate_extract_indirect(self, tables, table_ids, sel, bits, columns, queries):
         """index_rotate_extract with query q reading tables[table_ids[q]] (nb_index_rotate_extract_indirect): tables
@@ -772,15 +703,28 @@ class Engine:
         tables = self._dense(tables, torch.int32)
         sel = self._dense(sel, torch.int64)
         count, accs, stride, ids = self._index_tables(tables, table_ids, queries, 'index_rotate_extract_indirect')
+        return self._index_rotate('nb_index_rotate_extract_indirect',
+                                  (_ptr(tables), stride, count, ids.ctypes.data_as(ctypes.c_void_p)), accs, sel, bits,
+                                  columns, queries)
+
+    # the direct and _indirect calls: `src` holds the arguments that name their inputs, a pointer first
+    def _index_cmux(self, name, src, pairs, sel, bit, queries):
+        if pairs % 2:
+            raise ValueError('%s: an odd node count %d' % (name[3:], pairs))
+        sp, sstride = self._index_sel(sel, bit, queries, name[3:])
+        out = self.empty((queries, pairs // 2, 2, N), torch.int32)
+        if queries and pairs:
+            self._call(name, *src, sp, sstride, _ptr(out), pairs // 2, queries)
+        return out
+
+    def _index_rotate(self, name, src, accs, sel, bits, columns, queries):
         if accs != (columns if bits >= 10 else 1) or sel.dim() != 3 or sel.shape[1] != bits:
-            raise ValueError('index_rotate_extract_indirect: %d accumulators and %s selector spectra for %d columns of %d '
-                             'bits' % (accs, tuple(sel.shape), columns, bits))
-        sp, sstride = self._index_sel(sel, 0, queries, 'index_rotate_extract_indirect')
+            raise ValueError('%s: %d accumulators and %s selector spectra for %d columns of %d bits'
+                             % (name[3:], accs, tuple(sel.shape), columns, bits))
+        sp, sstride = self._index_sel(sel, 0, queries, name[3:])
         out_a, out_b = self.empty((columns, queries, N), torch.int32), self.empty((columns, queries), torch.int32)
         if queries:
-            self._call('nb_index_rotate_extract_indirect', _ptr(tables), stride, count,
-                       ids.ctypes.data_as(ctypes.c_void_p), sp, sstride, int(bits), columns, _ptr(out_a), _ptr(out_b),
-                       queries)
+            self._call(name, *src, sp, sstride, int(bits), columns, _ptr(out_a), _ptr(out_b), queries)
         return out_a, out_b
 
     # --- oblivious writes (nufhe_b200/index_write.py) ---------------------------------------------
@@ -855,13 +799,8 @@ class Engine:
         res_a, res_b = res
         B = res_b.numel()
         n = res_a.shape[-1]
-        a1 = b1 = a2 = b2 = None
-        if x1 is not None:
-            a1, b1 = self._dense(x1[0], torch.int32), self._dense(x1[1], torch.int32)
-        if x2 is not None:
-            a2, b2 = self._dense(x2[0], torch.int32), self._dense(x2[1], torch.int32)
-        self._call('nb_lwe_affine', _ptr(res_a), _ptr(res_b), _ptr(a1), _ptr(b1), _ptr(a2), _ptr(b2),
-                   int(c), int(s1), int(s2), B, n)
+        parts = self._lwe(x1, x2)
+        self._call('nb_lwe_affine', _ptr(res_a), _ptr(res_b), *map(_ptr, parts), int(c), int(s1), int(s2), B, n)
         return res
 
 
