@@ -4,7 +4,7 @@
  * nb_bootstrap_lut_extract), for compressed cloud keys and ciphertexts, whose uniform masks are regenerated on the
  * device from a seed (nb_seeded_uniform_i32), for public-key encryption (nb_pk_prepare, nb_pk_encrypt), and for
  * packing results into GLWE samples (nb_pack_digits, nb_ntt_mac, nb_pack_finish), and for compact public-key
- * encryption (nb_compact_finish, nb_compact_extract).
+ * encryption (nb_compact_finish, nb_compact_extract), and for re-encryption to another client's key (nb_reencrypt).
  *
  * The reference has no FFI: its boundary is the set of Python call signatures listed in SURVEY.md
  * section 8(b).  Each entry point below replaces the device work behind one of them; the reference
@@ -418,6 +418,23 @@ int nb_index_demux_level(nb_ctx *ctx, const int32_t *in, const uint64_t *sel, si
 int nb_compact_finish(nb_ctx *ctx, const int32_t *c, const int32_t *e1, const int32_t *e2, const int32_t *mus,
                       int mask_size, uint16_t *out, size_t batch);
 int nb_compact_extract(nb_ctx *ctx, const uint16_t *data, int mask_size, int32_t *out_a, int32_t *out_b, size_t rows);
+
+/* Re-encryption (DESIGN.md section 22).  A re-encryption key from the LWE key s_A (n words) to the GLWE key S_B is one
+ * GLWE sample C = (A_C, B_C) under S_B whose slot 2 i + j encrypts s_A[i] g_j, g_0 = 2^24, g_1 = 2^16 (slots from 2 n on
+ * encrypt 0).  The server keeps the mask spectrum (nb_ntt_forward_i32 of A_C, N uint64) and B_C (N int32) per key.
+ * nb_reencrypt: LWE samples a (rows, n), b (rows,) int32 under s_A -> out_a (rows, k N), out_b (rows,) int32 under the
+ *     extracted key of S_B, the layout nb_keyswitch reads: with d_p = d_j(a_i) for p = 2 i + j (the signed 8-bit digits
+ *     of nb_pack_digits) and P = -D . A_C, D(X) = d_0 - sum_{p >= 1} d_p X^(N - p) (an exact negacyclic product),
+ *     out_a[j] = P[0] for j = 0 and -P[N - j] otherwise, out_b = b - sum_p d_p B_C[p], all mod 2^32.  Its phase is
+ *     b - sum_i s_A[i] round_16(a_i) plus the key's noise terms.  Rows are split into segments as for the nb_mk_*
+ *     calls: counts_host[q] consecutive rows use the key whose spectrum is mask_spectra_host[q] and whose body is
+ *     bodies_host[q] (HOST arrays of device pointers; counts may be 0 and must add up to `rows`).  A CTA takes up to 4
+ *     rows of one segment.  NB_EUNSUPPORTED for k != 1 or n t > N (2 n > 1024); NB_EINVAL for a NULL pointer, n = 0,
+ *     counts that do not add up, out_a or a mask spectrum not 16-byte aligned, or a, b, out_b or a body not 4-byte
+ *     aligned.  rows = 0 is a no-op once the arguments are checked. */
+int nb_reencrypt(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t n, int mask_size,
+                 const uint64_t *const *mask_spectra_host, const int32_t *const *bodies_host, const size_t *counts_host,
+                 size_t keys, int32_t *out_a, int32_t *out_b, size_t rows);
 
 #ifdef __cplusplus
 }

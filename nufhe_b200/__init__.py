@@ -64,6 +64,12 @@ from .compact import (
     compact_encrypt,
     expand,
     )
+from .reencrypt import (
+    NuFHEReencryptionKey,
+    make_reencryption_key,
+    reencrypt_variance,
+    MAX_INPUT_VARIANCE,
+    )
 from .tree_lut import (
     NuFHETreeKey,
     TreeLookupTable,

@@ -92,6 +92,7 @@ SIGNATURES = {
     'nb_index_demux_level': [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp, _sz, _sz],
     'nb_compact_finish': [_vp, _vp, _vp, _vp, _vp, _int, _vp, _sz],
     'nb_compact_extract': [_vp, _vp, _int, _vp, _vp, _sz],
+    'nb_reencrypt': [_vp, _vp, _vp, _sz, _int, _vp, _vp, _vp, _sz, _vp, _vp, _sz],
 }
 _RESTYPES = {'nb_bk_row_u64': ctypes.c_size_t, 'nb_ks_prepared_bytes': ctypes.c_size_t, 'nb_bk_multibit_row_u64': ctypes.c_size_t, 'nb_pk_planes_bytes': ctypes.c_size_t,
              'nb_tree_planes_bytes': ctypes.c_size_t, 'nb_ctx_destroy': None, 'nb_last_error': ctypes.c_char_p,

@@ -9,6 +9,7 @@ from .lwe import LweSampleArray, lwe_copy, lwe_add_to
 from .compressed import CompressedLweSampleArray, CompressedCloudKey
 from .public_key import NuFHEPublicKey
 from .compact import NuFHECompactPublicKey, CompactLweSampleArray, expand
+from .reencrypt import NuFHEReencryptionKey, make_reencryption_key, reencrypt
 from .packing import (NuFHEPackingSecretKey, NuFHEPackingKey, PackedLweSampleArray, make_packing_keys, pack,
                       decrypt_packed, decrypt_packed_int)
 from .tree_lut import NuFHETreeKey, TreeLookupTable, lut_tree
@@ -147,6 +148,14 @@ class Context:
         entry.  TypeError for any other key, ValueError for a table or bit count out of range."""
         return encrypt_table(self.thread, self.rng, key, table, out=out, bits=bits)
 
+    def make_reencryption_key(self, secret_key: NuFHESecretKey, compact_public_key: NuFHECompactPublicKey):
+        """The NuFHEReencryptionKey (8 KB; DESIGN.md section 22) with which a server's `VirtualMachine.reencrypt` moves
+        ciphertexts under `secret_key` (the sender's) to the owner of `compact_public_key` (the recipient's), without
+        decrypting them.  Anyone holding both the key and the recipient's secret key recovers the sender's secret key:
+        the server must never give the key to the recipient (reencrypt.make_reencryption_key has the whole trust
+        model).  TypeError for other key types, ValueError for keys of different parameters."""
+        return make_reencryption_key(self.thread, self.rng, secret_key, compact_public_key)
+
     def make_public_key(self, secret_key: NuFHESecretKey):
         """A NuFHEPublicKey: whoever holds it can encrypt (`encrypt`, `encrypt_int`) but not decrypt."""
         return NuFHEPublicKey.from_secret_key(self.thread, self.rng, secret_key)
@@ -229,6 +238,11 @@ class Context:
         if isinstance(file_or_bytestring, bytes):
             return CompactLweSampleArray.loads(file_or_bytestring, self.thread)
         return CompactLweSampleArray.load(file_or_bytestring, self.thread)
+
+    def load_reencryption_key(self, file_or_bytestring):
+        if isinstance(file_or_bytestring, bytes):
+            return NuFHEReencryptionKey.loads(file_or_bytestring, self.thread)
+        return NuFHEReencryptionKey.load(file_or_bytestring, self.thread)
 
     def load_packed_ciphertext(self, file_or_bytestring):
         if isinstance(file_or_bytestring, bytes):
@@ -427,6 +441,14 @@ class VirtualMachine:
         if compact.params != self.params:
             raise ValueError('the compact ciphertexts were made for other parameters than this virtual machine')
         return expand(self.thread, self.params, self.cloud_key.keyswitch_key, compact)
+
+    def reencrypt(self, rekey: NuFHEReencryptionKey, ciphertexts: LweSampleArray, dest: LweSampleArray = None):
+        """The LweSampleArray, of the same shape and under this machine's cloud key, of `ciphertexts` under the sender's
+        key of the NuFHEReencryptionKey `rekey` (made for this machine's owner; nufhe_b200/reencrypt.py).  Its variances
+        are the input's plus reencrypt.reencrypt_variance and the key switch's.  TypeError for other types, ValueError for a
+        key of other parameters, ciphertexts of another LWE dimension, and inputs whose recorded variance is above
+        reencrypt.MAX_INPUT_VARIANCE (bootstrap them first)."""
+        return reencrypt(self.thread, self.params, self.cloud_key.keyswitch_key, rekey, ciphertexts, dest)
 
     def capture(self, circuit, reserve_batch=None):
         """Record `circuit()` -- any sequence of this VM's gates on device-resident ciphertexts -- into a CUDA graph;

@@ -9,6 +9,7 @@
 #include "kernels.cuh"
 #include "index_lookup.cuh"
 #include "compact.cuh"
+#include "reencrypt.cuh"
 #include "tables.h"
 
 using namespace nb;
@@ -249,6 +250,7 @@ int nb_ctx_create(int device, void *stream, nb_ctx **out)
     NB_TRY(check(ctx, cudaFuncSetAttribute(ntt_forward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ntt_smem_bytes(NTT_RAW_U64_BYTES)), "attr"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(ntt_inverse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ntt_smem_bytes(NTT_RAW_U64_BYTES)), "attr"));
     NB_TRY(check(ctx, cudaFuncSetAttribute(ntt_inverse_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ntt_smem_bytes(NTT_RAW_U64_BYTES)), "attr"));
+    NB_TRY(check(ctx, cudaFuncSetAttribute(reencrypt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)reenc_smem_bytes()), "attr"));
     return NB_OK;
 }
 
@@ -1636,6 +1638,38 @@ int nb_mk_ntt_mac(nb_ctx *ctx, const uint64_t *x, const uint64_t *const *key_hos
     ntt_mac_mk_kernel<<<grid, MAC_WARPS * 32, 0, ctx->stream>>>((const u64 *)x, reinterpret_cast<const u64 *const *>(ctx->d_mk),
                                                                (u64 *)out, (u32)rows, (u32)outs);
     return launch_check(ctx, "ntt_mac_mk_kernel");
+}
+
+// ---- re-encryption (reencrypt.cuh, DESIGN.md section 22) ----
+
+int nb_reencrypt(nb_ctx *ctx, const int32_t *a, const int32_t *b, size_t n, int mask_size,
+                 const uint64_t *const *mask_spectra_host, const int32_t *const *bodies_host, const size_t *counts_host,
+                 size_t keys, int32_t *out_a, int32_t *out_b, size_t rows)
+{
+    const char *what = "nb_reencrypt";
+    NB_TRY(mk_preamble(ctx, what, counts_host, keys, rows, a && b && out_a && out_b, "key", mask_spectra_host, bodies_host));
+    if (n == 0) return fail(ctx, NB_EINVAL, std::string(what) + ": n must be at least 1");
+    if (mask_size != 1 || n * REENC_LEVELS > (size_t)PACK_N)
+        return fail(ctx, NB_EUNSUPPORTED, std::string(what) + ": re-encryption is for k = 1 and n t <= 1024 only");
+    bool aligned = !(((uintptr_t)a | (uintptr_t)b | (uintptr_t)out_b) & 3) && !((uintptr_t)out_a & 15);
+    for (size_t q = 0; q < keys; q++)
+        aligned = aligned && !((uintptr_t)mask_spectra_host[q] & 15) && !((uintptr_t)bodies_host[q] & 3);
+    if (!aligned)
+        return fail(ctx, NB_EINVAL, std::string(what) + ": out_a and the mask spectra must be 16-byte aligned, a, b, out_b "
+                                                         "and the bodies 4-byte aligned");
+    if (rows == 0) return NB_OK;
+    const auto *spectra = reinterpret_cast<const u64 *const *>(mask_spectra_host);
+    std::vector<ReencTile> tiles(reenc_tiles(counts_host, keys, spectra, bodies_host, nullptr));
+    reenc_tiles(counts_host, keys, spectra, bodies_host, tiles.data());
+    NB_ON_DEVICE(ctx);
+    NvtxRange nvtx_range("nufhe_b200:reencrypt");
+    NB_TRY(mk_upload(ctx, tiles.data(), tiles.size() * sizeof(ReencTile)));
+    const size_t cap = (size_t)ctx->sm_count * REENC_CTAS;
+    const unsigned grid = (unsigned)(tiles.size() < cap ? tiles.size() : cap);
+    reencrypt_kernel<<<grid, NTT_SWEEP_THREADS, reenc_smem_bytes(), ctx->stream>>>(
+        reinterpret_cast<const ReencTile *>(ctx->d_mk), (u64)tiles.size(), a, b, (u32)n, out_a, out_b, ctx->d_ph_fwd,
+        ctx->d_ph_inv);
+    return launch_check(ctx, "reencrypt_kernel");
 }
 
 // ---- multi-key expansion of compressed cloud keys (DESIGN.md section 19) ----

@@ -13,6 +13,7 @@
 #include "pack_layout.cuh"
 #include "tree_layout.cuh"
 #include "compact_layout.cuh"
+#include "reencrypt_layout.cuh"
 #include "mk_layout.cuh"
 #include "mk_expand_layout.cuh"
 
@@ -640,6 +641,14 @@ void emul_compact_extract(const uint16_t *data, int k, u32 p, i32 *a, i32 *b)
     }
     *b = (i32)pack_unround16(data[k * PACK_N + p]);
 }
+
+// Re-encryption (reencrypt_layout.cuh): the key's slot of (i, j), the coefficient of -D that holds d_p and its sign,
+// the whole polynomial -D (N words) of one mask a (n words), and the output mask (N words) from a product P (N words).
+u32 emul_reenc_slot(u32 i, int j) { return reenc_slot(i, j); }
+u32 emul_reenc_coeff(u32 p) { return reenc_coeff(p); }
+int emul_reenc_negated(u32 p) { return reenc_negated(p) ? 1 : 0; }
+void emul_reenc_digits(const i32 *a, u32 n, i32 *out) { for (u32 c = 0; c < (u32)PACK_N; c++) out[c] = reenc_digit_coeff(a, n, c); }
+void emul_reenc_mask(const u32 *prod, i32 *out) { for (u32 j = 0; j < (u32)PACK_N; j++) out[j] = reenc_mask_word(prod, j); }
 
 // Tree-based programmable bootstrapping (tree_layout.cuh).  emul_tree_keyswitch: nb_tree_prepare, then
 // nb_tree_keyswitch.

@@ -596,6 +596,30 @@ class Engine:
             self._call('nb_compact_extract', _ptr(data), k1 - 1, _ptr(out_a), _ptr(out_b), rows)
         return out_a, out_b
 
+    def reencrypt(self, a, b, spectra, bodies, counts):
+        """LWE samples a (R, n), b (R,) int32 under the keys s_A of re-encryption keys -> out_a (R, k N), out_b (R,) under
+        the extracted key of S_B (nb_reencrypt): spectra[q] (k, N) (the NTT of the key's mask) and bodies[q] (N,) serve
+        counts[q] consecutive rows."""
+        a = self._dense(a, torch.int32)
+        b = self._dense(b, torch.int32).reshape(-1)
+        spectra = [self._dense(s, torch.int64) for s in spectra]
+        bodies = [self._dense(x, torch.int32) for x in bodies]
+        rows, n = a.shape
+        if b.numel() != rows or len(spectra) != len(bodies) or len(counts) != len(spectra):
+            raise ValueError('reencrypt: %d masks, %d bodies, %d keys, %d bodies and %d counts'
+                             % (rows, b.numel(), len(spectra), len(bodies), len(counts)))
+        k = spectra[0].shape[0] if spectra and spectra[0].dim() == 2 else 1
+        for s, x in zip(spectra, bodies):
+            if tuple(s.shape) != (k, N) or tuple(x.shape) != (N,):
+                raise ValueError('reencrypt: key spectra %s and bodies %s are not (k, N) and (N,)'
+                                 % (tuple(s.shape), tuple(x.shape)))
+        out_a, out_b = self.empty((rows, k * N), torch.int32), self.empty((rows,), torch.int32)
+        self._call('nb_reencrypt', _ptr(a), _ptr(b), n, k, self._host_array(ctypes.c_void_p, [s.data_ptr() for s in spectra]),
+                   self._host_array(ctypes.c_void_p, [x.data_ptr() for x in bodies]),
+                   self._host_array(ctypes.c_size_t, [int(c) for c in counts]), len(spectra), _ptr(out_a), _ptr(out_b),
+                   rows)
+        return out_a, out_b
+
     def tree_prepare(self, masks, body):
         """The tree key's masks (n, t, k, N) and bodies (n, t, N) int32 laid into the 4 byte planes that tree_keyswitch
         reads (nb_tree_prepare): a uint8 tensor of nb_tree_planes_bytes(n, k) bytes."""

@@ -30,7 +30,7 @@ from .packing import NuFHEPackingKey, PackedLweSampleArray
 from .compact import CompactLweSampleArray
 from .index_lookup import EncryptedIndexArray, EncryptedIndexTable, IndexTable
 from .batch_keys import TenantKeys
-from . import compact, gates, index_lookup, index_write, packing, tree_lut
+from . import compact, gates, index_lookup, index_write, packing, reencrypt, tree_lut
 
 # gates that need no key: run per tenant
 _KEYLESS = {'not': 1, 'copy': 1, 'constant': 1}
@@ -559,6 +559,30 @@ class MultiKeyVirtualMachine:
         keys = TenantKeys(thr, [counts[t] for t in active], kss=[self._ks[t] for t in active])
         compact.expand_groups(thr, self.params, keys, [compacts[t] for t in active], res)
         return self._results(res, active, shapes, counts, None)
+
+    @_in_rounds(('ciphertexts',), ('rekeys', 'dest'))
+    def reencrypt(self, rekeys, ciphertexts, dest=None):
+        """Every tenant's ciphertexts re-encrypted to it (VirtualMachine.reencrypt): rekeys[t] is the
+        NuFHEReencryptionKey from the sender of ciphertexts[t] to tenant t, the recipient (None for idle tenants).  One
+        nb_reencrypt launch with one segment per active tenant, then one multi-key key switch, a few rows per pass; each
+        tenant's rows are bit-identical to its own vm.reencrypt.  A list aligned with the tenants."""
+        active, shapes = self._active((ciphertexts,), dest)
+        if not isinstance(rekeys, (list, tuple)) or len(rekeys) != self.tenants:
+            raise ValueError('rekeys must be a list of %d entries, one per tenant' % self.tenants)
+        for t in active:
+            reencrypt.check_inputs(self.params, rekeys[t], ciphertexts[t], tenant=t)
+        out = [None] * self.tenants
+        if not active:
+            return out
+        thr = self.thread
+        counts = self._counts(active, shapes)
+        B = sum(counts)
+        res = (thr.empty((B, self.params.in_out_params.size), torch.int32), thr.empty((B,), torch.int32),
+               thr.empty((B,), torch.float32))
+        keys = TenantKeys(thr, [counts[t] for t in active], kss=[self._ks[t] for t in active])
+        parts = [(ciphertexts[t].a, ciphertexts[t].b, ciphertexts[t].current_variances) for t in active]
+        reencrypt.reencrypt_rows(thr, self.params, keys, [rekeys[t] for t in active], parts, res)
+        return self._results(res, active, shapes, counts, dest)
 
     @_in_rounds(('indexes',), ('table', 'dest'))
     def lookup(self, indexes, table, dest=None):
